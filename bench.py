@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — create_proof-schedule benchmark for the B200 back end (BASELINE.json metric:
+"""bench.py — create_proof-schedule benchmark for the H100 back end (BASELINE.json metric:
 "create_proof ms + MSM G1-pairs/s at k=19 ECDSA").
 
 One "step" = one pass of the prover hot path for ONE proof of a halo2-lib benchmark circuit: the witness-column
@@ -17,6 +17,10 @@ one polynomial is taken through lagrange_to_coeff -> coeff_to_extended -> extend
 Horner evaluations at domain points.  A mismatch exits with status 3 and prints no JSON line.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 1..5] [--sweep 1,2,4,5|none]
+                    [--dump-outputs DIR]
+
+--steps K sets the number of timed steps of every timed loop (headline, placements, end-to-end paths, sweep configs).
+--dump-outputs DIR writes what the last timed resident step of the headline config computed (see Workload.dump_outputs).
 """
 from __future__ import annotations
 import argparse
@@ -114,7 +118,7 @@ class Schedule:
                            if (self.n // max(gpus, 1)) >= (1 << 18) else
                            "MSM shards below 2^18 points are latency-bound chains, so the transforms run in one block before extended_to_coeff / the h(X) commitments instead of beside the phases")),
             "parallelism": (f"msm point-range sharded x{gpus} + fused NVLink peer all-reduce of the partial sums (one kernel per phase); NTT one polynomial per device" if gpus > 1 else "single GPU"),
-            "l2_policy": "inputs larger than L2: distinct scalar columns + two multi-level base tables + NTT buffers per step exceed the 126 MB L2 (k >= 16); smaller configs are sweep extras, not the headline",
+            "l2_policy": "inputs larger than L2: distinct scalar columns + two multi-level base tables + NTT buffers per step exceed the 50 MB L2 (k >= 16); smaller configs are sweep extras, not the headline",
         }
 
 
@@ -207,6 +211,16 @@ def point_matches(xyz_limbs, expect) -> bool:
     return X == expect[0] * z2 % P_MOD and Y == expect[1] * z2 * Z % P_MOD
 
 
+def jacobian_to_affine(xyz_limbs):
+    """12 u64 (Jacobian, Montgomery) as the library returns them -> canonical affine (x, y) ints, None for the identity"""
+    v = np.asarray(xyz_limbs, dtype=np.uint64).reshape(3, 4)
+    X, Y, Z = (limbs_to_int(v[i]) * MONT_RINV_P % P_MOD for i in range(3))
+    if Z == 0:
+        return None
+    zi = pow(Z, -1, P_MOD)
+    return X * zi * zi % P_MOD, Y * zi * zi * zi % P_MOD
+
+
 def horner_mont(coeff_limbs: np.ndarray, x: int) -> int:
     """sum_j c_j x^j mod r for Montgomery-limb coefficients; returns the canonical value"""
     acc = 0
@@ -216,7 +230,7 @@ def horner_mont(coeff_limbs: np.ndarray, x: int) -> int:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -261,14 +275,8 @@ class ClockSampler:
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": smax, "samples": len(sm), "reasons": sorted(reasons)}
 
 
-def measured_hbm_peak():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        try:
-            return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+def hbm_peak():
+    return 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s; not a measured peak)"
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
@@ -299,8 +307,13 @@ def cpu_sample(sched: Schedule, threads: int | None = None, reps: int = 3):
     composes the step time: sum(count_i * t_i).  Every op is repeated `reps` times per thread count; the minimum is
     used, min / median are reported.  ~10-30 s of CPU work on a typical host at k=19."""
     from oracle import oracle as orc
-    try:  # a -march=native build for the host it runs on (the shipped .so is x86-64-v3)
-        so = os.path.join(ROOT, "oracle", "_build", "liboracle_native.so")
+    try:  # a -march=native build for the host it runs on (the shipped .so is x86-64-v3), built outside the tree
+        import atexit
+        import shutil
+        import tempfile
+        tmp = tempfile.mkdtemp(prefix="h2b_oracle_")
+        atexit.register(shutil.rmtree, tmp, True)
+        so = os.path.join(tmp, "liboracle_native.so")
         subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle"), "-s", "MARCH=native", f"OUT={so}"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
         orc._lib = None
         orc._SO = so
@@ -854,6 +867,41 @@ class Workload:
         return {"lagrange_to_coeff": ok_intt, "coeff_to_extended": ok_coset, "extended_to_coeff_roundtrip": ok_back,
                 "points_checked": len(pts) + 1}
 
+    def dump_outputs(self, out_dir, rows=1 << 12):
+        """writes what the last resident step computed as float64 .npy files of little-endian 32-bit limbs (exact):
+        commitments.npy holds the commitments in canonical affine coordinates (x limbs, then y limbs; zeros for the
+        identity); the assigned columns and the transformed polynomials (Montgomery form, as the library leaves them on
+        the device) are sampled at `rows` fixed seeded row indices, stored in sample_rows*.npy"""
+        torch, s, dev = self.rig.torch, self.s, self.rig.dev
+        torch.cuda.synchronize()
+        os.makedirs(out_dir, exist_ok=True)
+        save = lambda name, a: np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
+        to_limbs32 = lambda v: [(v >> (32 * i)) & 0xFFFFFFFF for i in range(8)]
+        cms = []
+        for p in self.outs_dev.cpu().numpy().view(np.uint64):
+            xy = jacobian_to_affine(p)
+            cms.append([0] * 16 if xy is None else to_limbs32(xy[0]) + to_limbs32(xy[1]))
+        save("commitments", cms)
+        rng = np.random.default_rng(0x5EED)
+        idx = np.sort(rng.choice(s.n, min(s.n, rows), replace=False))
+        idx_ext = np.sort(rng.choice(1 << s.ext_k, min(1 << s.ext_k, rows), replace=False))
+        save("sample_rows", idx)
+        save("sample_rows_extended", idx_ext)
+        d_idx, d_idx_ext = torch.from_numpy(idx).to(dev), torch.from_numpy(idx_ext).to(dev)
+        rows_of = lambda t, i: t.index_select(0, i).cpu().numpy().view(np.uint32).astype(np.float64)
+        for c in range(s.A):
+            save(f"advice_column_{c}", rows_of(self.acols_dev[c], d_idx))
+        for c in range(s.L):
+            save(f"lookup_column_{c}", rows_of(self.lcols_dev[c], d_idx))
+        for i, p in self.polys_dev.items():
+            if self.my_ntt(i):
+                save(f"lagrange_to_coeff_{i}", rows_of(p, d_idx))
+        for i, e in self.ext_dev.items():
+            if i != 0 and self.my_ntt(s.n_poly + i):
+                save(f"coeff_to_extended_{i}", rows_of(e, d_idx_ext))
+        if self.my_ntt(2 * s.n_poly):  # ext_dev[0] ends the step as the extended_to_coeff result (n coefficients)
+            save("extended_to_coeff", rows_of(self.ext_dev[0], d_idx))
+
     def close(self):
         if self.side_pool:
             self.side_pool.shutdown()
@@ -871,6 +919,8 @@ def run_config(rig: Rig, sched: Schedule, steps: int, warmup: int, headline: boo
     prof = "k_accumulate" if headline else None
     ms_step, launches = rig.timed(wl.step_resident, steps, warmup, prof=prof)
     res["ms_per_step"], res["gpu_launches"] = ms_step, launches
+    if headline and getattr(args, "dump_outputs", None) and rig.rank == 0:
+        wl.dump_outputs(args.dump_outputs)
     if headline:
         res["acc"] = rig.ctx.profile_read("k_accumulate")
         res["bred"] = rig.ctx.profile_read("k_batch_affine")
@@ -879,7 +929,7 @@ def run_config(rig: Rig, sched: Schedule, steps: int, warmup: int, headline: boo
     if headline:
         # the other placement of the transforms, for the record (the rule in step_resident picks by shard size)
         dflt_overlap = wl.n_loc >= (1 << 18) or BENCH_BG_NTT > 0
-        ms_alt, _ = rig.timed(lambda: wl.step_resident(not dflt_overlap), max(1, min(steps, 5)), 1)
+        ms_alt, _ = rig.timed(lambda: wl.step_resident(not dflt_overlap), steps, 1)
         res["ms_per_step_seq"] = ms_alt if dflt_overlap else ms_step
         res["ms_per_step_ovl"] = ms_step if dflt_overlap else ms_alt
         res["transform_placement"] = "beside the commitment phases (side stream)" if dflt_overlap else "one block before the h(X) phase"
@@ -906,14 +956,14 @@ def run_b200(args):
     # host memory, commitments and evaluations come down, every column stays in HBM behind h2b_poly handles in between,
     # and the step contains the quotient / product-column / opening work create_proof does between the commitments
     wl.setup_prover()
-    ms_e2e, e2e_launches = rig.timed(wl.step_e2e_prover, max(1, min(args.steps, 10)), 2)
+    ms_e2e, e2e_launches = rig.timed(wl.step_e2e_prover, args.steps, 2)
     torch.cuda.synchronize()
     prover_check = wl.verify_prover()
     # ---- the round-1 end-to-end path for continuity: every call takes and returns HOST buffers (h2b_* without _dev)
     if os.environ.get("H2B_E2E_TRACE"):
         wl.trace = []
-    ms_e2e_ovl, _ = rig.timed(wl.step_e2e, max(1, min(args.steps, 5)), 1)
-    ms_e2e_seq, _ = rig.timed(lambda: wl.step_e2e(False), max(1, min(args.steps, 3)), 1)
+    ms_e2e_ovl, _ = rig.timed(wl.step_e2e, args.steps, 1)
+    ms_e2e_seq, _ = rig.timed(lambda: wl.step_e2e(False), args.steps, 1)
     torch.cuda.synchronize()
     verified_e2e = wl.verify_commitments(wl.outs_host)
     if wl.trace is not None and rank == 0:
@@ -960,7 +1010,7 @@ def run_b200(args):
         if cid == args.config:
             continue
         s2 = Schedule(cid)
-        st = 2 if s2.k >= 22 else 3
+        st = args.steps
         try:
             r2, w2 = run_config(rig, s2, st, 2, False, args)
             ntt2 = w2.verify_ntt()
@@ -987,9 +1037,9 @@ def run_b200(args):
                 "msm_only_ms": t_msm, "msm_only_pairs_per_s": s2.n / (t_msm / 1e3) * world,
                 "coset_ntt_ms": t_ntt, "ntt_elements_per_s": (1 << s2.ext_k) / (t_ntt / 1e3),
                 "assign_ms": t_asg, "assign_cells_per_s": (w2.n_cells + w2.n_lookup) / (t_asg / 1e3),
-                "roofline": {"msm_hbm_frac": 96.0 * w2.n_loc / (t_msm / 1e3) / 1e9 / measured_hbm_peak()[0],
-                             "ntt_hbm_frac": 64.0 * (1 << s2.ext_k) / (t_ntt / 1e3) / 1e9 / measured_hbm_peak()[0],
-                             "assign_hbm_frac": 64.0 * (w2.n_cells + w2.n_lookup) / (t_asg / 1e3) / 1e9 / measured_hbm_peak()[0]},
+                "roofline": {"msm_hbm_frac": 96.0 * w2.n_loc / (t_msm / 1e3) / 1e9 / hbm_peak()[0],
+                             "ntt_hbm_frac": 64.0 * (1 << s2.ext_k) / (t_ntt / 1e3) / 1e9 / hbm_peak()[0],
+                             "assign_hbm_frac": 64.0 * (w2.n_cells + w2.n_lookup) / (t_asg / 1e3) / 1e9 / hbm_peak()[0]},
                 "steps": st, "gpu_launches": r2["gpu_launches"], "e2e_resident_proof": e2e2,
                 "verified": {"msm": r2["verified_resident"], "of": len(s2.msm), "ntt": ntt2, "ok": rig.all_true(ok)},
             }
@@ -1020,7 +1070,7 @@ def run_b200(args):
 
     n_loc = n // world
     value = sched.pairs / (ms_step / 1e3)
-    peak, peak_src = measured_hbm_peak()
+    peak, peak_src = hbm_peak()
     # the dominant kernel: bucket accumulation = the batch-affine reduction passes + the XYZZ accumulation of what is left
     # a launch of the grouped pipeline accumulates the columns of a whole group (1-2 at k = 19): per launch the
     # algorithmic bytes are 96 B x pairs of ALL its columns, so the average is formed over the step's totals
@@ -1029,22 +1079,14 @@ def run_b200(args):
     iso_avg_ms = (iso_ms + iso_aff_ms) / max(iso_cnt, 1)
     achieved = 96.0 * n_loc * msm_per_launch / (acc_avg_ms / 1e3) / 1e9  # algorithmic 96 B per pair (32 B scalar + 64 B base), SURVEY.md §8d
     achieved_iso = 96.0 * n_loc / (iso_avg_ms / 1e3) / 1e9
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")  # dram bytes per launch from the committed ncu --set full capture
-    if os.path.exists(tpath):
-        try:
-            traffic = json.load(open(tpath)).get(f"k{k}_n{world}")  # per MSM column
-            traffic = traffic * msm_per_launch if traffic else None
-        except Exception:
-            traffic = None
     roofline = {"bound": "hbm", "kernel": "bucket accumulation (k_batch_affine passes + k_accumulate)", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "avg_launch_ms": acc_avg_ms, "launches_timed": acc_cnt, "msm_columns_per_launch": msm_per_launch,
                 "algorithmic_bytes_per_launch": 96 * n_loc * msm_per_launch,
                 "timed_region_note": "launches of the timed region overlap with the kernels of the other two MSM lanes, which stretches each launch",
                 "isolated": {"avg_launch_ms": iso_avg_ms, "launches": iso_cnt, "achieved": achieved_iso, "frac": achieved_iso / peak,
                              "k_accumulate_ms": iso_ms / max(iso_cnt, 1), "k_batch_affine_ms": iso_aff_ms / max(iso_cnt, 1)},
-                "note": "bucket accumulation is bound by the integer multiplier (IMAD.WIDE), not by HBM; see DESIGN.md 4.1/4.2 and profiles/"}
+                "note": "bucket accumulation is bound by the integer multiplier (IMAD.WIDE), not by HBM; see DESIGN.md 4.1/4.2"}
     npoly = sched.n_poly
     adv_bytes = (sched.A + sched.L) * n * 32
     # per step and rank 0: virtual column + looked-up cells, every MSM's scalar shard, the polynomials of the transforms
@@ -1195,7 +1237,7 @@ def run_single_process(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps of every timed loop (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", type=int, default=3, choices=[1, 2, 3, 4, 5], help="BASELINE.json config (1-based); 3 = ECDSA k=19 is the headline")
@@ -1204,7 +1246,11 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (profiling runs)")
     ap.add_argument("--inject-fault", default=None, choices=["skip_allreduce"], help="testing: break the multi-GPU exchange; the run must exit 3")
     ap.add_argument("--single-process", action="store_true", help="one process drives --gpus N devices through a device-group context (no torchrun)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step of the headline config computed to DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     args.sweep_ids = [] if args.sweep in ("none", "") else [int(x) for x in args.sweep.split(",")]
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-// assign.cu — column-wise witness assignment for sm_100a.
+// assign.cu — column-wise witness assignment for sm_90a.
 //
 // Replaces the per-cell loop of `assign_witnesses`
 // (halo2-base/src/gates/flex_gate/threads/single_phase.rs:273-312; each cell goes through

@@ -96,7 +96,7 @@ static std::vector<T> every_gth(T const* v, size_t m, size_t g, size_t G) {
 
 extern "C" {
 
-const char* h2b_version(void) { return "h2b200 0.1.0 (sm_100a)"; }
+const char* h2b_version(void) { return "h2b200 0.1.0 (sm_90a)"; }
 
 int h2b_ctx_create(int device, h2b_ctx** out) {
     if (!out) return H2B_ERR_ARG;
@@ -117,7 +117,7 @@ int h2b_ctx_create(int device, h2b_ctx** out) {
             // experiment knob: the MSM gathers 64-byte table points at random; H2B_L2_FETCH=32|64|128 sets the L2 fetch
             // granularity hint (cudaLimitMaxL2FetchGranularity)
             const char* e = getenv("H2B_L2_FETCH");
-            const int g = e ? atoi(e) : 0;  // measured: no effect on the MSM at k = 19 (profiles/), so the driver default stays
+            const int g = e ? atoi(e) : 0;  // unset: the driver default
             if (g == 32 || g == 64 || g == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g);
         }
         {   // the context's own stream sits at the lanes' priority: above the side queue (see the lane streams below)

@@ -1,10 +1,10 @@
-// field.cuh — BN254 Fq / Fr arithmetic for sm_100a: 254-bit Montgomery (R = 2^256), 8 x 32-bit limbs in registers.
+// field.cuh — BN254 Fq / Fr arithmetic for sm_90a: 254-bit Montgomery (R = 2^256), 8 x 32-bit limbs in registers.
 //
 // Memory layout is the `[u64;4]` little-endian Montgomery contract halo2-lib exposes
 // (halo2-base/src/utils/mod.rs:332-377; halo2curves-axiom 0.7.3 bn256::{Fq,Fr}): on a little-endian
 // machine 4 x u64 == 8 x u32, so host arrays are consumed as two 128-bit loads per element.
 //
-// The multiplier is written for the Blackwell integer pipe: every (mad.lo.cc, madc.hi.cc) pair on the same
+// The multiplier is written for the integer pipe: every (mad.lo.cc, madc.hi.cc) pair on the same
 // multiplicands is fused by ptxas into ONE `IMAD.WIDE.U32[.X]` with predicate carry, so a product row is
 // 4 wide-MADs for the even limbs of `a` + 4 for the odd limbs.  Even-limb and odd-limb partial products are
 // kept in two accumulators whose 64-bit register pairs never move; the Montgomery shift by one limb per
@@ -176,7 +176,7 @@ struct __align__(16) Fp {
     // Bounds: running total < 2p before a row and < 2^288 * 2^(32 i) after the products, so the chains
     // that would carry into position i+9 cannot, and the final sum is < 2p.
     __device__ __forceinline__ friend Fp operator*(const Fp& a, const Fp& b) {
-#ifdef H2B_MUL_KARATSUBA  // measured slower on B200 (see the note at mul_karatsuba): kept for reference only
+#ifdef H2B_MUL_KARATSUBA  // not the default (see the note at mul_karatsuba): kept for reference only
         return mul_karatsuba(a, b);
 #else
         return mul_cios(a, b);
@@ -306,11 +306,10 @@ struct __align__(16) Fp {
     }
 
     // ---- Karatsuba variant: 48 + 64 = 112 wide multiplies instead of 128 (NOT the default) ------------------------
-    // Measured on B200 (tools/latbench.cu, 8 warps per sub-partition): 599 cycles per warp-product against 556 for
-    // the CIOS form above, and k_accumulate 1.86 ms against 1.31 ms: ptxas needs 303 instructions (incl. IMAD.MOV /
-    // IMAD.X on the multiplier pipe) instead of 185 and the kernel becomes issue- and register-bound.
-    // The integer multiplier is the scarce resource on this part (IMAD.WIDE / IMAD.HI issue every ~4.2 cycles per
-    // sub-partition, plain adds run on the otherwise idle ALU pipe), so one Karatsuba level on the 8x8-limb product
+    // ptxas needs far more instructions for it than for the CIOS form above (incl. IMAD.MOV / IMAD.X on the multiplier
+    // pipe), which makes k_accumulate issue- and register-bound; tools/latbench.cu compares the two forms.
+    // The idea: the integer multiplier is the scarce resource (plain adds run on the otherwise idle ALU pipe), so one
+    // Karatsuba level on the 8x8-limb product
     // trades 16 wide multiplies for ~100 additions:  a = a0 + a1 X, b = b0 + b1 X, X = 2^128,
     //     a*b = z0 + (z0 + z2 - (a0 - a1)(b0 - b1)) X + z2 X^2,   z0 = a0 b0, z2 = a1 b1.
     // 4x4-limb product r[0..8) = x * y.  E / O are position-indexed accumulators for products that start at even /

@@ -83,7 +83,7 @@ struct h2b_ctx {
     cudaEvent_t side_ev[2] = {nullptr, nullptr};
     cudaEvent_t pipe_ev[3][3] = {};       // [buffer][uploaded, computed, downloaded]
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    int sm_count = 148;
+    int sm_count = 132;
     mutable std::mutex mu;
     std::string err;
     uint64_t launches = 0;

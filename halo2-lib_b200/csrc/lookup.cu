@@ -1,4 +1,4 @@
-// lookup.cu — the lookup argument's permuted columns for sm_100a (SURVEY.md §8(f) rank 2):
+// lookup.cu — the lookup argument's permuted columns for sm_90a (SURVEY.md §8(f) rank 2):
 // halo2-axiom 0.5.3 `plonk/lookup/prover.rs::permute_expression_pair` (not vendored; restated from the upstream
 // algorithm).  Given the compressed input column A and table column S over the usable rows u = n - (blinding + 1):
 //     A' = A sorted by Fr's `Ord` (integer order of the canonical value);

@@ -1,4 +1,4 @@
-// msm.cu — multi-scalar multiplication over BN254 G1 for sm_100a.
+// msm.cu — multi-scalar multiplication over BN254 G1 for sm_90a.
 //
 // Replaces halo2curves-axiom 0.7.3 `msm::best_multiexp(coeffs, bases)` as reached from
 // ParamsKZG::commit / commit_lagrange inside create_proof (sole halo2-lib call site of create_proof:
@@ -569,14 +569,15 @@ int msm_choose_c_fixed(size_t n) {
         int v = atoi(e);
         if (v >= 4 && v <= 24) return v;
     }
-    // W = ceil(255 / c) only drops at c = 13, 14, 15, 16, 17, 19, 20, 22; measured on B200 (tools/prof_ops.py,
-    // profiles/r02_window_sweep.txt): 2^19: c = 17 (W = 15) beats 16 / 19 / 20; 2^21 and 2^23: c = 20 (W = 13) beats
-    // 17 / 19 / 21 / 22 (the bucket-side work grows 2^c while the additions only shrink with W).  Small domains — the
-    // shards of a multi-GPU run and the k <= 16 configs — want c close to log2(n): the fixed tail is latency-bound and
-    // hardly grows with the bucket count, while fewer table levels shorten everything else (2^15: c = 15 runs in 402 us,
-    // the former c = 13 in 689 us; 2^16: 523 vs 646 us).
+    // W = ceil(255 / c) only drops at c = 13, 14, 15, 16, 17, 19, 20, 22, so only those are candidates (H2B_MSM_C and
+    // tools/prof_ops.py compare them): the bucket-side work grows 2^c while the additions only shrink with W.  Small
+    // domains — the shards of a multi-GPU run and the k <= 16 configs — want c close to log2(n): the fixed tail is
+    // latency-bound and hardly grows with the bucket count, while fewer table levels shorten everything else.
+    // Measured on an H100 80GB HBM3 at a 400 W power limit (one MSM, uniform / witness-like scalars): 2^19: c = 17
+    // 23.6 ms per k = 19 bench step against 24.0 (16), 27.4 (19), 27.8 (20); 2^21: c = 17 7.16 / 2.61 ms against
+    // 7.35 / 3.19 ms at c = 20; 2^23: c = 20 27.1 / 9.0 ms against 30.6 / 9.1 at c = 17.  2^22 is not measured.
     const int lg = ceil_log2(n ? n : 1);
-    if (lg >= 21) return 20;
+    if (lg >= 22) return 20;
     if (lg >= 17) return 17;
     if (lg == 16) return 16;
     if (lg >= 13) return 15;
@@ -599,10 +600,9 @@ void msm_build_table(h2b_ctx* ctx, const void* d_bases, size_t count, int c, int
                    t + (size_t)w * count, (u32)count, c);
 }
 
-// Number of batch-affine halving levels (batch_affine.cuh) in front of k_accumulate.  Measured on B200 (profiles/
-// r02_batch_affine.md): bit-exact, but NOT faster than the plain XYZZ accumulation at any size tried (k = 19 / 21 / 23) —
-// the warps of a CTA wait at the barrier around the single-lane inversion (ncu: barrier is the top stall, SM throughput
-// 43 % against 82 %), and the table points are gathered twice.  It therefore stays an opt-in path:
+// Number of batch-affine halving levels (batch_affine.cuh) in front of k_accumulate.  Bit-exact, but the warps of a CTA
+// wait at the barrier around the single-lane inversion and the table points are gathered twice, so it is not expected
+// to beat the plain XYZZ accumulation.  It therefore stays an opt-in path:
 // h2b_ctx_set_option("msm.affine_levels", 1..3) or H2B_AFF_LEVELS; default 0.
 static int msm_choose_levels(const h2b_ctx* ctx, int q_is_table) {
     static const int forced = [] {

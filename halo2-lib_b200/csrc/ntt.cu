@@ -1,4 +1,4 @@
-// ntt.cu — number-theoretic transform over BN254 Fr for sm_100a.
+// ntt.cu — number-theoretic transform over BN254 Fr for sm_90a.
 //
 // Replaces halo2-axiom 0.5.3 `arithmetic::best_fft(a, omega, log_n)` and the EvaluationDomain wrappers
 // lagrange_to_coeff / coeff_to_lagrange / coeff_to_extended / extended_to_coeff that create_proof calls per
@@ -21,7 +21,7 @@ namespace h2b {
 
 static constexpr int NTT_THREADS = 256;   // upper bound; small tiles run with TILE / 4 threads (one radix-4 group each)
 static constexpr int NTT_TILE_LOG = 11;  // largest tile: 2^11 elements * 32 B = 64 KB of shared memory
-static constexpr int NTT_SMEM_MAX = 227 * 1024;  // opt-in limit of dynamic shared memory per CTA on sm_100
+static constexpr int NTT_SMEM_MAX = 227 * 1024;  // opt-in limit of dynamic shared memory per CTA on sm_90
 static constexpr int NTT_MAX_R = 11;  // one column of the largest digit = 2^11 * 32 B = the whole 64 KB tile
 
 // Fr::ZETA and ZETA^2 in Montgomery form (halo2curves bn256::Fr::ZETA; SURVEY.md §8c); the same values are

@@ -1,4 +1,4 @@
-// poly.cu — opening arithmetic of the SHPLONK prover for sm_100a (SURVEY.md §8(f) rank 4):
+// poly.cu — opening arithmetic of the SHPLONK prover for sm_90a (SURVEY.md §8(f) rank 4):
 //     eval_polynomial(poly, x)   = sum_i a_i x^i                      (halo2-axiom 0.5.3 arithmetic.rs)
 //     kate_division(a, z)        = quotient of a(X) by (X - z)          (same file; the remainder a(z) is dropped)
 //     linear combinations of polynomials                                (poly/kzg/multiopen/shplonk/prover.rs)

@@ -1,4 +1,4 @@
-// scan.cu — Fr batch inversion and grand-product (prefix product) columns for sm_100a.
+// scan.cu — Fr batch inversion and grand-product (prefix product) columns for sm_90a.
 //
 // These are the primitives behind the permutation / lookup grand products of create_proof (SURVEY.md §3.3 step 4,
 // §8(f) rank 2; halo2-axiom 0.5.3 `plonk/permutation/prover.rs`, `plonk/lookup/prover.rs`, ff 0.13 `BatchInvert`):

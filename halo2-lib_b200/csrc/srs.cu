@@ -1,4 +1,4 @@
-// srs.cu — keygen-side SRS utilities for sm_100a (SURVEY.md §8(f) rank 3):
+// srs.cu — keygen-side SRS utilities for sm_90a (SURVEY.md §8(f) rank 3):
 //   g_to_lagrange   halo2-axiom 0.5.3 `poly/kzg/commitment.rs::g_to_lagrange` = best_fft over G1 with omega^-1, every
 //                   point scaled by 2^-k, batch-normalised:  g_lagrange[i] = (1/n) sum_j omega^(-i j) g[j]
 //   srs_setup       `ParamsKZG::setup` for a caller-supplied tau: g[i] = tau^i G, g_lagrange[i] = L_i(tau) G with

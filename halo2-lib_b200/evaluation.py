@@ -7,7 +7,7 @@ and of `arithmetic::{eval_polynomial, kate_division}` (rank 4), on top of the C 
     lookup_fold           one lookup argument's five terms
     eval_polynomial, kate_division, poly_lincomb
 
-The upstream file is not vendored under /root/reference; the program encoding is this library's own (see the header).
+The upstream file is not vendored under the reference tree; the program encoding is this library's own (see the header).
 Expressions are nested tuples:  ("constant", fr) ("fixed", col, rot) ("advice", col, rot) ("instance", col, rot)
 ("challenge", i) ("negated", e) ("sum", a, b) ("product", a, b) ("scaled", e, fr),  fr = Montgomery [u64;4] limbs.
 No field arithmetic happens here: constants are carried as limbs and everything is computed by the kernels."""

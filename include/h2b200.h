@@ -1,4 +1,4 @@
-/* h2b200.h — C ABI of libh2b200: the sm_100a back end for the create_proof hot path of halo2-lib
+/* h2b200.h — C ABI of libh2b200: the sm_90a back end for the create_proof hot path of halo2-lib
  * (multi-scalar multiplication over BN254 G1, NTT over BN254 Fr, column-wise witness assignment).
  *
  * This is the surface a `halo2_proofs`-compatible Rust crate binds with `extern "C"` in place of the rayon

@@ -5,7 +5,7 @@
  * never links, loads or calls it, and has no CPU fallback.
  *
  * PARITY STATUS: **unpinned by reference goldens** — the arithmetic lives in crates that are not
- * vendored under /root/reference and cannot be built here (no Rust toolchain):
+ * vendored under the reference tree and cannot be built here (no Rust toolchain):
  *   halo2curves-axiom 0.7.3 (Cargo.lock:1185-1188)  bn256::{Fq,Fr,G1,G1Affine}, msm::best_multiexp
  *   halo2-axiom 0.5.3 @5e4f0e5 (Cargo.lock:1063-1065) arithmetic::best_fft, poly::EvaluationDomain,
  *                                                      poly::kzg::commitment::ParamsKZG::commit{,_lagrange}

@@ -5,7 +5,7 @@ TEST INFRASTRUCTURE ONLY.  Nothing outside `tests/`, `__graft_entry__.smoke()` a
 path (halo2-lib_b200/) never routes through it.
 
 PARITY STATUS: **unpinned by reference goldens.**  The arithmetic restated here lives in
-third-party crates that are NOT vendored in /root/reference:
+third-party crates that are NOT vendored in the reference tree:
   * halo2curves-axiom 0.7.3 (Cargo.lock:1185-1188): bn256::{Fr,Fq,G1,G1Affine}, msm::best_multiexp
   * halo2-axiom 0.5.3 @5e4f0e5 (Cargo.lock:1063-1065): arithmetic::best_fft,
     poly::EvaluationDomain::{lagrange_to_coeff, coeff_to_extended, extended_to_coeff},

@@ -1,7 +1,7 @@
 //! Safe wrappers over `ffi` with the argument meaning of the halo2-axiom functions they replace.
 //! halo2curves `Fr` / `Fq` are `#[repr(transparent)] struct([u64; 4])` in Montgomery form and `G1Affine {x, y}`,
 //! `G1 {x, y, z}` are plain structs of those, so slices are passed as `*const u64` without copying — the `[u64; 4]`
-//! little-endian limb contract halo2-base itself relies on (/root/reference/halo2-base/src/utils/mod.rs:332-377).
+//! little-endian limb contract halo2-base itself relies on (halo2-base/src/utils/mod.rs:332-377).
 use crate::ffi::*;
 use halo2curves::bn256::{Fr, G1Affine, G1};
 use once_cell::sync::OnceCell;
@@ -99,7 +99,7 @@ impl Backend {
     }
 
     /// The prover branch of `SinglePhaseCoreManager::assign_raw`
-    /// (/root/reference/halo2-base/src/gates/flex_gate/threads/single_phase.rs:152-156 -> :273-312): `vcol` is the
+    /// (halo2-base/src/gates/flex_gate/threads/single_phase.rs:152-156 -> :273-312): `vcol` is the
     /// concatenation of `ctx.advice` over `self.threads` in order (parallelize.rs:8-29 fixes that order), as
     /// [`AssignedCell`] records straight from `Vec<Assigned<Fr>>`; `break_points` is the pinned `ThreadBreakPoints`
     /// of the phase (builder.rs:181-204).  Returns `ncols` columns of 2^k rows.

@@ -1,5 +1,5 @@
 //! `halo2_proofs_axiom_gpu`: what halo2-lib sees as `halo2_proofs` under its `cuda` feature
-//! (/root/reference/halo2-base/src/lib.rs:25-28).  The fork of halo2-axiom 0.5.3 keeps every public path halo2-lib
+//! (halo2-base/src/lib.rs:25-28).  The fork of halo2-axiom 0.5.3 keeps every public path halo2-lib
 //! imports (SURVEY.md §8(b) lists them) and replaces four bodies with calls into [`backend`]:
 //!
 //! | halo2-axiom function                                   | becomes                                   |
@@ -11,6 +11,6 @@
 //!
 //! No exception or abort crosses the boundary: every C entry point returns a status; [`backend::check`] turns a
 //! non-zero status into the panic the CPU path raises (`.expect("prover should not fail")`,
-//! /root/reference/halo2-base/src/utils/testing.rs:48), which is safe under `panic = "unwind"` (reference Cargo.toml:31).
+//! halo2-base/src/utils/testing.rs:48), which is safe under `panic = "unwind"` (reference Cargo.toml:31).
 pub mod backend;
 pub mod ffi;

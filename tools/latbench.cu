@@ -50,19 +50,19 @@ __global__ void k_gen(Affine* pts) {  // 1024 valid points: multiples of G
 }
 int main() {
     Affine* pts; XYZZ* out; long long* cyc; uint64_t* fo;
-    cudaMalloc(&pts, 1024 * sizeof(Affine)); cudaMalloc(&out, 148 * 1024 * sizeof(XYZZ)); cudaMalloc(&cyc, 8); cudaMalloc(&fo, 148*1024*32);
+    cudaMalloc(&pts, 1024 * sizeof(Affine)); cudaMalloc(&out, 132 * 1024 * sizeof(XYZZ)); cudaMalloc(&cyc, 8); cudaMalloc(&fo, 132*1024*32);
     k_gen<<<8, 128>>>(pts); cudaDeviceSynchronize();
     int iters = 200;
-    struct { int blocks, threads; const char* name; } cfg[] = {{1, 32, "1 warp"}, {1, 128, "1 CTA x 4 warps (1/SMSP)"}, {148, 128, "148 CTA x 4 warps"}, {148, 512, "148 x 16 warps (4/SMSP)"}, {148, 1024, "148 x 32 warps (8/SMSP)"}};
+    struct { int blocks, threads; const char* name; } cfg[] = {{1, 32, "1 warp"}, {1, 128, "1 CTA x 4 warps (1/SMSP)"}, {132, 128, "132 CTA x 4 warps"}, {132, 512, "132 x 16 warps (4/SMSP)"}, {132, 1024, "132 x 32 warps (8/SMSP)"}};
     {
         long long h2[2];
         cudaFree(cyc); cudaMalloc(&cyc, 16);
         k_quadchain<<<1, 32>>>(pts, out, iters, cyc); cudaDeviceSynchronize();
         cudaMemcpy(h2, cyc, 16, cudaMemcpyDeviceToHost);
         printf("quad_add chain  1 warp (8 quads)   %8.0f cycles/op    quad_dbl chain %8.0f cycles/op\n", (double)h2[0] / iters, (double)h2[1] / iters);
-        k_quadchain<<<148, 128>>>(pts, out, iters, cyc); cudaDeviceSynchronize();
+        k_quadchain<<<132, 128>>>(pts, out, iters, cyc); cudaDeviceSynchronize();
         cudaMemcpy(h2, cyc, 16, cudaMemcpyDeviceToHost);
-        printf("quad_add chain  148 x 4 warps      %8.0f cycles/op    quad_dbl chain %8.0f cycles/op\n", (double)h2[0] / iters, (double)h2[1] / iters);
+        printf("quad_add chain  132 x 4 warps      %8.0f cycles/op    quad_dbl chain %8.0f cycles/op\n", (double)h2[0] / iters, (double)h2[1] / iters);
     }
     for (auto& c : cfg) {
         long long h;

@@ -1,6 +1,6 @@
-// pipebench.cu — issue-rate microbenchmark of the sm_100a pipes the 254-bit field arithmetic can use.
+// pipebench.cu — issue-rate microbenchmark of the sm_90a pipes the 254-bit field arithmetic can use.
 // Prints warp-instructions per clock per SM for IMAD.WIDE.U32, IMAD, IMAD.HI, DFMA, IADD3 and mixes.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipebench tools/pipebench.cu ; run on the GPU box.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipebench tools/pipebench.cu ; run on the GPU box.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -50,7 +50,7 @@ void run(const char* name, uint64_t* d_out, int blocks) {
 int main() {
     uint64_t* d_out;
     cudaMalloc(&d_out, 8 * 4096);
-    int sms = 148;
+    int sms = 132;
     run<0>("IMAD.WIDE.U32", d_out, sms);
     run<1>("IMAD (lo)", d_out, sms);
     run<2>("IMAD.HI.U32", d_out, sms);

@@ -1,7 +1,7 @@
 """Device timings of the "next-row" kernels (SURVEY.md §8(f) ranks 1, 2, 4) at the ECDSA shape (k = 19, extended 2^21),
 resident inputs, CUDA events on the launching stream; algorithmic bytes per call and the HBM fraction beside them, and
-the CPU oracle timed on the same inputs.  Usage (on the GPU box): python tools/prof_quotient.py [k] > profiles/...txt"""
-import os, sys, time, json, ctypes as C
+the CPU oracle timed on the same inputs.  Usage (on the GPU box): python tools/prof_quotient.py [k]"""
+import os, sys, time, ctypes as C
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np, torch
@@ -18,11 +18,7 @@ dev = torch.device("cuda", 0)
 ctx = h.Context(0)
 stream = torch.cuda.Stream(device=dev); torch.cuda.set_stream(stream); ctx.set_stream(stream.cuda_stream)
 rng = np.random.default_rng(5)
-try:
-    peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    peak = float(peak.get("hbm_gbs") or 0) or 7000.0
-except Exception:
-    peak = 7000.0
+peak = 3350.0  # GB/s: H100 SXM data-sheet HBM3 bandwidth
 
 def rnd(m):
     x = rng.integers(0, 1 << 62, size=(m, 4), dtype=np.int64).astype(np.uint64); x[:, 3] &= np.uint64((1 << 60) - 1); return x
