@@ -113,13 +113,6 @@ int h2b_ctx_create(int device, h2b_ctx** out) {
         H2B_CUDA(cudaSetDevice(device));
         ctx = new h2b_ctx();
         ctx->device = device;
-        {
-            // experiment knob: the MSM gathers 64-byte table points at random; H2B_L2_FETCH=32|64|128 sets the L2 fetch
-            // granularity hint (cudaLimitMaxL2FetchGranularity)
-            const char* e = getenv("H2B_L2_FETCH");
-            const int g = e ? atoi(e) : 0;  // unset: the driver default
-            if (g == 32 || g == 64 || g == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)g);
-        }
         {   // the context's own stream sits at the lanes' priority: above the side queue (see the lane streams below)
             int lo_prio = 0, hi_prio = 0;
             H2B_CUDA(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
@@ -139,8 +132,7 @@ int h2b_ctx_create(int device, h2b_ctx** out) {
                 // beside the commitments — the polynomial transforms fill the bubbles the MSM pipeline leaves.
                 int lo_prio = 0, hi_prio = 0;
                 H2B_CUDA(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
-                static const int flat = [] { const char* e = getenv("H2B_LANE_PRIORITY"); return e ? atoi(e) == 0 : 0; }();
-                H2B_CUDA(cudaStreamCreateWithPriority(&ctx->lane_stream[l], cudaStreamNonBlocking, flat ? lo_prio : (lo_prio + hi_prio) / 2));
+                H2B_CUDA(cudaStreamCreateWithPriority(&ctx->lane_stream[l], cudaStreamNonBlocking, (lo_prio + hi_prio) / 2));
                 H2B_CUDA(cudaStreamCreateWithPriority(&ctx->lane_tail[l], cudaStreamNonBlocking, hi_prio));
             }
             H2B_CUDA(cudaEventCreateWithFlags(&ctx->lane_acc[l], cudaEventDisableTiming));
@@ -287,11 +279,7 @@ int h2b_ctx_set_option(h2b_ctx* ctx, const char* key, int64_t value) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(key, "set_option: null key");
         const std::string k(key);
-        if (k == "msm.affine_levels") { H2B_REQUIRE(value >= -1 && value <= 3, "msm.affine_levels: -1 (default) .. 3"); ctx->opt_affine_levels = (int)value; }
-        else if (k == "msm.affine_k") { H2B_REQUIRE(value == -1 || (value >= 8 && value <= 128 && value % 4 == 0), "msm.affine_k: multiple of 4 in [8, 128]"); ctx->opt_affine_k = (int)value; }
-        else if (k == "msm.affine_per_thread_inverse") { H2B_REQUIRE(value >= -1 && value <= 1, "msm.affine_per_thread_inverse: -1, 0 or 1"); ctx->opt_affine_pt = (int)value; }
-        else if (k == "msm.tail_priority") { H2B_REQUIRE(value >= -1 && value <= 1, "msm.tail_priority: -1 (default), 0 or 1"); ctx->opt_tail_priority = (int)value; }
-        else if (k == "ntt.max_ctas_per_sm") { H2B_REQUIRE(value >= 0 && value <= 2, "ntt.max_ctas_per_sm: 0 (no limit), 1 or 2"); ctx->opt_ntt_ctas = (int)value; }
+        if (k == "ntt.max_ctas_per_sm") { H2B_REQUIRE(value >= 0 && value <= 2, "ntt.max_ctas_per_sm: 0 (no limit), 1 or 2"); ctx->opt_ntt_ctas = (int)value; }
         else if (k == "msm.batch_group") { H2B_REQUIRE(value >= 0 && value <= 16, "msm.batch_group: 0 (default) .. 16 MSMs per pipeline"); ctx->opt_msm_group = (int)value; }
         else if (k == "lookup.leftover_order") { H2B_REQUIRE(value == 0 || value == 1, "lookup.leftover_order: 0 (front to back) or 1 (zcash: from the back)"); ctx->opt_lookup_backward = (int)value; }
         else H2B_REQUIRE(false, "set_option: unknown key");
@@ -1429,7 +1417,7 @@ int h2b_poly_lincomb(h2b_ctx* ctx, const uint64_t* const* polys, const uint64_t*
 // ------------------------------------------------------------------------------------------------ test hook
 int h2b_test_field_op(h2b_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) {
     return guarded(ctx, [&] {
-        H2B_REQUIRE(a && out && (b || (op > 2 && op < 7) || op == 9 || op == 10) && (field == 0 || field == 1) && op >= 0 && op <= 10, "field_op: bad argument");
+        H2B_REQUIRE(a && out && (b || (op > 2 && op < 7) || op == 9) && (field == 0 || field == 1) && op >= 0 && op <= 9, "field_op: bad argument");
         if (n == 0) return;
         char* d = (char*)ctx->get(WS_ASSIGN_IN, 3 * n * 32);
         H2B_CUDA(cudaMemcpyAsync(d, a, n * 32, cudaMemcpyHostToDevice, ctx->stream));

@@ -176,11 +176,7 @@ struct __align__(16) Fp {
     // Bounds: running total < 2p before a row and < 2^288 * 2^(32 i) after the products, so the chains
     // that would carry into position i+9 cannot, and the final sum is < 2p.
     __device__ __forceinline__ friend Fp operator*(const Fp& a, const Fp& b) {
-#ifdef H2B_MUL_KARATSUBA  // not the default (see the note at mul_karatsuba): kept for reference only
-        return mul_karatsuba(a, b);
-#else
         return mul_cios(a, b);
-#endif
     }
     __device__ __forceinline__ static Fp mul_cios(const Fp& a, const Fp& b) {
         u32 E[17], O[17];
@@ -305,133 +301,12 @@ struct __align__(16) Fp {
         return mul_add_mul(a, b, c.neg(), d);
     }
 
-    // ---- Karatsuba variant: 48 + 64 = 112 wide multiplies instead of 128 (NOT the default) ------------------------
-    // ptxas needs far more instructions for it than for the CIOS form above (incl. IMAD.MOV / IMAD.X on the multiplier
-    // pipe), which makes k_accumulate issue- and register-bound; tools/latbench.cu compares the two forms.
-    // The idea: the integer multiplier is the scarce resource (plain adds run on the otherwise idle ALU pipe), so one
-    // Karatsuba level on the 8x8-limb product
-    // trades 16 wide multiplies for ~100 additions:  a = a0 + a1 X, b = b0 + b1 X, X = 2^128,
-    //     a*b = z0 + (z0 + z2 - (a0 - a1)(b0 - b1)) X + z2 X^2,   z0 = a0 b0, z2 = a1 b1.
-    // 4x4-limb product r[0..8) = x * y.  E / O are position-indexed accumulators for products that start at even /
-    // odd limb positions; every chain ends in a carry limb that so far holds only carry counts (see operator*).
-    __device__ __forceinline__ static void mul4(const u32* x, const u32* y, u32* r) {
-        u32 E[10], O[10];
-#pragma unroll
-        for (int k = 0; k < 10; k++) { E[k] = 0; O[k] = 0; }
-#pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const u32 yi = y[i];
-            // products x[j]*y[i] at position i+j; j and j+2 share parity: one carry chain per parity
-            u32* A = (i & 1) ? O : E;  // gets j = 0, 2 (positions i, i+2)
-            u32* B = (i & 1) ? E : O;  // gets j = 1, 3 (positions i+1, i+3)
-            mad_lo_cc(A[i], x[0], yi);      madc_hi_cc(A[i + 1], x[0], yi);
-            madc_lo_cc(A[i + 2], x[2], yi); madc_hi_cc(A[i + 3], x[2], yi);
-            addc(A[i + 4], A[i + 4], 0);
-            mad_lo_cc(B[i + 1], x[1], yi);  madc_hi_cc(B[i + 2], x[1], yi);
-            madc_lo_cc(B[i + 3], x[3], yi); madc_hi_cc(B[i + 4], x[3], yi);
-            addc(B[i + 5], B[i + 5], 0);
-        }
-        add_cc(r[0], E[0], O[0]);
-#pragma unroll
-        for (int k = 1; k < 7; k++) addc_cc(r[k], E[k], O[k]);
-        addc(r[7], E[7], O[7]);
-    }
-    // |x - y| over 4 limbs; returns all-ones if x < y
-    __device__ __forceinline__ static u32 absdiff4(const u32* x, const u32* y, u32* d) {
-        u32 t[4], borrow;
-        sub_cc(t[0], x[0], y[0]);
-        subc_cc(t[1], x[1], y[1]);
-        subc_cc(t[2], x[2], y[2]);
-        subc_cc(t[3], x[3], y[3]);
-        subc(borrow, 0, 0);
-        // negate when negative: (t ^ borrow) - borrow
-        sub_cc(d[0], t[0] ^ borrow, borrow);
-        subc_cc(d[1], t[1] ^ borrow, borrow);
-        subc_cc(d[2], t[2] ^ borrow, borrow);
-        subc(d[3], t[3] ^ borrow, borrow);
-        return borrow;
-    }
-    __device__ __forceinline__ static Fp mul_karatsuba(const Fp& a, const Fp& b) {
-        u32 z0[8], z2[8], zm[8], da[4], db[4];
-        mul4(a.l, b.l, z0);
-        mul4(a.l + 4, b.l + 4, z2);
-        const u32 sa = absdiff4(a.l, a.l + 4, da), sb = absdiff4(b.l, b.l + 4, db);
-        mul4(da, db, zm);
-        // mid = z0 + z2 -+ zm  (9 limbs).  neg = all-ones when (a0-a1)(b0-b1) > 0, i.e. zm is SUBTRACTED
-        const u32 neg = ~(sa ^ sb);
-        u32 mid[9];
-        add_cc(mid[0], z0[0], z2[0]);
-#pragma unroll
-        for (int k = 1; k < 8; k++) addc_cc(mid[k], z0[k], z2[k]);
-        addc(mid[8], 0, 0);
-        // mid += (zm ^ neg) + (neg & 1), top limb += neg  (two's complement subtraction when neg)
-        add_cc(mid[0], mid[0], neg & 1u);
-#pragma unroll
-        for (int k = 1; k < 8; k++) addc_cc(mid[k], mid[k], 0);
-        addc(mid[8], mid[8], 0);
-        add_cc(mid[0], mid[0], zm[0] ^ neg);
-#pragma unroll
-        for (int k = 1; k < 8; k++) addc_cc(mid[k], mid[k], zm[k] ^ neg);
-        addc(mid[8], mid[8], neg);
-        // T = z0 + mid * 2^128 + z2 * 2^256  (16 limbs: lo = T[0..8), hi = T[8..16))
-        u32 lo[8], hi[8];
-#pragma unroll
-        for (int k = 0; k < 4; k++) lo[k] = z0[k];
-        add_cc(lo[4], z0[4], mid[0]);
-        addc_cc(lo[5], z0[5], mid[1]);
-        addc_cc(lo[6], z0[6], mid[2]);
-        addc_cc(lo[7], z0[7], mid[3]);
-        addc_cc(hi[0], z2[0], mid[4]);
-        addc_cc(hi[1], z2[1], mid[5]);
-        addc_cc(hi[2], z2[2], mid[6]);
-        addc_cc(hi[3], z2[3], mid[7]);
-        addc_cc(hi[4], z2[4], mid[8]);
-        addc_cc(hi[5], z2[5], 0);
-        addc_cc(hi[6], z2[6], 0);
-        addc(hi[7], z2[7], 0);
-        // Montgomery reduction of the low half (8 rows, same even/odd accumulators as operator*), then + hi
-        u32 E[17], O[17];
-#pragma unroll
-        for (int k = 0; k < 17; k++) { E[k] = 0; O[k] = 0; }
-#pragma unroll
-        for (int k = 0; k < 8; k++) E[k] = lo[k];
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            u32* X = (i & 1) ? O : E;
-            u32* Y = (i & 1) ? E : O;
-            if (i > 0) add_cc(X[i], X[i], Y[i]);  // fold Y's live limb; the carry enters the Y chain below
-            const u32 m = X[i] * P::INV;
-            if (i > 0) { madc_lo_cc(Y[i + 1], m, P::MOD(1)); } else { mad_lo_cc(Y[i + 1], m, P::MOD(1)); }
-            madc_hi_cc(Y[i + 2], m, P::MOD(1));
-            madc_lo_cc(Y[i + 3], m, P::MOD(3)); madc_hi_cc(Y[i + 4], m, P::MOD(3));
-            madc_lo_cc(Y[i + 5], m, P::MOD(5)); madc_hi_cc(Y[i + 6], m, P::MOD(5));
-            madc_lo_cc(Y[i + 7], m, P::MOD(7)); madc_hi(Y[i + 8], m, P::MOD(7));
-            mad_lo_cc(X[i], m, P::MOD(0));      madc_hi_cc(X[i + 1], m, P::MOD(0));
-            madc_lo_cc(X[i + 2], m, P::MOD(2)); madc_hi_cc(X[i + 3], m, P::MOD(2));
-            madc_lo_cc(X[i + 4], m, P::MOD(4)); madc_hi_cc(X[i + 5], m, P::MOD(4));
-            madc_lo_cc(X[i + 6], m, P::MOD(6)); madc_hi_cc(X[i + 7], m, P::MOD(6));
-            addc(X[i + 8], X[i + 8], 0);
-        }
-        Fp s;
-        add_cc(s.l[0], E[8], O[8]);
-#pragma unroll
-        for (int k = 1; k < 7; k++) addc_cc(s.l[k], E[8 + k], O[8 + k]);
-        addc(s.l[7], E[15], O[15]);
-        add_cc(s.l[0], s.l[0], hi[0]);
-#pragma unroll
-        for (int k = 1; k < 7; k++) addc_cc(s.l[k], s.l[k], hi[k]);
-        addc(s.l[7], s.l[7], hi[7]);
-        return reduce_once(s);
-    }
     // Montgomery square: the same row structure as mul_cios, but row i only multiplies a_i by the limbs j >= i of
     //     a_i, (a_{i+1} << 1), d_{i+2}, ..., d_7        with d = 2a (funnel-shifted limbs),
     // i.e. a_i^2 plus the doubled cross products, each computed once: 36 + 64 = 100 wide multiplies instead of 128.
     // (2 * sum_{j>i} a_j 2^(32j) = sum_{j>i} d_j 2^(32j) minus the top bit of a_i that leaked into d_{i+1}; a < 2^254
     // so d_8 = 0.)  Skipped products of the odd-limb chain still have to pass the carry on: two adds instead of a MAD.
     __device__ __forceinline__ Fp sqr() const {
-#ifdef H2B_NO_DEDICATED_SQR
-        return (*this) * (*this);
-#else
         const Fp& a = *this;
         u32 d[8];
         d[0] = a.l[0] << 1;
@@ -489,7 +364,6 @@ struct __align__(16) Fp {
         for (int k = 1; k < 7; k++) addc_cc(s.l[k], E[8 + k], O[8 + k]);
         addc(s.l[7], E[15], O[15]);
         return reduce_once(s);
-#endif
     }
 
     // Montgomery form -> canonical integer (what `to_repr()` yields; best_multiexp slices these bits)
@@ -567,156 +441,6 @@ struct __align__(16) Fp {
             else { sub_if_geq(v, u); x2 = x2 - x1; }
         }
         return r * (r2() * r2());  // R^2 * R^2 * R^-1 = R^3;  r * R^3 * R^-1 = r R^2 = a^-1 R
-    }
-
-    // ---- a^-1 by constant-time "safegcd" (Bernstein-Yang divsteps; the 30-bit batched form of libsecp256k1's modinv32,
-    // restated): 20 rounds of 30 divsteps on the low words build a 2x2 transition matrix that is then applied to the
-    // full-width (f, g) and, modulo p, to (d, e) with f = d*A, g = e*A.  No data-dependent branch: every lane of a warp
-    // can invert its own element at once, and the work is ~10k add / shift / logic instructions plus ~1800 wide
-    // multiplies (the cost of ~15 products) — it runs mostly on the ALU pipe that the Montgomery products leave idle.
-    // Used where EVERY thread needs its own inverse (per-thread Montgomery trick in the batch-affine path); the
-    // single-lane paths keep inv_bgcd.  inv(0) = 0.  Signed 30-bit limbs: value = sum l[i] 2^(30 i), l[0..7] in [0, 2^30).
-    __host__ __device__ static constexpr u32 MOD30(int i) {  // limb i of p in base 2^30
-        u64 lo = 0;
-        // bits [30 i, 30 i + 30) of the 256-bit modulus
-        const int bit = 30 * i, w = bit >> 5, off = bit & 31;
-        lo = (u64)(w < 8 ? P::MOD(w) : 0u) | ((u64)(w + 1 < 8 ? P::MOD(w + 1) : 0u) << 32);
-        return (u32)((lo >> off) & 0x3fffffffu);
-    }
-    __host__ __device__ static constexpr u32 MODINV30() {  // p^-1 mod 2^30 (Newton iteration on the low word)
-        u32 p0 = P::MOD(0), x = p0;  // x = p^-1 mod 2^3 for odd p
-        for (int i = 0; i < 5; i++) x *= 2u - p0 * x;
-        return x & 0x3fffffffu;
-    }
-    __device__ __noinline__ Fp inv_safegcd() const {
-        constexpr int32_t M30 = 0x3fffffff;
-        int32_t d[9], e[9], f[9], g[9];
-        // A (Montgomery limbs, 8 x 32 bits) -> g; p -> f; d = 0, e = 1
-        {
-            u32 w[9];
-#pragma unroll
-            for (int i = 0; i < 8; i++) w[i] = l[i];
-            w[8] = 0;
-#pragma unroll
-            for (int i = 0; i < 9; i++) {
-                const int bit = 30 * i, wi = bit >> 5, off = bit & 31;
-                u64 two = (u64)w[wi] | ((u64)(wi + 1 < 9 ? w[wi + 1] : 0u) << 32);
-                g[i] = (int32_t)((two >> off) & 0x3fffffffu);
-                f[i] = (int32_t)MOD30(i);
-                d[i] = 0;
-                e[i] = 0;
-            }
-            e[0] = 1;
-        }
-        int32_t zeta = -1;  // -(delta + 1/2), delta = 1/2
-#pragma unroll 1
-        for (int round = 0; round < 20; round++) {
-            // 30 divsteps on the low words
-            u32 u = 1, v = 0, q = 0, r = 1;
-            u32 ff = (u32)f[0] | ((u32)f[1] << 30), gg = (u32)g[0] | ((u32)g[1] << 30);
-#pragma unroll 6
-            for (int i = 0; i < 30; i++) {
-                u32 c1 = (u32)(zeta >> 31);
-                const u32 mask2 = 0u - (gg & 1u);
-                const u32 x = (ff ^ c1) - c1, y = (u ^ c1) - c1, z = (v ^ c1) - c1;
-                gg += x & mask2;
-                q += y & mask2;
-                r += z & mask2;
-                c1 &= mask2;
-                zeta = (int32_t)(((u32)zeta ^ c1) - 1u);
-                ff += gg & c1;
-                u += q & c1;
-                v += r & c1;
-                gg >>= 1;
-                u <<= 1;
-                v <<= 1;
-            }
-            const int64_t tu = (int32_t)u, tv = (int32_t)v, tq = (int32_t)q, tr = (int32_t)r;
-            // (d, e) <- t * (d, e) / 2^30 mod p
-            {
-                const int32_t sd = d[8] >> 31, se = e[8] >> 31;
-                int32_t md = ((int32_t)tu & sd) + ((int32_t)tv & se), me = ((int32_t)tq & sd) + ((int32_t)tr & se);
-                int64_t cd = tu * d[0] + tv * e[0], ce = tq * d[0] + tr * e[0];
-                md -= (int32_t)((MODINV30() * (u32)cd + (u32)md) & (u32)M30);
-                me -= (int32_t)((MODINV30() * (u32)ce + (u32)me) & (u32)M30);
-                cd += (int64_t)MOD30(0) * md;
-                ce += (int64_t)MOD30(0) * me;
-                cd >>= 30;
-                ce >>= 30;
-#pragma unroll
-                for (int i = 1; i < 9; i++) {
-                    cd += tu * d[i] + tv * e[i] + (int64_t)MOD30(i) * md;
-                    ce += tq * d[i] + tr * e[i] + (int64_t)MOD30(i) * me;
-                    d[i - 1] = (int32_t)cd & M30;
-                    e[i - 1] = (int32_t)ce & M30;
-                    cd >>= 30;
-                    ce >>= 30;
-                }
-                d[8] = (int32_t)cd;
-                e[8] = (int32_t)ce;
-            }
-            // (f, g) <- t * (f, g) / 2^30 (exact)
-            {
-                int64_t cf = tu * f[0] + tv * g[0], cg = tq * f[0] + tr * g[0];
-                cf >>= 30;
-                cg >>= 30;
-#pragma unroll
-                for (int i = 1; i < 9; i++) {
-                    cf += tu * f[i] + tv * g[i];
-                    cg += tq * f[i] + tr * g[i];
-                    f[i - 1] = (int32_t)cf & M30;
-                    g[i - 1] = (int32_t)cg & M30;
-                    cf >>= 30;
-                    cg >>= 30;
-                }
-                f[8] = (int32_t)cf;
-                g[8] = (int32_t)cg;
-            }
-        }
-        // g = 0, f = +-1 (f = p when A = 0, then d = 0): result = sign(f) * d, brought into [0, p)
-        // signed limbs -> 288-bit two's complement words
-        u32 w[9];
-        {
-            int64_t acc = 0;
-            int have = 0, li = 0;
-#pragma unroll
-            for (int j = 0; j < 9; j++) {
-#pragma unroll
-                for (int rep = 0; rep < 3; rep++) {
-                    if (have < 32 && li < 9) {
-                        acc += (int64_t)((u64)(li < 8 ? (int64_t)d[li] : (int64_t)d[8]) << have);
-                        have += 30;
-                        li++;
-                    }
-                }
-                w[j] = (u32)acc;
-                acc >>= 32;
-                have -= 32;
-            }
-        }
-        const u32 negf = (u32)(f[8] >> 31);  // all ones when f = -1
-        {   // w <- negf ? -w : w
-            u32 c;
-            add_cc(w[0], w[0] ^ negf, negf & 1u);
-#pragma unroll
-            for (int i = 1; i < 8; i++) addc_cc(w[i], w[i] ^ negf, 0);
-            addc(w[8], w[8] ^ negf, 0);
-            (void)c;
-        }
-        // w in (-2p, 2p): add p while negative (twice), then subtract p once if >= p
-#pragma unroll
-        for (int rep = 0; rep < 2; rep++) {
-            const u32 neg = (u32)((int32_t)w[8] >> 31);
-            add_cc(w[0], w[0], P::MOD(0) & neg);
-#pragma unroll
-            for (int i = 1; i < 8; i++) addc_cc(w[i], w[i], P::MOD(i) & neg);
-            addc(w[8], w[8], 0);
-        }
-        Fp res;
-#pragma unroll
-        for (int i = 0; i < 8; i++) res.l[i] = w[i];
-        res = reduce_once(res);  // w[8] == 0 now and the value is < 2p
-        return res * (r2() * r2());  // plain residue (aR)^-1 -> Montgomery a^-1 R
     }
 };
 

@@ -61,8 +61,6 @@ enum WsSlot {
     WS_ASSIGN_OUT,
     WS_MISC,
     WS_MISC2,
-    WS_RED_A,         // batch-affine group sums (ping)
-    WS_RED_B,         // batch-affine group sums (pong)
     WS_PROD,          // product-column scratch (numerators, denominators, power tables)
     WS_COUNT
 };
@@ -88,11 +86,7 @@ struct h2b_ctx {
     std::string err;
     uint64_t launches = 0;
     bool ntt_attr_set = false;
-    int opt_affine_levels = -1;  // h2b_ctx_set_option("msm.affine_levels"): -1 = default
-    int opt_affine_k = -1;       // "msm.affine_k"
-    int opt_affine_pt = -1;      // "msm.affine_per_thread_inverse": 1 = every thread inverts (safegcd), 0 = one inversion per tile
-    int opt_tail_priority = -1;  // "msm.tail_priority": bucket reductions of lane MSMs on high-priority streams (-1 = default on)
-    int opt_ntt_ctas = 0;        // "ntt.max_ctas_per_sm": 0 = as many as fit, 1 or 2 = background transform (see ntt_run)
+    int opt_ntt_ctas = 0;        // h2b_ctx_set_option("ntt.max_ctas_per_sm"): 0 = as many as fit, 1 or 2 = background transform (see ntt_run)
     int opt_msm_group = 0;       // "msm.batch_group": MSMs of a batch call that share one sort / accumulate / reduce pipeline (0 = by size)
     int opt_lookup_backward = 0; // "lookup.leftover_order": 0 = front to back (PSE / axiom walk), 1 = zcash (pop from the back)
     void* peer = nullptr;  // PeerState (peer.cu): NVLink mailboxes of the multi-GPU all-reduce

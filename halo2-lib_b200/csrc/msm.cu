@@ -25,7 +25,6 @@
 // windows of a scalar fall into ONE bucket set: no per-window reduction and no final doublings.
 #include "curve.cuh"
 #include "quad.cuh"
-#include "batch_affine.cuh"
 #include "h2b_internal.cuh"
 
 namespace h2b {
@@ -132,13 +131,12 @@ __global__ void __launch_bounds__(256) k_digits(const __grid_constant__ MsmScala
 // k_scan_tiles: off[b] = exclusive prefix inside the tile, tile_sums[tile] = tile total.
 // k_scan_apply: adds the sum of the preceding tile totals; cursor[b] = off[b]; off[nb] = grand total.
 static constexpr int SCAN_TILE = 2048;
-// `gmask` = G - 1: every bucket's run is padded to a multiple of G = 2^R slots (batch_affine.cuh); 0 = no padding.
 __global__ void __launch_bounds__(256) k_scan_tiles(const u32* __restrict__ hist, u32 nb, u32* __restrict__ off,
-                                                    u32* __restrict__ tile_sums, u32 gmask) {
+                                                    u32* __restrict__ tile_sums) {
     __shared__ u32 sh[SCAN_TILE];
     __shared__ u32 wsum[8];
     const u32 base = blockIdx.x * SCAN_TILE, t = threadIdx.x;
-    for (u32 e = t; e < SCAN_TILE; e += 256) sh[e] = (base + e < nb) ? ((hist[base + e] + gmask) & ~gmask) : 0;  // coalesced
+    for (u32 e = t; e < SCAN_TILE; e += 256) sh[e] = (base + e < nb) ? hist[base + e] : 0;  // coalesced
     __syncthreads();
     u32 v[8], sum = 0;
 #pragma unroll
@@ -163,12 +161,9 @@ __global__ void __launch_bounds__(256) k_scan_tiles(const u32* __restrict__ hist
         if (base + e < nb) off[base + e] = sh[e];
     if (t == 255) tile_sums[blockIdx.x] = run;
 }
-// With padding (shift = R > 0) the slots [off[b] + hist[b], off[b + 1]) of every bucket are filled with BA_PAD here, and the
-// chunk length is chosen for the M' >> R group sums k_accumulate will walk.
 __global__ void __launch_bounds__(256) k_scan_apply(u32 nb, u32 ntiles, const u32* __restrict__ tile_sums,
                                                     u32* __restrict__ off, u32* __restrict__ cursor, u32 slots,
-                                                    u32 l_min, u32 l_max, u32* __restrict__ d_L, const u32* __restrict__ hist,
-                                                    u32* __restrict__ vals, int shift) {
+                                                    u32 l_min, u32 l_max, u32* __restrict__ d_L) {
     __shared__ u32 red[256];
     const u32 t = threadIdx.x;
     u32 s = 0;
@@ -185,15 +180,10 @@ __global__ void __launch_bounds__(256) k_scan_apply(u32 nb, u32 ntiles, const u3
             u32 o = off[base + e] + add;
             off[base + e] = o;
             cursor[base + e] = o;
-            if (shift) {
-                const u32 h = hist[base + e], gm = (1u << shift) - 1u;
-                for (u32 p = o + h; p < o + ((h + gm) & ~gm); p++) vals[p] = BA_PAD;
-            }
         }
     if (blockIdx.x == ntiles - 1 && t == 0) {
-        const u32 mv_all = add + tile_sums[ntiles - 1];
-        off[nb] = mv_all;
-        const u32 mv = mv_all >> shift;
+        const u32 mv = add + tile_sums[ntiles - 1];
+        off[nb] = mv;
         // chunk length for k_accumulate: whole waves of equally long chunks (see k_accumulate)
         u32 L = l_max;
         if (mv < l_max * slots) {  // less than one full wave of l_max-chunks: spread the entries over every slot
@@ -211,15 +201,13 @@ __device__ __forceinline__ Affine load_signed(const Affine* __restrict__ table, 
     return p;
 }
 
-// Offsets are stored in units of sorted entries; with batch-affine reduction k_accumulate and the collect kernels walk
-// group sums, i.e. positions in units of 2^sh entries (every offset is a multiple of 2^sh then).
-__device__ __forceinline__ u32 offs(const u32* __restrict__ off, u32 b, int sh) { return __ldg(off + b) >> sh; }
+__device__ __forceinline__ u32 offs(const u32* __restrict__ off, u32 b) { return __ldg(off + b); }
 // first bucket b in [lo, nb) with off[b + 1] > pos  (the bucket that owns sorted position pos)
-__device__ __forceinline__ u32 bucket_of(const u32* __restrict__ off, u32 lo, u32 nb, u32 pos, int sh) {
+__device__ __forceinline__ u32 bucket_of(const u32* __restrict__ off, u32 lo, u32 nb, u32 pos) {
     u32 hi = nb;
     while (lo < hi) {
         u32 mid = (lo + hi) >> 1;
-        if (offs(off, mid + 1, sh) > pos) hi = mid; else lo = mid + 1;
+        if (offs(off, mid + 1) > pos) hi = mid; else lo = mid + 1;
     }
     return lo;
 }
@@ -229,26 +217,21 @@ __device__ __forceinline__ u32 bucket_of(const u32* __restrict__ off, u32 lo, u3
 // 32-entry chunks (sparse witness columns, small shards) L = ceil(entries / slots), slots = resident threads of
 // this kernel, so that every SM is busy.  (Whole-wave balancing of dense columns was measured: no gain, the
 // kernel is multiplier-bound and a partially filled last wave simply runs faster.)
-// DIRECT = false: entry i is the table point vals[i] (index | sign).  DIRECT = true: entry i is the affine point pts[i]
-// (the group sums left by the batch-affine passes), positions in units of 2^sh sorted entries.
-template <bool DIRECT>
+// Entry i is the table point vals[i] (index | table bit | sign).
 __global__ void __launch_bounds__(128, 4) k_accumulate(const u32* __restrict__ vals, const u32* __restrict__ off,
                                                        u32 nb_total, const u32* __restrict__ d_L,
                                                        const Affine* __restrict__ table, const Affine* __restrict__ table_b,
-                                                       XYZZ* __restrict__ buckets, XYZZ* __restrict__ partials, int sh) {
+                                                       XYZZ* __restrict__ buckets, XYZZ* __restrict__ partials) {
     const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
     const u32 L = __ldg(d_L);
-    const u32 mv = offs(off, nb_total, sh);  // number of entries (non-zero digits, or group sums)
+    const u32 mv = offs(off, nb_total);  // number of entries (non-zero digits)
     const u64 cs64 = (u64)t * L;
     if (cs64 >= mv) return;
     const u32 cs = (u32)cs64;
     const u32 ce = (mv - cs < (u32)L) ? mv : cs + L;
-    u32 cur = bucket_of(off, 0, nb_total, cs, sh);
-    u32 run_end = offs(off, cur + 1, sh);
-    auto fetch = [&](u32 i) -> Affine {
-        if (DIRECT) return Affine::load(table + i);
-        return load_signed(table, table_b, __ldg(vals + i));
-    };
+    u32 cur = bucket_of(off, 0, nb_total, cs);
+    u32 run_end = offs(off, cur + 1);
+    auto fetch = [&](u32 i) -> Affine { return load_signed(table, table_b, __ldg(vals + i)); };
     XYZZ acc = XYZZ::identity();
     Affine p = fetch(cs);
     for (u32 i = cs; i < ce; i++) {
@@ -258,7 +241,7 @@ __global__ void __launch_bounds__(128, 4) k_accumulate(const u32* __restrict__ v
         xyzz_madd(acc, p);
         if (!more || i + 1 == run_end) {
             // the run of bucket `cur` ends here (inside this chunk or at its border)
-            const u32 s = offs(off, cur, sh);
+            const u32 s = offs(off, cur);
             if (s >= cs && run_end - cs <= (u32)L) acc.store(buckets + cur);    // bucket lies inside the chunk
             else if (s <= cs) acc.store(partials + 2 * (size_t)t);              // covers the chunk start
             else acc.store(partials + 2 * (size_t)t + 1);                        // starts inside, runs past the end
@@ -266,12 +249,12 @@ __global__ void __launch_bounds__(128, 4) k_accumulate(const u32* __restrict__ v
             if (more) {  // next non-empty bucket: a few linear steps, then binary search (long empty gaps)
                 u32 b = cur + 1;
                 int steps = 0;
-                while (offs(off, b + 1, sh) <= i + 1) {
+                while (offs(off, b + 1) <= i + 1) {
                     b++;
-                    if (++steps == 4) { b = bucket_of(off, b, nb_total, i + 1, sh); break; }
+                    if (++steps == 4) { b = bucket_of(off, b, nb_total, i + 1); break; }
                 }
                 cur = b;
-                run_end = offs(off, cur + 1, sh);
+                run_end = offs(off, cur + 1);
             }
         }
         if (more) p = pn;
@@ -285,11 +268,11 @@ __device__ __forceinline__ const XYZZ* partial_of(const XYZZ* partials, u32 s, u
 // one thread per bucket: empty -> identity; spans several chunks -> add their partials
 __global__ void __launch_bounds__(128) k_collect(const u32* __restrict__ off, u32 nb_total, const u32* __restrict__ d_L,
                                                  const XYZZ* __restrict__ partials, XYZZ* __restrict__ buckets,
-                                                 u32* __restrict__ big_list, u32* __restrict__ big_count, int sh) {
+                                                 u32* __restrict__ big_list, u32* __restrict__ big_count) {
     u32 b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nb_total) return;
     const u32 L = __ldg(d_L);
-    const u32 s = offs(off, b, sh), e = offs(off, b + 1, sh);
+    const u32 s = offs(off, b), e = offs(off, b + 1);
     if (s == e) {
         XYZZ::identity().store(buckets + b);
         return;
@@ -312,7 +295,7 @@ __global__ void __launch_bounds__(128) k_collect(const u32* __restrict__ off, u3
 static constexpr int BIG_SEG = 64;
 __global__ void __launch_bounds__(256) k_collect_big1(const u32* __restrict__ off, const u32* __restrict__ d_L, const XYZZ* __restrict__ partials,
                                                       const u32* __restrict__ big_list, const u32* __restrict__ big_count,
-                                                      XYZZ* __restrict__ seg, int shf) {
+                                                      XYZZ* __restrict__ seg) {
     __shared__ XYZZ sh[8];
     const u32 nbig = *big_count;
     const u32 L = __ldg(d_L);
@@ -321,7 +304,7 @@ __global__ void __launch_bounds__(256) k_collect_big1(const u32* __restrict__ of
     u32 g = blockIdx.x;  // next segment of this CTA (segments are numbered across all big buckets)
     for (u32 j = 0; j < nbig; j++) {
         const u32 b = big_list[j];
-        const u32 s = offs(off, b, shf), e = offs(off, b + 1, shf);
+        const u32 s = offs(off, b), e = offs(off, b + 1);
         const u32 t_lo = s / L, t_hi = (e - 1) / L;
         const u32 cnt = t_hi - t_lo + 1, nseg = (cnt + BIG_SEG - 1) / BIG_SEG;
         for (; g < seg_base + nseg; g += gridDim.x) {
@@ -337,7 +320,7 @@ __global__ void __launch_bounds__(256) k_collect_big1(const u32* __restrict__ of
 }
 __global__ void __launch_bounds__(256) k_collect_big2(const u32* __restrict__ off, const u32* __restrict__ d_L, const XYZZ* __restrict__ seg,
                                                       XYZZ* __restrict__ buckets, const u32* __restrict__ big_list,
-                                                      const u32* __restrict__ big_count, int shf) {
+                                                      const u32* __restrict__ big_count) {
     __shared__ XYZZ sh[8];
     const u32 nbig = *big_count;
     const u32 L = __ldg(d_L);
@@ -345,7 +328,7 @@ __global__ void __launch_bounds__(256) k_collect_big2(const u32* __restrict__ of
     u32 seg_base = 0;
     for (u32 j = 0; j < nbig; j++) {
         const u32 b = big_list[j];
-        const u32 s = offs(off, b, shf), e = offs(off, b + 1, shf);
+        const u32 s = offs(off, b), e = offs(off, b + 1);
         const u32 cnt = (e - 1) / L - s / L + 1, nseg = (cnt + BIG_SEG - 1) / BIG_SEG;
         if (j % gridDim.x == blockIdx.x) {
             XYZZ acc = XYZZ::identity();
@@ -556,7 +539,6 @@ __global__ void __launch_bounds__(128) k_field_op(int op, const uint64_t* __rest
         case 7: r = F::mul_add_mul(x, y, x + y, x - y); break;  // a*b + (a+b)(a-b)
         case 8: r = F::mul_sub_mul(x, y, y, y); break;          // a*b - b*b
         case 9: r = x.inv_bgcd(); break;
-        case 10: r = x.inv_safegcd(); break;
         default: r = x.to_mont(); break;
     }
     r.store(out + 4 * (size_t)i);
@@ -565,12 +547,8 @@ __global__ void __launch_bounds__(128) k_field_op(int op, const uint64_t* __rest
 // ------------------------------------------------------------------------------------------------ host side
 int msm_choose_c_fixed(size_t n) {
     // one bucket set of 2^(c-1) buckets, ceil(255/c) table levels: cost ~ 10*n*W + 32*2^(c-1) field mults
-    if (const char* e = getenv("H2B_MSM_C")) {  // experiment override
-        int v = atoi(e);
-        if (v >= 4 && v <= 24) return v;
-    }
-    // W = ceil(255 / c) only drops at c = 13, 14, 15, 16, 17, 19, 20, 22, so only those are candidates (H2B_MSM_C and
-    // tools/prof_ops.py compare them): the bucket-side work grows 2^c while the additions only shrink with W.  Small
+    // W = ceil(255 / c) only drops at c = 13, 14, 15, 16, 17, 19, 20, 22, so only those are candidates (a sweep edits the
+    // constants below and rebuilds): the bucket-side work grows 2^c while the additions only shrink with W.  Small
     // domains — the shards of a multi-GPU run and the k <= 16 configs — want c close to log2(n): the fixed tail is
     // latency-bound and hardly grows with the bucket count, while fewer table levels shorten everything else.
     // Measured on an H100 80GB HBM3 at a 400 W power limit (one MSM, uniform / witness-like scalars): 2^19: c = 17
@@ -600,21 +578,6 @@ void msm_build_table(h2b_ctx* ctx, const void* d_bases, size_t count, int c, int
                    t + (size_t)w * count, (u32)count, c);
 }
 
-// Number of batch-affine halving levels (batch_affine.cuh) in front of k_accumulate.  Bit-exact, but the warps of a CTA
-// wait at the barrier around the single-lane inversion and the table points are gathered twice, so it is not expected
-// to beat the plain XYZZ accumulation.  It therefore stays an opt-in path:
-// h2b_ctx_set_option("msm.affine_levels", 1..3) or H2B_AFF_LEVELS; default 0.
-static int msm_choose_levels(const h2b_ctx* ctx, int q_is_table) {
-    static const int forced = [] {
-        const char* e = getenv("H2B_AFF_LEVELS");
-        return e ? atoi(e) : -1;
-    }();
-    if (!q_is_table) return 0;
-    if (ctx->opt_affine_levels >= 0 && ctx->opt_affine_levels <= 3) return ctx->opt_affine_levels;
-    if (forced >= 0 && forced <= 3) return forced;
-    return 0;
-}
-
 // m MSMs of the same size through one pipeline (table mode: q == W, one bucket set per MSM; ad-hoc mode: m == 1).
 // The m results are stored at d_out + 96 * j.
 void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, int W, int q, const void* const* d_scalars, size_t m,
@@ -629,10 +592,7 @@ void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, i
     const u32 nb_total = (u32)m * nb_group;
     const size_t M = (size_t)W * n * m;
     cudaStream_t st = ctx->stream;
-    const int R = m == 1 ? msm_choose_levels(ctx, q == W) : 0;  // batch-affine halving passes; groups of G = 2^R entries
-    const size_t G = (size_t)1 << R;
-    const size_t Mp = M + (G - 1) * nb_total;  // upper bound of the padded entry count
-    H2B_REQUIRE(Mp < ((size_t)1 << 32), "msm: padded entry count exceeds 32 bits");
+    H2B_REQUIRE(M < ((size_t)1 << 32), "msm: entry count exceeds 32 bits");
     MsmScalars cols;
     const Affine* tab_a = (const Affine*)d_tables[0];
     const Affine* tab_b = tab_a;
@@ -646,34 +606,18 @@ void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, i
     }
     H2B_REQUIRE(table_mask == 0 || (size_t)W * n < ((size_t)1 << 30), "msm: two-table groups need n * windows < 2^30");
 
-    u32* vals = (u32*)ctx->get(WS_VALS_A, Mp * 4 + 16);
-    u32* cnt = (u32*)ctx->get(WS_KEYS_A, (2 * ((size_t)nb_total + 2) + nb_total / SCAN_TILE + 8) * 4);  // histogram, cursors, tile sums, L, tile cursor
+    u32* vals = (u32*)ctx->get(WS_VALS_A, M * 4 + 16);
+    u32* cnt = (u32*)ctx->get(WS_KEYS_A, (2 * ((size_t)nb_total + 2) + nb_total / SCAN_TILE + 8) * 4);  // histogram, cursors, tile sums, L
     u32* hist = cnt;
     u32* cursor = cnt + nb_total + 2;
     u32* off = (u32*)ctx->get(WS_OFFSETS, ((size_t)nb_total + 2) * 4);
     XYZZ* buckets = (XYZZ*)ctx->get(WS_BUCKETS, (size_t)nb_total * sizeof(XYZZ));
-    static const int L_MAX = [] {  // H2B_ACC_L pins the chunk length (experiments); default: device-chosen in [12, 32]
-        const char* e = getenv("H2B_ACC_L");
-        int v = e ? atoi(e) : 0;
-        return (v >= 8 && v <= 64) ? v : 0;
-    }();
-    const u32 l_min = L_MAX ? (u32)L_MAX : 12u, l_max = L_MAX ? (u32)L_MAX : (u32)ACC_L_DEFAULT;
+    const u32 l_min = 12u, l_max = (u32)ACC_L_DEFAULT;  // chunk length of k_accumulate, chosen on the device in [12, 32]
     const u32 slots = (u32)ctx->sm_count * 512u;  // k_accumulate: 128 registers -> 4 CTAs x 128 threads per SM
     // chunks of k_accumulate: L < l_max is only chosen when the entries do not fill one wave, i.e. at most `slots` chunks
-    const size_t Macc = Mp >> R;
-    const size_t n_chunks = L_MAX ? (Macc + l_min - 1) / l_min : std::max((Macc + l_max - 1) / l_max, (size_t)slots) + 1;
+    const size_t n_chunks = std::max((M + l_max - 1) / l_max, (size_t)slots) + 1;
     XYZZ* partials = (XYZZ*)ctx->get(WS_PARTIALS, 2 * n_chunks * sizeof(XYZZ));
     u32* big = (u32*)ctx->get(WS_BIGLIST, ((size_t)nb_total + 1) * 4);  // [0] = counter, list follows
-    // batch-affine scratch: sums of levels 1..3 and the prefix products of a level (all indexed by pair)
-    Affine* red[3] = {nullptr, nullptr, nullptr};
-    Fq* red_pref = nullptr;
-    if (R >= 1) {
-        char* a = (char*)ctx->get(WS_RED_A, (Mp / 2 + Mp / 4 + Mp / 8 + 8) * sizeof(Affine));
-        red[0] = (Affine*)a;
-        red[1] = red[0] + Mp / 2;
-        red[2] = red[1] + Mp / 4;
-        red_pref = (Fq*)ctx->get(WS_RED_B, (Mp / 2 + 8) * sizeof(Fq));
-    }
 
     // counting sort by bucket: histogram -> exclusive scan -> scatter (digits are recomputed, not stored)
     H2B_CUDA(cudaMemsetAsync(hist, 0, ((size_t)nb_total + 1) * 4, st));
@@ -681,52 +625,19 @@ void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, i
     H2B_LAUNCH(ctx, k_digits<0>, dgrid, 256, 0, cols, (u32)n, c, W, q, nbw, nsets, table_mask, hist, (u32*)nullptr);
     const u32 ntiles = (nb_total + SCAN_TILE - 1) / SCAN_TILE;
     u32* tile_sums = cursor + nb_total + 2;
-    H2B_LAUNCH(ctx, k_scan_tiles, ntiles, 256, 0, hist, nb_total, off, tile_sums, (u32)(G - 1));
+    H2B_LAUNCH(ctx, k_scan_tiles, ntiles, 256, 0, hist, nb_total, off, tile_sums);
     u32* d_L = tile_sums + ntiles + 1;
-    H2B_LAUNCH(ctx, k_scan_apply, ntiles, 256, 0, nb_total, ntiles, tile_sums, off, cursor, slots, l_min, l_max, d_L, hist, vals, R);
+    H2B_LAUNCH(ctx, k_scan_apply, ntiles, 256, 0, nb_total, ntiles, tile_sums, off, cursor, slots, l_min, l_max, d_L);
     H2B_LAUNCH(ctx, k_digits<1>, dgrid, 256, 0, cols, (u32)n, c, W, q, nbw, nsets, table_mask, cursor, vals);
     if (after_digits) H2B_CUDA(cudaEventRecord(after_digits, st));
 
     H2B_CUDA(cudaMemsetAsync(big, 0, 4, st));
-    if (R == 0) {
-        H2B_LAUNCH(ctx, k_accumulate<false>, ceil_div(n_chunks, 128), 128, 0, vals, off, nb_total, d_L, tab_a, tab_b, buckets, partials, 0);
-    } else {
-        // R halving levels in affine coordinates, one fused launch: every CTA takes its tile through all levels
-        static const int BA_K_ENV = [] {  // nominal level-1 pairs per thread and tile (H2B_BA_K: experiments)
-            const char* e = getenv("H2B_BA_K");
-            const int v = e ? atoi(e) : 32;
-            return (v >= 8 && v <= 128 && v % 4 == 0) ? v : 32;
-        }();
-        const int BA_K = (ctx->opt_affine_k >= 8 && ctx->opt_affine_k <= 128 && ctx->opt_affine_k % 4 == 0) ? ctx->opt_affine_k : BA_K_ENV;
-        static const int BA_CTAS = [] {  // persistent CTAs per SM (register-bound: 4 at 128 registers)
-            const char* e = getenv("H2B_BA_CTAS");
-            const int v = e ? atoi(e) : 4;
-            return (v >= 1 && v <= 8) ? v : 4;
-        }();
-        u32* ba_cursor = d_L + 1;
-        H2B_CUDA(cudaMemsetAsync(ba_cursor, 0, 4, st));
-        static const int BA_PT_ENV = [] {  // H2B_BA_PT=1: per-thread safegcd inversion instead of one inversion per tile
-            const char* e = getenv("H2B_BA_PT");
-            return e ? atoi(e) : 0;
-        }();
-        const bool per_thread = ctx->opt_affine_pt >= 0 ? ctx->opt_affine_pt != 0 : BA_PT_ENV != 0;
-        if (per_thread)
-            H2B_LAUNCH(ctx, k_batch_affine<true>, ctx->sm_count * BA_CTAS, BA_T, 0, vals, tab_a, red[0], red[1], red[2], red_pref,
-                       off + nb_total, ba_cursor, R, BA_K);
-        else
-            H2B_LAUNCH(ctx, k_batch_affine<false>, ctx->sm_count * BA_CTAS, BA_T, 0, vals, tab_a, red[0], red[1], red[2], red_pref,
-                       off + nb_total, ba_cursor, R, BA_K);
-        H2B_LAUNCH(ctx, k_accumulate<true>, ceil_div(n_chunks, 128), 128, 0, (const u32*)nullptr, off, nb_total, d_L, (const Affine*)red[R - 1], (const Affine*)nullptr, buckets, partials, R);
-    }
+    H2B_LAUNCH(ctx, k_accumulate, ceil_div(n_chunks, 128), 128, 0, vals, off, nb_total, d_L, tab_a, tab_b, buckets, partials);
     // From here on the work is a few hundred CTAs of dependent point additions.  Inside a lane (other MSMs of the batch are
     // in flight on the other lanes) it moves to the lane's high-priority stream: the block scheduler hands freed SM slots to
     // it before the queued accumulation waves of the next MSM, so the latency-bound tail overlaps that accumulation instead
     // of waiting for it to drain.  The lane stream waits for the tail (same order for the caller, workspaces stay safe).
-    static const int tail_env = [] {
-        const char* e = getenv("H2B_TAIL_PRIORITY");
-        return e ? atoi(e) : 1;
-    }();
-    const bool tail_hp = ctx->in_lane && (ctx->opt_tail_priority >= 0 ? ctx->opt_tail_priority != 0 : tail_env != 0);
+    const bool tail_hp = ctx->in_lane;
     struct TailScope {  // restores the lane stream and makes it wait for the tail on every exit path
         h2b_ctx* c; cudaStream_t lane; bool on;
         ~TailScope() {
@@ -741,10 +652,10 @@ void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, i
         ctx->stream = ctx->lane_tail[ctx->cur_lane];
         H2B_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->lane_acc[ctx->cur_lane], 0));
     }
-    H2B_LAUNCH(ctx, k_collect, ceil_div(nb_total, 128), 128, 0, off, nb_total, d_L, partials, buckets, big + 1, big, R);
+    H2B_LAUNCH(ctx, k_collect, ceil_div(nb_total, 128), 128, 0, off, nb_total, d_L, partials, buckets, big + 1, big);
     XYZZ* seg = (XYZZ*)ctx->get(WS_POOL, (2 * (n_chunks / BIG_SEG) + 64) * sizeof(XYZZ));
-    H2B_LAUNCH(ctx, k_collect_big1, 2 * ctx->sm_count, 256, 0, off, d_L, partials, big + 1, big, seg, R);
-    H2B_LAUNCH(ctx, k_collect_big2, 64, 256, 0, off, d_L, seg, buckets, big + 1, big, R);
+    H2B_LAUNCH(ctx, k_collect_big1, 2 * ctx->sm_count, 256, 0, off, d_L, partials, big + 1, big, seg);
+    H2B_LAUNCH(ctx, k_collect_big2, 64, 256, 0, off, d_L, seg, buckets, big + 1, big);
 
     // bucket reduction: row/column sums of the 2^mh x 2^ml bucket grid, small scalar multiples, final combine
     const int mm = c - 1, ml = (mm + 1) / 2, mh = mm - ml;
@@ -810,13 +721,8 @@ struct LaneScope {
 // single MSMs overlap one MSM's sort / tail with the next one's accumulation; small domains (k <= 17, the shards of a
 // multi-GPU run) are bound by the latency of the bucket reduction, which a group pays once.
 size_t msm_group_size(const h2b_ctx* ctx, size_t n, size_t m, int W) {
-    if (msm_choose_levels(ctx, 1) > 0) return 1;  // the batch-affine passes are built for one MSM at a time
     if ((size_t)W * n >= ((size_t)1 << 30)) return 1;  // no room for the table bit in a sorted entry: one MSM per pipeline
-    static const int forced = [] {
-        const char* e = getenv("H2B_MSM_GROUP");
-        return e ? atoi(e) : 0;
-    }();
-    size_t g = ctx->opt_msm_group > 0 ? (size_t)ctx->opt_msm_group : (forced > 0 ? (size_t)forced : 0);
+    size_t g = ctx->opt_msm_group > 0 ? (size_t)ctx->opt_msm_group : 0;
     if (g == 0) {
         const int lg = ceil_log2(n);
         g = lg <= 17 ? MSM_MAX_GROUP : (lg <= 19 ? (m + 1) / 2 : (m + 2) / 3);

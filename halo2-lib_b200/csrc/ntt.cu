@@ -353,14 +353,9 @@ void ntt_run(h2b_ctx* ctx, const void* d_src, size_t n_src, void* d_dst, uint32_
     // Tile size: 2^11 elements for large transforms; smaller domains take smaller tiles so that the grid still covers the
     // GPU several times over (2^19: 512 CTAs of 2^10 instead of 256 of 2^11; 2^16: 256 CTAs instead of 32) — the passes are
     // latency-bound there, more resident warps hide the multiplier's dependent chains.
-    static const int tile_env = [] {
-        const char* e = getenv("H2B_NTT_TILE");
-        return e ? atoi(e) : 0;
-    }();
     int r_max = 0;
     for (int t = 0; t < p->npass; t++) r_max = std::max(r_max, p->r[t]);
-    int tile_log = std::min(NTT_TILE_LOG, std::max(r_max, (int)log_n - 10));
-    if (tile_env >= r_max && tile_env <= NTT_TILE_LOG) tile_log = tile_env;
+    const int tile_log = std::min(NTT_TILE_LOG, std::max(r_max, (int)log_n - 10));
     int consumed = 0;
     for (int t = 0; t < p->npass; t++) {
         const bool last = (t == p->npass - 1), first = (t == 0);

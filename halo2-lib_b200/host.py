@@ -73,7 +73,7 @@ class Context:
         self.check(lib.h2b_ctx_synchronize(self.h))
 
     def set_option(self, key: str, value: int):
-        """tuning / experiment switches (h2b_ctx_set_option); results never depend on them"""
+        """tuning switches (h2b_ctx_set_option); results never depend on them"""
         self.check(lib.h2b_ctx_set_option(self.h, key.encode(), int(value)))
 
     @property

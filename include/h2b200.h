@@ -78,13 +78,7 @@ int h2b_ctx_synchronize(h2b_ctx* ctx);
 int h2b_ctx_side_begin(h2b_ctx* ctx);
 int h2b_ctx_side_end(h2b_ctx* ctx);
 int h2b_ctx_side_join(h2b_ctx* ctx);
-/* Tuning / experiment switches (results never depend on them).  Keys:
- *   "msm.affine_levels"  0..3 (-1 = default 0): batch-affine halving levels in front of the XYZZ bucket accumulation
- *   "msm.affine_k"       multiple of 4 in [8, 128] (-1 = default 32): pairs per thread and tile of those levels
- *   "msm.affine_per_thread_inverse"  1: every thread inverts its own denominator product (constant-time safegcd), 0: one
- *                        inversion per tile (product tree + single lane); -1 = default
- *   "msm.tail_priority"  1 (default): the bucket reduction of an MSM that runs on one of the batch lanes is enqueued on a
- *                        high-priority stream, so it overlaps the next MSM's accumulation; 0: everything on the lane stream
+/* Tuning switches (results never depend on them).  Keys:
  *   "ntt.max_ctas_per_sm" 0 (default: as many as fit), 1 or 2: the transforms of this context leave room on every SM — for a
  *                        transform that runs in the background of a latency-bound MSM pipeline (small multi-GPU shards)
  *   "msm.batch_group"    1..16 (0 = default, chosen from the domain size): how many MSMs of one batch call share a single
@@ -440,8 +434,7 @@ int h2b_eval_polynomial_batch_dev(h2b_ctx* ctx, const void* const* d_polys, cons
 /* ---- test hooks (field arithmetic of the kernels, element-wise on the device) --------------------- */
 /* field: 0 = Fq, 1 = Fr; op: 0 mul, 1 add, 2 sub, 3 inv(a), 4 from_mont(a), 5 to_mont(a), 6 sqr(a),
  * 7 a*b + (a+b)(a-b) and 8 a*b - b*b through the fused two-product Montgomery routine of the group law,
- * 9 inv(a) by the binary extended Euclidean routine the single-lane inversions use, 10 inv(a) by the constant-time
- * safegcd routine (every lane inverts its own element) */
+ * 9 inv(a) by the binary extended Euclidean routine the single-lane inversions use */
 int h2b_test_field_op(h2b_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out);
 
 #ifdef __cplusplus

@@ -68,7 +68,7 @@ public:
         if (rc != H2B_OK) throw Error(rc, h2b_last_error(ctx_));
     }
     void set_stream(void* cuda_stream) { check(h2b_ctx_set_stream(ctx_, cuda_stream)); }
-    // tuning switches ("msm.batch_group", "msm.tail_priority", "ntt.max_ctas_per_sm", ...; include/h2b200.h): never change a result
+    // tuning switches ("msm.batch_group", "ntt.max_ctas_per_sm"; include/h2b200.h): never change a result
     void set_option(const char* key, int64_t value) { check(h2b_ctx_set_option(ctx_, key, value)); }
     void synchronize() { check(h2b_ctx_synchronize(ctx_)); }
     G1 sum(const std::vector<G1>& pts) const {  // combine per-GPU partial commitments

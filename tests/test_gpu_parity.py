@@ -27,8 +27,8 @@ def norm(ctx, xyz):
 
 
 # ------------------------------------------------------------------ L0: field arithmetic of the kernels
-@pytest.mark.parametrize("which,m", [(0, P), (1, R)])
-def test_field_ops(ctx, which, m):
+@pytest.mark.parametrize("which,m", [(0, P), (1, R)], ids=["Fq", "Fr"])
+def test_field_ops(ctx, h2b, which, m):
     rng = np.random.default_rng(100 + which)
     edge = [0, 1, 2, m - 1, m - 2, (1 << 64) - 1, 1 << 64, (1 << 128) - 1, 1 << 253, m >> 1, (1 << 32) - 1, 1 << 32]
     a = edge + rand_ints(rng, 4000, m)
@@ -50,7 +50,8 @@ def test_field_ops(ctx, which, m):
     assert np.array_equal(ctx.field_op(which, 5, ints_to_limbs(a)), A)
     assert np.array_equal(ctx.field_op(which, 3, A[:300]), orc.f_inv(which, A[:300]))
     assert np.array_equal(ctx.field_op(which, 9, A[:600]), orc.f_inv(which, A[:600]))  # binary-Euclid inversion (single-lane paths)
-    assert np.array_equal(ctx.field_op(which, 10, A[:3000]), orc.f_inv(which, A[:3000]))  # constant-time safegcd (every lane inverts)
+    with pytest.raises(h2b.H2BError):  # the ops end at 9
+        ctx.field_op(which, 10, A[:3000])
     # products of edge x edge (carry patterns)
     ea = [x for x in edge for _ in edge]
     eb = [y for _ in edge for y in edge]
@@ -269,50 +270,46 @@ def test_msm_group_pipeline(h2b, group):
         c.close()
 
 
-@pytest.mark.parametrize("levels,per_thread", [(1, 0), (2, 0), (3, 0), (2, 1), (3, 1)])
-def test_msm_batch_affine_levels(h2b, levels, per_thread):
-    """the opt-in batch-affine bucket reduction (csrc/batch_affine.cuh): groups of 2^levels sorted entries are summed in
-    affine coordinates with a shared inversion before the XYZZ accumulation.  Same group element, every edge included:
-    identity bases, repeated bases (tangent case), P + (-P) inside a bucket, hot buckets, witness-like columns."""
-    c = h2b.Context(0)
-    c.set_option("msm.affine_levels", levels)
-    c.set_option("msm.affine_k", 8 if levels == 1 else 32)
-    c.set_option("msm.affine_per_thread_inverse", per_thread)  # 1: every thread inverts (constant-time safegcd), no barrier
+@pytest.mark.parametrize("k,case", [(6, "uniform"), (10, "witness"), (13, "uniform"), (13, "zero"), (9, "one-base")])
+def test_msm_table_edge_vectors(ctx, h2b, k, case):
+    """the tabulated-SRS MSM (ParamsKZG.commit) on the inputs that stress the bucket accumulation: identity bases, repeated
+    bases (P + P inside a bucket), P + (-P) cancelling inside a bucket, an all-zero column, and one base repeated 512 times
+    with one repeated scalar (every entry in one bucket)."""
+    n = 1 << k
+    rng = np.random.default_rng(900 + k)
+    if case == "one-base":
+        B = np.repeat(_bases(ctx, 1, a0=2, delta=3), n, axis=0)
+        S = mont([123456789] * n, R)
+    elif case == "zero":
+        B = _bases(ctx, n, a0=2, delta=3)
+        S = np.zeros((n, 4), dtype=np.uint64)
+    else:
+        B = _bases(ctx, n, a0=5 + k, delta=3)
+        B[3] = 0            # identity base (0,0)
+        B[11] = B[10]       # repeated base: equal points meet in one bucket
+        sc = rand_ints(rng, n, R) if case == "uniform" else witness_like_ints(rng, n)
+        sc[10], sc[11] = 777, 777                      # P + P inside a bucket
+        sc[20], sc[21] = 424242, 424242
+        B[21, 4:] = mont([(P - v) % P for v in unmont(B[20, 4:].reshape(1, 4), P)], P)[0]  # B[21] = -B[20]: cancels
+        B[21, :4] = B[20, :4]
+        S = mont(sc, R)
+    params = h2b.ParamsKZG(ctx, k, g=B)
     try:
-        rng = np.random.default_rng(900 + levels)
-        for k, dist in [(6, "uniform"), (10, "witness"), (13, "uniform")]:
-            n = 1 << k
-            B = _bases(c, n, a0=5 + k, delta=3)
-            B[3] = 0            # identity base (0,0)
-            B[11] = B[10]       # repeated base: equal points meet in one bucket
-            sc = rand_ints(rng, n, R) if dist == "uniform" else witness_like_ints(rng, n)
-            sc[10], sc[11] = 777, 777                      # P + P inside a bucket
-            sc[20], sc[21] = 424242, 424242
-            B[21, 4:] = mont([(P - v) % P for v in unmont(B[20, 4:].reshape(1, 4), P)], P)[0]  # B[21] = -B[20]: cancels
-            B[21, :4] = B[20, :4]
-            S = mont(sc, R)
-            params = h2b.ParamsKZG(c, k, g=B)
-            assert np.array_equal(norm(c, params.commit(S)), orc.msm_pippenger(S, B)), (k, dist)
-            params.close()
-        # one value for most of the column: a single bucket of thousands of entries
-        k = 13
-        n = 1 << k
-        B = _bases(c, n, a0=2, delta=3)
-        S = mont([1] * (n - 100) + rand_ints(rng, 100, R), R)
-        params = h2b.ParamsKZG(c, k, g=B)
-        assert np.array_equal(norm(c, params.commit(S)), orc.msm_pippenger(S, B))
-        # all-zero column and a column of one repeated base with one repeated scalar
-        assert jac_limbs_to_affine(norm(c, params.commit(np.zeros((n, 4), dtype=np.uint64)))) is None
+        got = norm(ctx, params.commit(S))
+    finally:
         params.close()
-        Beq = np.repeat(B[:1], 512, axis=0)
-        Seq = mont([123456789] * 512, R)
-        params = h2b.ParamsKZG(c, 9, g=Beq)
-        assert np.array_equal(norm(c, params.commit(Seq)), orc.msm_pippenger(Seq, Beq))
-        params.close()
-        with pytest.raises(h2b.H2BError):
-            c.set_option("msm.affine_levels", 9)
-        with pytest.raises(h2b.H2BError):
-            c.set_option("no.such.option", 1)
+    assert np.array_equal(got, orc.msm_pippenger(S, B)), (k, case)
+    if case == "zero":
+        assert jac_limbs_to_affine(got) is None
+
+
+def test_set_option_rejects_unknown_keys(h2b):
+    """a key that is not one of the switches listed in include/h2b200.h fails with H2BError instead of being ignored"""
+    c = h2b.Context(0)
+    try:
+        for key in ("msm.affine_levels", "msm.affine_k", "msm.affine_per_thread_inverse", "msm.tail_priority", "no.such.option"):
+            with pytest.raises(h2b.H2BError):
+                c.set_option(key, 1)
     finally:
         c.close()
 

@@ -1,5 +1,5 @@
 // latbench.cu — latency/throughput of chained G1 point additions for one warp vs many warps.
-// Build twice: default and -DH2B_MUL_NOINLINE.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --expt-relaxed-constexpr -o tools/latbench tools/latbench.cu ; run on the GPU box.
 #include <cstdio>
 #include "../halo2-lib_b200/csrc/quad.cuh"
 using namespace h2b;
