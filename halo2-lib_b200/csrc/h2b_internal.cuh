@@ -86,6 +86,7 @@ struct h2b_ctx {
     std::string err;
     uint64_t launches = 0;
     bool ntt_attr_set = false;
+    bool sort_attr_set = false;  // MSM sort kernels allowed their larger dynamic shared memory (msm_run_group)
     int opt_ntt_ctas = 0;        // h2b_ctx_set_option("ntt.max_ctas_per_sm"): 0 = as many as fit, 1 or 2 = background transform (see ntt_run)
     int opt_msm_group = 0;       // "msm.batch_group": MSMs of a batch call that share one sort / accumulate / reduce pipeline (0 = by size)
     int opt_lookup_backward = 0; // "lookup.leftover_order": 0 = front to back (PSE / axiom walk), 1 = zcash (pop from the back)
@@ -107,7 +108,7 @@ struct h2b_ctx {
     bool in_lane = false;                                             // the current stream is lane_stream[cur_lane]
     cudaEvent_t lane_done[NLANES] = {nullptr, nullptr, nullptr};
     cudaEvent_t lane_ready[NLANES] = {nullptr, nullptr, nullptr};     // staging buffer filled (host batch API)
-    cudaEvent_t lane_consumed[NLANES] = {nullptr, nullptr, nullptr};  // staging buffer read by k_digits
+    cudaEvent_t lane_consumed[NLANES] = {nullptr, nullptr, nullptr};  // staging buffer read by the MSM sort
     cudaEvent_t fork_ev = nullptr;
     int cur_lane = 0;  // workspace set used by get()
     Buf ws[NLANES][h2b::WS_COUNT];

@@ -6,10 +6,14 @@
 //
 // Pipeline (no host synchronisation; up to 16 MSMs of one size — the columns a prover phase commits — share ONE pipeline,
 // their bucket sets side by side, msm_run_group; the bucket reduction of a lane's group runs on a high-priority stream):
-//   k_digits<0>       scalars (Montgomery) -> canonical -> signed base-2^c digits -> histogram of bucket keys
+//   k_sort_count      scalars (Montgomery) -> canonical -> signed base-2^c digits -> bucket keys (stored) and a shared
+//                     histogram of coarse bins (key >> F) -> one global add per (tile, bin); the last CTA scans the bin
+//                     counts and splits every bin into chunks for the fine passes
+//   k_sort_partition  writes (low F key bits, table index | table bit | sign) into the bins' regions, one global atomic
+//                     per (tile, bin) reserves a tile's run
+//   k_sort_fine<0>    per chunk of a bin: shared histogram of its 2^F buckets -> one global add per (chunk, bucket)
 //   k_scan_tiles/apply exclusive scan: first sorted position of every bucket
-//   k_digits<1>       same recoding, scatters (table index | table bit | sign) to its sorted position (counting
-//                     sort; warp-aggregated atomics so that hot buckets cost one atomic per warp)
+//   k_sort_fine<1>    per chunk: reserves a run per (chunk, bucket), ranks in shared memory, writes the sorted entries
 //   k_accumulate      every thread owns EXACTLY L consecutive sorted entries (perfect balance under any
 //                     scalar distribution, witness columns are dominated by 0/1/88-bit limbs), gathers the
 //                     64-byte affine points with 128-bit loads, XYZZ mixed adds; buckets that end inside
@@ -40,9 +44,9 @@ struct MsmScalars { const uint64_t* p[MSM_MAX_GROUP]; };
 // The MSMs of a group read at most TWO distinct tables (the SRS has two bases); bit 30 of a sorted entry selects one.
 static constexpr u32 TABLE_BIT = 0x40000000u;
 
-// ------------------------------------------------------------------------------------------------ digits + counting sort
-// Signed base-2^c recoding of one canonical scalar; calls f(w, digit_magnitude (1..2^(c-1)), negative) for every
-// non-zero digit.  W*c >= 255 so the last carry is absorbed.
+// ------------------------------------------------------------------------------------------------ digits + bucket sort
+// Signed base-2^c recoding of one canonical scalar; calls f(w, digit_magnitude (0..2^(c-1)), negative) for every
+// window, zero digits included.  W*c >= 255 so the last carry is absorbed.
 template <class F>
 __device__ __forceinline__ void for_each_digit(const Fr& s, int c, int W, F&& f) {
     const u32 half = 1u << (c - 1);
@@ -105,26 +109,242 @@ __device__ __forceinline__ u32 warp_agg_add(u32* counters, u32 key, bool active,
     return atomicAdd(counters + key, 1u);
 }
 
-// MODE 0: histogram of bucket keys.  MODE 1: scatter (table index | sign) to its sorted position via the cursors.
-// One thread per scalar; window w belongs to bucket set w / q and table level w % q.  Zero digits are dropped.
-// blockIdx.y = MSM of the group; its bucket sets start at bucket blockIdx.y * spm * nbw (spm = sets per MSM).
-template <int MODE>
-__global__ void __launch_bounds__(256) k_digits(const __grid_constant__ MsmScalars cols, u32 n, int c, int W, int q, u32 nbw, u32 spm,
-                                                u32 table_mask, u32* __restrict__ counters, u32* __restrict__ vals_sorted) {
+// Two-level sort of the non-zero digits by bucket key.  A one-level counting sort pays a global atomic and a scattered 4-byte
+// store per digit (7.9 M of each per 2^19 MSM).  Here the per-digit counting and ranking happen in shared memory, a global
+// atomic stands for a whole (tile, bin) or (chunk, bucket) run, and every pass stages its entries in shared memory sorted by
+// destination so that the stores go out in contiguous runs.
+//   coarse bins  bin = key >> F, nbins <= SORT_BINS_MAX (F chosen per shape by msm_run_group); fine: the 2^F keys of a bin
+//   k_sort_count      per tile of scalars: recodes, stores every digit's key (coalesced, [msm][window][scalar]) and
+//                     counts the bins in shared memory -> bin_count (one global add per non-empty bin).  The only kernel
+//                     that reads the scalars.  Its last CTA scans bin_count into bin_base and cuts every bin into chunks
+//                     for the fine passes.
+//   k_sort_partition  per tile of keys: reserves a run per (tile, bin) and writes (key & (2^F - 1), entry) pairs into the
+//                     bins' regions of tmp_low / tmp_val
+//   k_sort_fine<0>    per chunk of one bin: shared histogram of the bin's 2^F buckets -> hist (one add per bucket)
+//   k_scan_tiles/apply exclusive scan of hist: off[] (first sorted position of every bucket), cursor[], off[nb], L
+//   k_sort_fine<1>    per chunk: reserves a run per (chunk, bucket) from cursor[] and writes the chunk's entries there
+// Entry order inside a bucket depends on the order of the atomics (as in any counting sort on the GPU); the sum does not.
+static constexpr int SORT_BINS_MAX = 4096;  // coarse bins at most (2^23 buckets with F = 11)
+static constexpr int SORT_F_MAX = 11;       // fine buckets per bin at most 2^11: a chunk still averages 4 entries per bucket
+static constexpr int SORT_PART_TS = 256;    // scalars per CTA of k_sort_partition
+static constexpr u32 SORT_CHUNK = 8192;     // entries per CTA of the fine passes
+static constexpr int SORT_FINE_U = 4;       // entries per thread and step of the fine passes (loads in flight)
+static constexpr int SORT_PART_SMEM_MAX = 2 * SORT_BINS_MAX * 4 + 43 * SORT_PART_TS * 12;  // W <= 43 (ad-hoc c = 6)
+static constexpr int SORT_FINE_SMEM = (2 << SORT_F_MAX) * 4 + SORT_CHUNK * 6;
+
+// Exclusive scan of a[0, len) in shared memory by the whole block (blockDim.x a multiple of 32).  `a` must be complete
+// (a __syncthreads() before the call); returns the total after a final __syncthreads().
+__device__ u32 block_exclusive_scan(u32* a, u32 len, u32* wsum /* [32] */) {
+    const u32 t = threadIdx.x, nt = blockDim.x, per = (len + nt - 1) / nt;
+    const u32 b0 = min(t * per, len), b1 = min(b0 + per, len);
+    u32 sum = 0;
+    for (u32 j = b0; j < b1; j++) sum += a[j];
+    u32 inc = sum;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const u32 o = __shfl_up_sync(0xffffffffu, inc, d);
+        if ((t & 31) >= (u32)d) inc += o;
+    }
+    if ((t & 31) == 31) wsum[t >> 5] = inc;
+    __syncthreads();
+    u32 run = inc - sum, total = 0;
+    for (u32 w = 0; w < nt / 32; w++) {
+        if (w < (t >> 5)) run += wsum[w];
+        total += wsum[w];
+    }
+    for (u32 j = b0; j < b1; j++) {
+        const u32 v = a[j];
+        a[j] = run;
+        run += v;
+    }
+    __syncthreads();
+    return total;
+}
+
+// Window w belongs to bucket set w / q and table level w % q.  Zero digits are dropped.  blockIdx.y = MSM of the group; its
+// bucket sets start at bucket blockIdx.y * spm * nbw (spm = sets per MSM).  q is W (tabulated bases) or 1 (ad-hoc bases):
+// both are answered without an integer division.
+__device__ __forceinline__ u32 window_set(int w, int q) { return q == 1 ? (u32)w : (w < q ? 0u : (u32)(w / q)); }
+__device__ __forceinline__ u32 window_level(int w, int q) { return q == 1 ? 0u : (w < q ? (u32)w : (u32)(w % q)); }
+__device__ __forceinline__ u32 digit_key(u32 msm, int w, int q, u32 nbw, u32 spm, u32 d) {
+    return msm * spm * nbw + window_set(w, q) * nbw + (d - 1);
+}
+static constexpr u32 NO_DIGIT = ~0u;  // k_sort_count's key of a zero digit
+
+// One scalar per thread.  The last CTA to finish turns the bin counts into bin_base[b] = first position of bin b
+// (bin_base[nbins] = entry count), bin_cursor = bin_base (consumed by k_sort_partition) and chunk_pre[b] = first fine-pass
+// chunk of bin b (chunk_pre[nbins] = chunk count).  `done` is zero at the launch.
+__global__ void __launch_bounds__(256) k_sort_count(const __grid_constant__ MsmScalars cols, u32 n, int c, int W, int q, u32 nbw,
+                                                    u32 spm, int F, u32 nbins, u32* __restrict__ bin_count,
+                                                    u32* __restrict__ keys, u32* __restrict__ done, u32* __restrict__ bin_base,
+                                                    u32* __restrict__ bin_cursor, u32* __restrict__ chunk_pre) {
+    __shared__ u32 h[SORT_BINS_MAX], nch[SORT_BINS_MAX];
+    __shared__ u32 wsum[32];
+    __shared__ bool is_last;
+    for (u32 b = threadIdx.x; b < nbins; b += blockDim.x) h[b] = 0;
+    __syncthreads();
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool live = i < n;
-    const uint64_t* __restrict__ scalars = cols.p[blockIdx.y];
-    const u32 key0 = blockIdx.y * spm * nbw;
-    const u32 tbit = ((table_mask >> blockIdx.y) & 1u) ? TABLE_BIT : 0u;
     Fr s = Fr::zero();
-    if (live) s = Fr::load_nc(scalars + 4 * (size_t)i).from_mont();  // canonical integer, as `to_repr()` gives
+    if (live) s = Fr::load_nc(cols.p[blockIdx.y] + 4 * (size_t)i).from_mont();  // canonical integer, as `to_repr()` gives
     for_each_digit(s, c, W, [&](int w, u32 d, bool neg) {
         const bool active = live && d != 0;
-        const u32 key = active ? key0 + (u32)(w / q) * nbw + (d - 1) : 0;
+        const u32 key = active ? digit_key(blockIdx.y, w, q, nbw, spm, d) : 0;
         // tiny digits and the (narrow) top window are where hot buckets come from: group them before the atomic
-        const u32 slot = warp_agg_add(counters, key, active, d <= 4 || w == W - 1);
-        if (MODE == 1 && active) vals_sorted[slot] = ((u32)(w % q) * n + i) | tbit | (neg ? SIGN_BIT : 0u);
+        warp_agg_add(h, key >> F, active, d <= 4 || w == W - 1);
+        if (live) keys[((size_t)blockIdx.y * W + w) * n + i] = active ? key | (neg ? SIGN_BIT : 0u) : NO_DIGIT;
     });
+    __syncthreads();
+    for (u32 b = threadIdx.x; b < nbins; b += blockDim.x)
+        if (h[b]) atomicAdd(bin_count + b, h[b]);
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) is_last = atomicAdd(done, 1u) == gridDim.x * gridDim.y - 1;
+    __syncthreads();
+    if (!is_last) return;
+    __threadfence();
+    for (u32 b = threadIdx.x; b < nbins; b += blockDim.x) {
+        h[b] = __ldcg(bin_count + b);
+        nch[b] = (h[b] + SORT_CHUNK - 1) / SORT_CHUNK;
+    }
+    __syncthreads();
+    const u32 total = block_exclusive_scan(h, nbins, wsum);
+    const u32 chunks = block_exclusive_scan(nch, nbins, wsum);
+    for (u32 b = threadIdx.x; b < nbins; b += blockDim.x) {
+        bin_base[b] = h[b];
+        bin_cursor[b] = h[b];
+        chunk_pre[b] = nch[b];
+    }
+    if (threadIdx.x == 0) {
+        bin_base[nbins] = total;
+        chunk_pre[nbins] = chunks;
+    }
+}
+
+// Tile = SORT_PART_TS scalars, one per thread.  The keys k_sort_count recorded wait in shared memory (with their rank inside
+// the tile's run of the bin) until one global atomic per non-empty bin has reserved the tile's runs; then they are put in bin
+// order in shared memory and stored in contiguous runs.
+__global__ void __launch_bounds__(SORT_PART_TS) k_sort_partition(const u32* __restrict__ keys, u32 n, int W, int q, u32 nbw,
+                                                                 u32 table_mask, int F, u32 nbins, u32* __restrict__ bin_cursor,
+                                                                 uint16_t* __restrict__ tmp_low, u32* __restrict__ tmp_val) {
+    extern __shared__ u32 sdyn[];
+    __shared__ u32 wsum[32];
+    const u32 ts = SORT_PART_TS, t = threadIdx.x, ne = (u32)W * ts;
+    u32* h = sdyn;                                 // [nbins] count, then first position of the bin in the tile's order
+    u32* dlt = h + nbins;                          // [nbins] global position - tile position
+    u32* skey = dlt + nbins;                       // [W][ts] key | sign, NO_DIGIT for a zero digit
+    u32* okey = skey + ne;                         // [ne] key | sign in bin order
+    uint16_t* srank = (uint16_t*)(okey + ne);      // [W][ts] rank inside the tile's run of the bin
+    uint16_t* osrc = srank + ne;                   // [ne] w << 8 | thread, in bin order
+    for (u32 b = t; b < nbins; b += ts) h[b] = 0;
+    __syncthreads();
+    const u32 i = blockIdx.x * ts + t;
+    const bool live = i < n;
+    const u32* __restrict__ mk = keys + (size_t)blockIdx.y * W * n + i;
+#pragma unroll 4
+    for (int w = 0; w < W; w++) skey[w * ts + t] = live ? mk[(size_t)w * n] : NO_DIGIT;  // independent loads first
+    for (int w = 0; w < W; w++) {
+        const u32 k = skey[w * ts + t], key = k & ~SIGN_BIT;
+        // digit - 1 is the key's offset in its bucket set: the same grouping of hot buckets as in k_sort_count
+        const u32 r = warp_agg_add(h, key >> F, k != NO_DIGIT, (key & (nbw - 1)) < 4 || w == W - 1);
+        srank[w * ts + t] = (uint16_t)r;
+    }
+    __syncthreads();
+    for (u32 b = t; b < nbins; b += ts) dlt[b] = h[b] ? atomicAdd(bin_cursor + b, h[b]) : 0u;
+    const u32 total = block_exclusive_scan(h, nbins, wsum);
+    for (u32 b = t; b < nbins; b += ts) dlt[b] -= h[b];
+    for (int w = 0; w < W; w++) {
+        const u32 k = skey[w * ts + t];
+        if (k == NO_DIGIT) continue;
+        const u32 p = h[(k & ~SIGN_BIT) >> F] + srank[w * ts + t];
+        okey[p] = k;
+        osrc[p] = (uint16_t)((w << 8) | t);
+    }
+    __syncthreads();
+    const u32 tbit = ((table_mask >> blockIdx.y) & 1u) ? TABLE_BIT : 0u;
+    const u32 fmask = (1u << F) - 1u;
+    for (u32 j = t; j < total; j += ts) {
+        const u32 k = okey[j], key = k & ~SIGN_BIT, src = osrc[j];
+        const u32 pos = dlt[key >> F] + j;
+        tmp_low[pos] = (uint16_t)(key & fmask);
+        tmp_val[pos] = (window_level(src >> 8, q) * n + blockIdx.x * ts + (src & 255u)) | tbit | (k & SIGN_BIT);
+    }
+}
+
+// The fine passes run one CTA per chunk of SORT_CHUNK entries of one bin (chunks never straddle bins).  False: no such chunk.
+__device__ __forceinline__ bool sort_chunk(const u32* __restrict__ chunk_pre, const u32* __restrict__ bin_base, u32 nbins,
+                                           u32& bin, u32& s, u32& e) {
+    const u32 g = blockIdx.x;
+    if (g >= chunk_pre[nbins]) return false;
+    u32 lo = 0, hi = nbins;  // chunk_pre[lo] <= g < chunk_pre[hi]
+    while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (chunk_pre[mid] <= g) lo = mid; else hi = mid;
+    }
+    bin = lo;
+    s = bin_base[lo] + (g - chunk_pre[lo]) * SORT_CHUNK;
+    e = min(s + SORT_CHUNK, bin_base[lo + 1]);
+    return true;
+}
+
+// MODE 0: hist[bin * 2^F + low] += the chunk's count of that bucket.
+// MODE 1: reserves the chunk's run of every bucket from cursor[], puts the chunk in bucket order in shared memory and stores
+// it to vals in contiguous runs.
+template <int MODE>
+__global__ void __launch_bounds__(512) k_sort_fine(const u32* __restrict__ chunk_pre, const u32* __restrict__ bin_base, u32 nbins,
+                                                   int F, const uint16_t* __restrict__ tmp_low, const u32* __restrict__ tmp_val,
+                                                   u32* __restrict__ counters, u32* __restrict__ vals) {
+    extern __shared__ u32 h[];  // [2^F] count, then (MODE 1) running position in the chunk's bucket order
+    __shared__ u32 wsum[32];
+    u32 bin, s, e;
+    if (!sort_chunk(chunk_pre, bin_base, nbins, bin, s, e)) return;
+    const u32 nf = 1u << F, t = threadIdx.x;
+    for (u32 j = t; j < nf; j += blockDim.x) h[j] = 0;
+    __syncthreads();
+    // all 32 lanes of a warp call warp_agg_add: the loop bound is uniform.  A hot bucket fills whole warps.  SORT_FINE_U
+    // independent loads are issued before their atomics.
+    const u32 bd = blockDim.x;
+    for (u32 i0 = s; i0 < e; i0 += SORT_FINE_U * bd) {
+        u32 lw[SORT_FINE_U];
+#pragma unroll
+        for (int u = 0; u < SORT_FINE_U; u++) lw[u] = i0 + u * bd + t < e ? tmp_low[i0 + u * bd + t] : 0u;
+#pragma unroll
+        for (int u = 0; u < SORT_FINE_U; u++) warp_agg_add(h, lw[u], i0 + u * bd + t < e, false);
+    }
+    __syncthreads();
+    u32* ctr = counters + ((size_t)bin << F);
+    if (MODE == 0) {
+        for (u32 j = t; j < nf; j += blockDim.x)
+            if (h[j]) atomicAdd(ctr + j, h[j]);
+        return;
+    }
+    u32* dlt = h + nf;                              // [2^F] global position - chunk position
+    u32* oval = dlt + nf;                           // [chunk] entries in bucket order
+    uint16_t* olow = (uint16_t*)(oval + SORT_CHUNK);  // [chunk] their buckets
+    for (u32 j = t; j < nf; j += blockDim.x) dlt[j] = h[j] ? atomicAdd(ctr + j, h[j]) : 0u;
+    block_exclusive_scan(h, nf, wsum);
+    for (u32 j = t; j < nf; j += blockDim.x) dlt[j] -= h[j];
+    __syncthreads();  // h becomes the running position below
+    for (u32 i0 = s; i0 < e; i0 += SORT_FINE_U * bd) {
+        u32 lw[SORT_FINE_U], vw[SORT_FINE_U];
+#pragma unroll
+        for (int u = 0; u < SORT_FINE_U; u++) {
+            const u32 i = i0 + u * bd + t;
+            lw[u] = i < e ? tmp_low[i] : 0u;
+            vw[u] = i < e ? tmp_val[i] : 0u;
+        }
+#pragma unroll
+        for (int u = 0; u < SORT_FINE_U; u++) {
+            const bool active = i0 + u * bd + t < e;
+            const u32 p = warp_agg_add(h, lw[u], active, false);
+            if (active) {
+                oval[p] = vw[u];
+                olow[p] = (uint16_t)lw[u];
+            }
+        }
+    }
+    __syncthreads();
+    for (u32 j = t; j < e - s; j += blockDim.x) vals[dlt[olow[j]] + j] = oval[j];
 }
 
 // Exclusive scan of the histogram in two launches.  Tile = 2048 counters per CTA.
@@ -606,10 +826,36 @@ void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, i
     }
     H2B_REQUIRE(table_mask == 0 || (size_t)W * n < ((size_t)1 << 30), "msm: two-table groups need n * windows < 2^30");
 
-    u32* vals = (u32*)ctx->get(WS_VALS_A, M * 4 + 16);
-    u32* cnt = (u32*)ctx->get(WS_KEYS_A, (2 * ((size_t)nb_total + 2) + nb_total / SCAN_TILE + 8) * 4);  // histogram, cursors, tile sums, L
-    u32* hist = cnt;
-    u32* cursor = cnt + nb_total + 2;
+    // coarse bins of the sort: key >> F.  About 256 bins: a partition tile (256 scalars x W digits) then writes runs of ~15
+    // entries per bin, and a bin's 2^F buckets are counted in shared memory by the fine passes.
+    int F = 0;
+    while (F < SORT_F_MAX && (((size_t)nb_total + (1u << F) - 1) >> F) > 256) F++;
+    const u32 nbins = (u32)(((size_t)nb_total + (1u << F) - 1) >> F);
+    H2B_REQUIRE(nbins <= (u32)SORT_BINS_MAX, "msm: too many buckets for the sort");
+    const size_t part_smem = 2 * (size_t)nbins * 4 + (size_t)W * SORT_PART_TS * 12;
+    H2B_REQUIRE(part_smem <= (size_t)SORT_PART_SMEM_MAX, "msm: too many windows for the sort");
+    if (!ctx->sort_attr_set) {  // per context: the attribute belongs to the device the context is bound to
+        H2B_CUDA(cudaFuncSetAttribute(k_sort_partition, cudaFuncAttributeMaxDynamicSharedMemorySize, SORT_PART_SMEM_MAX));
+        H2B_CUDA(cudaFuncSetAttribute(k_sort_fine<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SORT_FINE_SMEM));
+        ctx->sort_attr_set = true;
+    }
+
+    u32* vals = (u32*)ctx->get(WS_VALS_A, M * 4 + 16);  // W * n * m: room for every digit, zero or not
+    // the partitioned entries: low key bits and sorted-entry value, 6 bytes per non-zero digit
+    uint16_t* tmp_low = (uint16_t*)ctx->get(WS_KEYS_B, M * 2 + 16);
+    u32* tmp_val = (u32*)ctx->get(WS_VALS_B, M * 4 + 16);
+    const u32 ntiles = (nb_total + SCAN_TILE - 1) / SCAN_TILE;
+    // bin counts and bucket histogram (zeroed together; hist[nb_total] counts the finished CTAs of k_sort_count), cursors,
+    // scan tile sums, L, bin bases, bin cursors, chunk prefix
+    u32* cnt = (u32*)ctx->get(WS_KEYS_A, (2 * ((size_t)nb_total + 2) + ntiles + 4 * (size_t)nbins + 8) * 4);
+    u32* bin_count = cnt;
+    u32* hist = bin_count + nbins;
+    u32* cursor = hist + nb_total + 2;
+    u32* tile_sums = cursor + nb_total + 2;
+    u32* d_L = tile_sums + ntiles + 1;
+    u32* bin_base = d_L + 1;
+    u32* bin_cursor = bin_base + nbins + 1;
+    u32* chunk_pre = bin_cursor + nbins;
     u32* off = (u32*)ctx->get(WS_OFFSETS, ((size_t)nb_total + 2) * 4);
     XYZZ* buckets = (XYZZ*)ctx->get(WS_BUCKETS, (size_t)nb_total * sizeof(XYZZ));
     const u32 l_min = 12u, l_max = (u32)ACC_L_DEFAULT;  // chunk length of k_accumulate, chosen on the device in [12, 32]
@@ -619,17 +865,22 @@ void msm_run_group(h2b_ctx* ctx, const void* const* d_tables, size_t n, int c, i
     XYZZ* partials = (XYZZ*)ctx->get(WS_PARTIALS, 2 * n_chunks * sizeof(XYZZ));
     u32* big = (u32*)ctx->get(WS_BIGLIST, ((size_t)nb_total + 1) * 4);  // [0] = counter, list follows
 
-    // counting sort by bucket: histogram -> exclusive scan -> scatter (digits are recomputed, not stored)
-    H2B_CUDA(cudaMemsetAsync(hist, 0, ((size_t)nb_total + 1) * 4, st));
-    const dim3 dgrid(ceil_div(n, 256), (unsigned)m);
-    H2B_LAUNCH(ctx, k_digits<0>, dgrid, 256, 0, cols, (u32)n, c, W, q, nbw, nsets, table_mask, hist, (u32*)nullptr);
-    const u32 ntiles = (nb_total + SCAN_TILE - 1) / SCAN_TILE;
-    u32* tile_sums = cursor + nb_total + 2;
+    // two-level sort by bucket (see k_sort_count): digits are recomputed from the scalars, not stored
+    H2B_CUDA(cudaMemsetAsync(cnt, 0, ((size_t)nbins + nb_total + 1) * 4, st));
+    // the keys of all digits ([msm][window][scalar], NO_DIGIT for a zero digit) live in `vals` until k_sort_fine<1> overwrites it
+    u32* keys = vals;
+    H2B_LAUNCH(ctx, k_sort_count, dim3(ceil_div(n, 256), (unsigned)m), 256, 0, cols, (u32)n, c, W, q, nbw, nsets, F, nbins,
+               bin_count, keys, hist + nb_total, bin_base, bin_cursor, chunk_pre);
+    if (after_digits) H2B_CUDA(cudaEventRecord(after_digits, st));  // the scalars are not read after this point
+    H2B_LAUNCH(ctx, k_sort_partition, dim3(ceil_div(n, SORT_PART_TS), (unsigned)m), SORT_PART_TS, part_smem, keys, (u32)n, W, q,
+               nbw, table_mask, F, nbins, bin_cursor, tmp_low, tmp_val);
+    const unsigned fine_grid = ceil_div(M, SORT_CHUNK) + nbins;  // chunks of all bins together: at most this many
+    H2B_LAUNCH(ctx, k_sort_fine<0>, fine_grid, 512, (size_t)4 << F, chunk_pre, bin_base, nbins, F, tmp_low, tmp_val, hist,
+               (u32*)nullptr);
     H2B_LAUNCH(ctx, k_scan_tiles, ntiles, 256, 0, hist, nb_total, off, tile_sums);
-    u32* d_L = tile_sums + ntiles + 1;
     H2B_LAUNCH(ctx, k_scan_apply, ntiles, 256, 0, nb_total, ntiles, tile_sums, off, cursor, slots, l_min, l_max, d_L);
-    H2B_LAUNCH(ctx, k_digits<1>, dgrid, 256, 0, cols, (u32)n, c, W, q, nbw, nsets, table_mask, cursor, vals);
-    if (after_digits) H2B_CUDA(cudaEventRecord(after_digits, st));
+    H2B_LAUNCH(ctx, k_sort_fine<1>, fine_grid, 512, ((size_t)8 << F) + SORT_CHUNK * 6, chunk_pre, bin_base, nbins, F, tmp_low,
+               tmp_val, cursor, vals);
 
     H2B_CUDA(cudaMemsetAsync(big, 0, 4, st));
     H2B_LAUNCH(ctx, k_accumulate, ceil_div(n_chunks, 128), 128, 0, vals, off, nb_total, d_L, tab_a, tab_b, buckets, partials);

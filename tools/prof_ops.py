@@ -25,7 +25,7 @@ params = h.ParamsKZG(ctx, k, g=d_pts.data_ptr(), device_ptrs=True)
 cols = {"uniform": torch.from_numpy(bench.uniform_residues(rng, n).view(np.int64)).to(dev),
         "witness": torch.from_numpy(ctx.field_op(1, 5, bench.witness_like(rng, n)).view(np.int64)).to(dev)}
 out = torch.zeros(12, dtype=torch.int64, device=dev)
-KERNELS = ["k_digits<0>", "k_scan", "k_digits<1>", "k_accumulate", "k_collect_big", "k_collect<", "k_rowcol_sums", "k_weighted_final", "k_ntt_pass"]
+KERNELS = ["k_sort_count", "k_sort_partition", "k_sort_fine<0>", "k_scan", "k_sort_fine<1>", "k_accumulate", "k_collect_big", "k_collect<", "k_rowcol_sums", "k_weighted_final", "k_ntt_pass"]
 
 def run(label, fn, reps=5):
     fn(); torch.cuda.synchronize()
@@ -38,7 +38,7 @@ def run(label, fn, reps=5):
     tot = a.elapsed_time(b) / reps
     print(f"== {label}: {tot*1e3:.1f} us per op (with event overhead)")
     acc = 0
-    for kn in ["k_digits<0>", "k_scan", "k_digits<1>", "k_accumulate", "k_collect_big", "k_collect", "k_rowcol_sums", "k_rowcol_weights", "k_weighted_final", "k_ntt_pass"]:
+    for kn in ["k_sort_count", "k_sort_partition", "k_sort_fine<0>", "k_scan", "k_sort_fine<1>", "k_accumulate", "k_collect_big", "k_collect", "k_rowcol_sums", "k_rowcol_weights", "k_weighted_final", "k_ntt_pass"]:
         ms, cnt = ctx.profile_read(kn)
         if kn == "k_collect":
             ms2, cnt2 = ctx.profile_read("k_collect_big"); ms -= ms2; cnt -= cnt2
