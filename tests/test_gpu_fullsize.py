@@ -1,6 +1,7 @@
 """GPU parity at BASELINE.json's full sizes (k = 19, 20, 23; extended domains up to 2^25) through size-independent
-properties — the oracle cannot finish these sizes in seconds, so the checks are closed forms, linearity, round
-trips and agreement between independent device paths (fixed-base table vs ad-hoc windows).  All comparisons are exact."""
+properties: closed forms, linearity, round trips and agreement between independent device paths (fixed-base table vs
+ad-hoc windows).  All comparisons are exact.  Element-by-element parity with the oracle at these sizes is in
+test_gpu_large_sizes.py."""
 import ctypes as C
 import numpy as np
 import pytest
