@@ -15,6 +15,8 @@ from .host import (  # noqa: F401
     assign_witnesses,
     assign_witnesses_assigned,
     assign_lookups,
+    apply_rational_dev,
+    assign_lookups_indexed_dev,
     omega,
 )
 from .evaluation import (  # noqa: F401,E402

@@ -98,6 +98,8 @@ SIGNATURES = {
     "h2b_assign_lookups_dev": (_int, [_vp, _vp, _sz, _u32, _sz, _vp]),
     "h2b_eval_rational": (_int, [_vp, _vp, _vp, _sz, _vp]),
     "h2b_eval_rational_dev": (_int, [_vp, _vp, _vp, _sz, _vp]),
+    "h2b_apply_rational_dev": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "h2b_assign_lookups_indexed_dev": (_int, [_vp, _vp, _sz, _vp, _sz, _u32, _sz, _vp, _vp]),
     "h2b_batch_invert_fr": (_int, [_vp, _vp, _sz]),
     "h2b_batch_invert_fr_dev": (_int, [_vp, _vp, _sz]),
     "h2b_grand_product_fr": (_int, [_vp, _vp, _vp, _sz, _vp]),

@@ -99,6 +99,47 @@ __global__ void __launch_bounds__(256) k_assign_lookups(const uint4* __restrict_
     cols[g] = v;
 }
 
+// halo2-base form of the witness: lookup cell j = values[index[j]] (the copy LookupAnyManager::assign_raw makes), laid out
+// as k_assign_lookups lays out the values.  An index >= N yields zero and sets bit 0 of *status.
+__global__ void __launch_bounds__(256) k_assign_lookups_indexed(const uint4* __restrict__ vals, size_t N, const uint64_t* __restrict__ index,
+                                                                size_t n_lookup, u32 rows_log, u32 L, uint4* __restrict__ cols,
+                                                                u32* __restrict__ status) {
+    size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    size_t total = ((size_t)L << rows_log) * 2;
+    if (g >= total) return;
+    size_t cell = g >> 1;
+    u32 half = (u32)(g & 1);
+    u32 c = (u32)(cell >> rows_log);
+    size_t r = cell & (((size_t)1 << rows_log) - 1);
+    size_t j = r * L + c;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (j < n_lookup) {
+        const uint64_t idx = __ldg(index + j);
+        if (idx < N)
+            v = __ldg(vals + 2 * idx + half);
+        else if (half == 0)
+            atomicOr(status, 1u);
+    }
+    cols[g] = v;
+}
+
+// Assigned::Rational(n, d) cells of the halo2-base form: values[index[i]] holds n, den_inv[i] = d^-1 (0 for d = 0).  Each
+// thread checks its own entry: index[i] < N (else bit 0 of *status) and index[i] > index[i-1] (else bit 1).  A valid entry
+// is the only writer of its cell, because the valid indices strictly increase.
+__global__ void __launch_bounds__(256) k_apply_rational(uint64_t* __restrict__ values, size_t N, const uint64_t* __restrict__ index,
+                                                        const uint64_t* __restrict__ den_inv, size_t R, u32* __restrict__ status) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= R) return;
+    const uint64_t idx = __ldg(index + i);
+    u32 bad = idx < N ? 0u : 1u;
+    if (i > 0 && idx <= __ldg(index + i - 1)) bad |= 2u;
+    if (bad) {
+        atomicOr(status, bad);
+        return;
+    }
+    (Fr::load(values + 4 * idx) * Fr::load_nc(den_inv + 4 * i)).store(values + 4 * idx);
+}
+
 // Assigned::Rational(num, den) -> num * den^-1 (den = 0 -> 0), what batch_invert_assigned produces
 __global__ void __launch_bounds__(128) k_eval_rational(const uint64_t* __restrict__ num, const uint64_t* __restrict__ den,
                                                        u32 n, uint64_t* __restrict__ out) {
@@ -182,6 +223,29 @@ void assign_lookups_run(h2b_ctx* ctx, const void* d_vals, size_t N, uint32_t k, 
     if ((N + L - 1) / L > rows) throw StatusError{H2B_ERR_LAYOUT, "assign_lookups: range lookups would be assigned to unusable rows (builder.rs:368-372)"};
     size_t total = L * rows * 2;
     H2B_LAUNCH(ctx, k_assign_lookups, ceil_div(total, 256), 256, 0, (const uint4*)d_vals, N, k, (u32)L, (uint4*)d_cols);
+}
+
+void assign_lookups_indexed_run(h2b_ctx* ctx, const void* d_vals, size_t N, const uint64_t* d_index, size_t n_lookup, uint32_t k, size_t L,
+                                void* d_cols, uint32_t* d_status) {
+    H2B_REQUIRE(k <= 28, "assign: k out of range");
+    const size_t rows = (size_t)1 << k;
+    if (L == 0 && n_lookup != 0)
+        throw StatusError{H2B_ERR_LAYOUT, "assign_lookups: values present but no lookup advice columns (builder.rs:366)"};
+    if (L && (n_lookup + L - 1) / L > rows)
+        throw StatusError{H2B_ERR_LAYOUT, "assign_lookups: range lookups would be assigned to unusable rows (builder.rs:368-372)"};
+    H2B_CUDA(cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+    if (L == 0) return;
+    size_t total = L * rows * 2;
+    H2B_LAUNCH(ctx, k_assign_lookups_indexed, ceil_div(total, 256), 256, 0, (const uint4*)d_vals, N, d_index, n_lookup, k, (u32)L,
+               (uint4*)d_cols, d_status);
+}
+
+// d_den is inverted in place (batch_invert_run: zeros stay zero), then multiplied into the cells it belongs to
+void apply_rational_run(h2b_ctx* ctx, void* d_values, size_t N, const uint64_t* d_index, void* d_den, size_t R, uint32_t* d_status) {
+    H2B_CUDA(cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+    if (R == 0) return;
+    batch_invert_run(ctx, d_den, R);
+    H2B_LAUNCH(ctx, k_apply_rational, ceil_div(R, 256), 256, 0, (uint64_t*)d_values, N, d_index, (const uint64_t*)d_den, R, d_status);
 }
 
 void eval_rational_run(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out) {

@@ -988,6 +988,19 @@ int h2b_eval_rational_dev(h2b_ctx* ctx, const void* d_num, const void* d_den, si
         eval_rational_batched_run(ctx, d_num, d_den, n, d_out);
     });
 }
+int h2b_apply_rational_dev(h2b_ctx* ctx, void* d_values, size_t N, const void* d_index, void* d_den, size_t R, uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_status && (d_values || N == 0) && ((d_index && d_den) || R == 0), "apply_rational: null pointer");
+        apply_rational_run(ctx, d_values, N, (const uint64_t*)d_index, d_den, R, d_status);
+    });
+}
+int h2b_assign_lookups_indexed_dev(h2b_ctx* ctx, const void* d_values, size_t N, const void* d_index, size_t n_lookup, uint32_t k, size_t L,
+                                   void* d_cols, uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_status && (d_values || N == 0) && (d_index || n_lookup == 0) && (d_cols || L == 0), "assign_lookups_indexed: null pointer");
+        assign_lookups_indexed_run(ctx, d_values, N, (const uint64_t*)d_index, n_lookup, k, L, d_cols, d_status);
+    });
+}
 int h2b_eval_rational(h2b_ctx* ctx, const uint64_t* num, const uint64_t* den, size_t n, uint64_t* out) {
     return guarded(ctx, [&] {
         H2B_REQUIRE((num && den && out) || n == 0, "eval_rational: null pointer");

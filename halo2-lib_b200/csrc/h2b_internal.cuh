@@ -197,6 +197,10 @@ void assign_columns_run(h2b_ctx* ctx, const void* d_vcol, size_t N, const uint64
 void assigned_flatten_run(h2b_ctx* ctx, const void* d_recs, size_t N, void* d_values, uint32_t* d_stats, int invert);
 void assign_lookups_run(h2b_ctx* ctx, const void* d_vals, size_t N, uint32_t k, size_t L, void* d_cols);
 void eval_rational_run(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out);
+// halo2-base form of the witness (asynchronous; violations land in *d_status, which both zero first)
+void apply_rational_run(h2b_ctx* ctx, void* d_values, size_t N, const uint64_t* d_index, void* d_den, size_t R, uint32_t* d_status);
+void assign_lookups_indexed_run(h2b_ctx* ctx, const void* d_vals, size_t N, const uint64_t* d_index, size_t n_lookup, uint32_t k, size_t L,
+                                void* d_cols, uint32_t* d_status);
 // ---- peer.cu
 void peer_create(h2b_ctx* ctx, int rank, int nranks, uint8_t* handle_out);
 void peer_connect(h2b_ctx* ctx, const uint8_t* handles);

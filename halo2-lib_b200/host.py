@@ -338,6 +338,21 @@ def assign_witnesses_assigned(ctx: Context, cells, break_points, k: int, ncols: 
     return cols
 
 
+def apply_rational_dev(ctx: Context, d_values: int, N: int, d_index: int, d_den: int, R: int, d_status: int):
+    """halo2-base form, device pointers, asynchronous: values[index[i]] *= den[i]^-1 (d = 0 -> 0), den inverted in place;
+    the verdict word at d_status (u32) gets bit 0 for an index >= N, bit 1 for indices that do not strictly increase"""
+    vp = C.c_void_p
+    ctx.check(lib.h2b_apply_rational_dev(ctx.h, vp(d_values), N, vp(d_index), vp(d_den), R, vp(d_status)))
+
+
+def assign_lookups_indexed_dev(ctx: Context, d_values: int, N: int, d_index: int, n_lookup: int, k: int, L: int, d_cols: int,
+                               d_status: int):
+    """`assign_raw` from virtual-column indices, device pointers, asynchronous: lookup cell j = values[index[j]] goes to
+    column j mod L, row j div L of d_cols (L x 2^k cells); bit 0 of the verdict word at d_status for an index >= N"""
+    vp = C.c_void_p
+    ctx.check(lib.h2b_assign_lookups_indexed_dev(ctx.h, vp(d_values), N, vp(d_index), n_lookup, k, L, vp(d_cols), vp(d_status)))
+
+
 def assign_lookups(ctx: Context, values, k: int, L: int) -> np.ndarray:
     v = _u64(values, 4)
     cols = np.empty((L, 1 << k, 4), dtype=np.uint64)

@@ -22,7 +22,7 @@ from __future__ import annotations
 import ctypes as C
 import hashlib
 import numpy as np
-from ._capi import lib, BASIS_MONOMIAL, BASIS_LAGRANGE
+from ._capi import lib, BASIS_MONOMIAL, BASIS_LAGRANGE, H2B_ERR_ARG
 from .host import Context, ParamsKZG, H2BError
 from . import evaluation as ev
 
@@ -352,8 +352,11 @@ class ProverSession:
         self.h = P(ne)                                  # quotient values, then its coefficients (degree - 1 pieces of n)
         self.tmp = [P(n) for _ in range(4)]
         self.tmp_side = [P(n) for _ in range(3)]
-        self.d_out = P(48)                              # commitments of a phase: up to 16 x 12 limbs (3 elements each)
+        # commitments of a phase: up to 16 x 12 limbs (3 elements each); element 48 holds the verdict words of the halo2-base
+        # witness form (u32 at byte 0: the Rational list, at byte 4: the lookup indices), downloaded with phase 0's commitments
+        self.d_out = P(49)
         self.d_status = P(max(1, cs.n_lookups))         # verdict word of every lookup permutation
+        self.grown = {}                                 # halo2-base witness form: buffers grown to the largest R / n_lookup seen
         self.zero = P(1)                                # one zero element (never written)
         self.h2d_bytes = self.d2h_bytes = 0
         self.begin, self.n_loc, self.allreduce = 0, n, None
@@ -367,8 +370,9 @@ class ProverSession:
         self.begin, self.n_loc, self.allreduce = begin, n_loc, allreduce
 
     # ---- helpers
-    def _commit(self, items) -> np.ndarray:
-        """items: list of (basis, device pointer); batched launches of up to 16, the commitments come down in one copy each"""
+    def _commit(self, items, verdict: bool = False) -> np.ndarray:
+        """items: list of (basis, device pointer); batched launches of up to 16, the commitments come down in one copy each.
+        verdict: the first copy also brings element 48 (the witness-form verdict words) down, into self.verdict"""
         ctx = self.ctx
         outs = []
         for lo in range(0, len(items), 16):
@@ -385,10 +389,13 @@ class ProverSession:
                     ctx.synchronize()
                     self._raw_download(p, arr)
                     self.keep.setdefault("committed", []).append((b, arr))
-            out = np.empty((m * 3, 4), dtype=np.uint64)
-            ctx.check(lib.h2b_poly_download(ctx.h, self.d_out.h, 0, C.c_void_p(out.ctypes.data), m * 3))
-            self.d2h_bytes += m * 96
-            outs.append(g1_normalize_host_batch(out))
+            cnt = 49 if verdict and lo == 0 else m * 3
+            out = np.empty((cnt, 4), dtype=np.uint64)
+            ctx.check(lib.h2b_poly_download(ctx.h, self.d_out.h, 0, C.c_void_p(out.ctypes.data), cnt))
+            self.d2h_bytes += cnt * 32
+            if cnt == 49:
+                self.verdict = (int(out[48, 0]) & 0xFFFFFFFF, int(out[48, 0]) >> 32)
+            outs.append(g1_normalize_host_batch(out[: m * 3]))
         return np.concatenate(outs)
 
     def _raw_download(self, dev_ptr: int, arr: np.ndarray):
@@ -398,6 +405,32 @@ class ProverSession:
                 self.ctx.check(lib.h2b_poly_download(self.ctx.h, p.h, (dev_ptr - p.ptr) // 32, C.c_void_p(arr.ctypes.data), len(arr)))
                 return
         raise ValueError("pointer outside the session's polynomials")
+
+    def _grown(self, name: str, n: int) -> Poly:
+        """a session buffer of at least n elements; reallocated only when a proof needs more than any proof before it"""
+        p = self.grown.get(name)
+        if p is None or p.n < n:
+            if p is not None:
+                self.polys.remove(p)
+                p.free()
+            p = Poly(self.ctx, max(n, 1))
+            self.polys.append(p)
+            self.grown[name] = p
+        return p
+
+    def _upload_u64(self, name: str, host_ptr: int, count: int) -> Poly:
+        """count uint64 words from host_ptr into the session buffer `name`: whole 32-byte elements straight from the caller's
+        array, the last 1..3 words through a zero-padded element (nothing past the end of the caller's array is read)"""
+        p = self._grown(name, (count + 3) // 4)
+        full = count // 4
+        if full:
+            p.upload_ptr(host_ptr, full)
+        if count % 4:
+            tail = np.zeros(4, dtype=np.uint64)
+            C.memmove(tail.ctypes.data, host_ptr + 32 * full, 8 * (count % 4))
+            p.upload(tail, full)
+        self.h2d_bytes += 8 * count
+        return p
 
     def _blind(self, col, first_row: int, rng: np.random.Generator):
         cnt = self.cs.n - first_row
@@ -425,11 +458,23 @@ class ProverSession:
             first = False
 
     def prove(self, witness_ptr: int, n_cells: int, random_poly_ptr: int, seed: int = 0, break_points=None,
-              lookup_ptr: int = 0, n_lookup: int = 0) -> dict:
+              lookup_ptr: int = 0, n_lookup: int = 0, rational_index_ptr: int = 0, rational_den_ptr: int = 0, n_rational: int = 0,
+              lookup_index_ptr: int = 0) -> dict:
         """witness_ptr: host pointer (pinned) to the n_cells Montgomery Fr cells of the virtual column, `break_points` as
-        keygen pinned them; lookup_ptr / n_lookup: the cells to look up (L > 0); random_poly_ptr: n elements"""
+        keygen pinned them; lookup_ptr / n_lookup: the cells to look up (L > 0); random_poly_ptr: n elements.
+
+        halo2-base's own witness form (`Vec<Assigned<F>>` walked once, nothing inverted): the witness holds n for every
+        Rational(n, d) cell, rational_index_ptr / rational_den_ptr the n_rational (uint64 virtual-column index, Montgomery d)
+        pairs, indices strictly increasing; lookup_index_ptr (instead of lookup_ptr) the n_lookup uint64 virtual-column
+        indices of the looked-up cells in `assign_raw` order.  The device makes of them what batch_invert_assigned and
+        assign_raw make (d = 0 -> 0).  A bad index raises H2BError once phase 0's commitments are down; no proof is returned."""
         ctx, cs, vp = self.ctx, self.cs, C.c_void_p
         k, n, ext_k, bf, u, A, L = cs.k, cs.n, cs.ext_k, cs.bf, cs.u, cs.A, cs.L
+        if lookup_ptr and lookup_index_ptr:
+            raise ValueError("prove: pass the looked-up cells either as values (lookup_ptr) or as indices (lookup_index_ptr)")
+        if n_rational and not (rational_index_ptr and rational_den_ptr):
+            raise ValueError("prove: n_rational > 0 needs rational_index_ptr and rational_den_ptr")
+        hb_form = bool(n_rational or lookup_index_ptr)
         rng = np.random.default_rng(seed)
         tr = Transcript()
         self.h2d_bytes = self.d2h_bytes = 0
@@ -454,29 +499,53 @@ class ProverSession:
             finally:
                 ctx.check(lib.h2b_ctx_side_end(ctx.h))
 
-        def commit(items):
-            cm = self._commit(items)
+        def commit(items, verdict=False):
+            cm = self._commit(items, verdict)
             res["commitments"] += list(cm)
             tr.absorb(cm)
 
         # ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside it)
         self.v.upload_ptr(witness_ptr, n_cells)
         self.h2d_bytes += n_cells * 32
-        if L:
+        if n_rational:
+            den = self._grown("rational_den", n_rational)
+            den.upload_ptr(rational_den_ptr, n_rational)
+            self.h2d_bytes += n_rational * 32
+            rat_idx = self._upload_u64("rational_index", rational_index_ptr, n_rational)
+        if L and lookup_index_ptr:
+            lk_idx = self._upload_u64("lookup_index", lookup_index_ptr, n_lookup)
+        elif L:
             self.lkv.upload_ptr(lookup_ptr, n_lookup)
             self.h2d_bytes += n_lookup * 32
         ctx.check(lib.h2b_ctx_side_begin(ctx.h))
         ctx.check(lib.h2b_poly_upload_async(ctx.h, self.rnd.h, 0, vp(random_poly_ptr), n))
         ctx.check(lib.h2b_ctx_side_end(ctx.h))
         self.h2d_bytes += n * 32
+        verdict = self.d_out.at(48)
+        if hb_form:  # zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
+            ctx.check(lib.h2b_apply_rational_dev(ctx.h, vp(self.v.ptr), n_cells, vp(rat_idx.ptr if n_rational else 0),
+                                                 vp(den.ptr if n_rational else 0), n_rational, vp(verdict)))
         nbp = 0 if break_points is None else len(break_points)
         bp_arr = (C.c_uint64 * max(1, nbp))(*[int(b) for b in (break_points if nbp else [])])
         ctx.check(lib.h2b_assign_columns_dev(ctx.h, vp(self.v.ptr), n_cells, bp_arr if nbp else None, nbp, k, A, vp(self.adv_block.ptr)))
-        if L:
+        if L and lookup_index_ptr:
+            ctx.check(lib.h2b_assign_lookups_indexed_dev(ctx.h, vp(self.v.ptr), n_cells, vp(lk_idx.ptr), n_lookup, k, L,
+                                                         vp(self.adv_block.at(A * n)), vp(verdict + 4)))
+        elif L:
             ctx.check(lib.h2b_assign_lookups_dev(ctx.h, vp(self.lkv.ptr), n_lookup, k, L, vp(self.adv_block.at(A * n))))
         for nm in cs.adv_names:
             self._blind(self.lagr[nm], u, rng)
-        commit([(BASIS_LAGRANGE, self.lagr[nm].ptr) for nm in cs.adv_names])
+        commit([(BASIS_LAGRANGE, self.lagr[nm].ptr) for nm in cs.adv_names], verdict=hb_form)
+        rat, lk = self.verdict if hb_form else (0, 0)
+        if not (L and lookup_index_ptr):
+            lk = 0  # the lookup word is only written by the indexed gather
+        if rat or lk:
+            ctx.check(lib.h2b_ctx_side_join(ctx.h))  # nothing of this proof stays in flight behind the error
+            ctx.synchronize()
+            why = (["a Rational index is >= the witness length"] if rat & 1 else []) + \
+                  (["the Rational indices do not strictly increase"] if rat & 2 else []) + \
+                  (["a lookup index is >= the witness length"] if lk & 1 else [])
+            raise H2BError(H2B_ERR_ARG, "prove: " + "; ".join(why))
         theta = tr.squeeze()
         mark("phase0 advice")
         ctx.check(lib.h2b_ctx_side_join(ctx.h))  # the random polynomial arrived while phase 0 ran

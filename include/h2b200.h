@@ -261,6 +261,18 @@ int h2b_assign_lookups_dev(h2b_ctx* ctx, const void* d_vals, size_t N, uint32_t 
  * (what the prover's batch_invert_assigned yields before committing). */
 int h2b_eval_rational(h2b_ctx* ctx, const uint64_t* num, const uint64_t* den, size_t n, uint64_t* out);
 int h2b_eval_rational_dev(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out);
+/* The halo2-base form of the witness, as one walk over ctx.advice yields it without inverting anything:
+ *   values  N cells: Zero -> 0, Trivial(x) -> x, Rational(n, d) -> n;
+ *   index / den  R pairs (uint64 virtual-column index, Montgomery d), one per Rational cell, indices strictly increasing;
+ *   lookup index  n_lookup uint64 virtual-column indices in LookupAnyManager::assign_raw order (the cells it copies).
+ * h2b_apply_rational_dev turns values into what `batch_invert_assigned` yields: values[index[i]] *= den[i]^-1, d = 0 -> 0.
+ * den is overwritten with its inverses.  h2b_assign_lookups_indexed_dev writes values[index[j]] to lookup column j mod L,
+ * row j div L, zero elsewhere, as h2b_assign_lookups (same H2B_ERR_LAYOUT rule).  Both are asynchronous: they zero the
+ * caller's device verdict word *d_status first and set bit 0 for an index >= N; apply_rational also sets bit 1 for an index
+ * not greater than the one before it.  A call with a non-zero verdict leaves its output undefined. */
+int h2b_apply_rational_dev(h2b_ctx* ctx, void* d_values, size_t N, const void* d_index, void* d_den, size_t R, uint32_t* d_status);
+int h2b_assign_lookups_indexed_dev(h2b_ctx* ctx, const void* d_values, size_t N, const void* d_index, size_t n_lookup, uint32_t k, size_t L,
+                                   void* d_cols, uint32_t* d_status);
 
 /* ---- grand-product primitives (SURVEY.md §8(f) rank 2: permutation / lookup arguments of create_proof, §3.3 step 4) */
 /* ff 0.13 `BatchInvert::batch_invert`: a[i] <- a[i]^-1 in place, zeros stay zero. */

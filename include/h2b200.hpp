@@ -215,6 +215,16 @@ inline std::vector<std::vector<Fr>> assign_lookups(const Context& ctx, const std
     return cols;
 }
 
+// halo2-base's own witness form on the device (asynchronous, device pointers; see h2b200.h): batch_invert_assigned of the
+// Rational cells in place, and assign_raw from virtual-column indices.  Violations land in the device word *d_status.
+inline void apply_rational_dev(const Context& ctx, void* d_values, size_t N, const void* d_index, void* d_den, size_t R, uint32_t* d_status) {
+    ctx.check(h2b_apply_rational_dev(ctx.raw(), d_values, N, d_index, d_den, R, d_status));
+}
+inline void assign_lookups_indexed_dev(const Context& ctx, const void* d_values, size_t N, const void* d_index, size_t n_lookup, uint32_t k,
+                                       size_t L, void* d_cols, uint32_t* d_status) {
+    ctx.check(h2b_assign_lookups_indexed_dev(ctx.raw(), d_values, N, d_index, n_lookup, k, L, d_cols, d_status));
+}
+
 // arithmetic::eval_polynomial(poly, point)
 inline Fr eval_polynomial(const Context& ctx, const std::vector<Fr>& poly, const Fr& point) {
     Fr out{};

@@ -378,6 +378,15 @@ public:
 };
 
 // ------------------------------------------------------------------------------------------------ one proof
+// halo2-base's own witness form (one walk over ctx.advice, nothing inverted): the witness holds n for every Rational(n, d)
+// cell; rational_index / rational_den are its (virtual-column index, Montgomery d) pairs, indices strictly increasing;
+// lookup_index replaces the looked-up values with the virtual-column indices of the cells assign_raw copies, in its order.
+struct AssignedWitness {
+    std::vector<uint64_t> rational_index;
+    std::vector<Fr> rational_den;
+    std::vector<uint64_t> lookup_index;
+};
+
 struct Proof {
     std::vector<G1> commitments;
     std::vector<std::pair<std::pair<std::string, int>, Fr>> evals;  // ((column, rotation), value) in query order
@@ -410,30 +419,45 @@ public:
         h = own(ne);
         for (auto& t : tmp) t = own(n);
         for (auto& t : tmp_side) t = own(n);
-        d_out = own(48);
+        d_out = own(49);  // up to 16 commitments; element 48: the verdict words of the halo2-base witness form
         d_status = own(std::max<size_t>(1, cs.n_lookups));
         zero = own(1);  // one zero element (never written)
     }
 
     // witness: the virtual column of the gate cells (Montgomery), break_points as keygen pinned them, lookup_cells in
-    // assign_raw order (L > 0), random_poly: the vanishing argument's random polynomial (n coefficients)
+    // assign_raw order (L > 0), random_poly: the vanishing argument's random polynomial (n coefficients).
+    // form: the halo2-base witness form (see AssignedWitness; then lookup_cells stays empty); a bad index throws once phase 0's
+    // commitments are down
     Proof create_proof(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
-                       const std::vector<Fr>& random_poly, const BlindSource& blind) {
+                       const std::vector<Fr>& random_poly, const BlindSource& blind, const AssignedWitness* form = nullptr) {
         const uint32_t k = cs.k, ext_k = cs.ext_k, bf = cs.bf;
         const size_t n = cs.n, u = cs.u, A = cs.A, L = cs.L;
         h2b_ctx* c = ctx.raw();
         Transcript tr;
         Proof res;
-        auto commit = [&](const std::vector<std::pair<int, void*>>& items, bool absorb) {
+        if (form && !lookup_cells.empty() && !form->lookup_index.empty())
+            throw Error(H2B_ERR_ARG, "create_proof: pass the looked-up cells either as values or as indices");
+        if (form && form->rational_index.size() != form->rational_den.size())
+            throw Error(H2B_ERR_ARG, "create_proof: rational_index and rational_den differ in length");
+        const bool lk_indexed = form && L && !form->lookup_index.empty();
+        uint64_t verdict = 0;  // phase 0: the verdict words, read with the first download of its commitments
+        auto commit = [&](const std::vector<std::pair<int, void*>>& items, bool absorb, bool with_verdict = false) {
             for (size_t lo = 0; lo < items.size(); lo += 16) {
                 const size_t m = std::min<size_t>(16, items.size() - lo);
                 std::vector<const void*> ptrs(m);
                 std::vector<int> bs(m);
                 for (size_t i = 0; i < m; i++) { bs[i] = items[lo + i].first; ptrs[i] = items[lo + i].second; }
                 ctx.check(h2b_msm_g1_batch_dev(c, params.raw(), bs.data(), ptrs.data(), m, n, d_out->at()));
+                const size_t cnt = with_verdict && lo == 0 ? 49 : m * 3;
                 std::vector<G1> out(m);
-                ctx.check(h2b_poly_download(c, d_out->raw(), 0, out[0].x.data(), m * 3));
-                res.d2h_bytes += m * 96;
+                if (cnt == 49) {
+                    std::vector<Fr> raw = d_out->download(0, 49);
+                    std::memcpy(out[0].x.data(), raw.data(), m * sizeof(G1));
+                    verdict = raw[48][0];
+                } else {
+                    ctx.check(h2b_poly_download(c, d_out->raw(), 0, out[0].x.data(), m * 3));
+                }
+                res.d2h_bytes += cnt * 32;
                 for (auto& pt : out) pt = g1_normalize_host(pt);  // affine form: what the transcript and the proof hold
                 if (absorb) tr.absorb(out.data(), m * sizeof(G1));
                 res.commitments.insert(res.commitments.end(), out.begin(), out.end());
@@ -473,7 +497,15 @@ public:
         // ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside it)
         v->upload(witness.data(), witness.size());
         res.h2d_bytes += witness.size() * 32;
-        if (L) {
+        const size_t R = form ? form->rational_index.size() : 0;
+        if (R) {
+            grown(rat_den, R)->upload(form->rational_den.data(), R);
+            res.h2d_bytes += R * 32;
+            upload_u64(rat_idx, form->rational_index, res);
+        }
+        if (lk_indexed) {
+            upload_u64(lk_idx, form->lookup_index, res);
+        } else if (L) {
             lkv->upload(lookup_cells.data(), lookup_cells.size());
             res.h2d_bytes += lookup_cells.size() * 32;
         }
@@ -481,15 +513,32 @@ public:
         rnd->upload_async(random_poly.data(), n);
         ctx.check(h2b_ctx_side_end(c));
         res.h2d_bytes += n * 32;
+        uint32_t* d_verdict = static_cast<uint32_t*>(d_out->at(48));
+        if (form)  // zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
+            ctx.check(h2b_apply_rational_dev(c, v->at(), witness.size(), R ? rat_idx->at() : nullptr, R ? rat_den->at() : nullptr, R, d_verdict));
         ctx.check(h2b_assign_columns_dev(c, v->at(), witness.size(), break_points.empty() ? nullptr : break_points.data(), break_points.size(), k, A,
                                          adv_block->at()));
-        if (L) ctx.check(h2b_assign_lookups_dev(c, lkv->at(), lookup_cells.size(), k, L, adv_block->at(A * n)));
+        if (lk_indexed)
+            ctx.check(h2b_assign_lookups_indexed_dev(c, v->at(), witness.size(), lk_idx->at(), form->lookup_index.size(), k, L, adv_block->at(A * n),
+                                                     d_verdict + 1));
+        else if (L)
+            ctx.check(h2b_assign_lookups_dev(c, lkv->at(), lookup_cells.size(), k, L, adv_block->at(A * n)));
         std::vector<std::pair<int, void*>> items;
         for (auto& nm : cs.adv_names) {
             blind_col(lagr[nm], u);
             items.push_back({H2B_BASIS_LAGRANGE, lagr[nm].ptr()});
         }
-        commit(items, true);
+        commit(items, true, form != nullptr);
+        const uint32_t rat_bad = uint32_t(verdict), lk_bad = lk_indexed ? uint32_t(verdict >> 32) : 0;
+        if (rat_bad || lk_bad) {
+            h2b_ctx_side_join(c);  // nothing of this proof stays in flight behind the error
+            h2b_ctx_synchronize(c);
+            std::string why;
+            if (rat_bad & 1) why += "; a Rational index is >= the witness length";
+            if (rat_bad & 2) why += "; the Rational indices do not strictly increase";
+            if (lk_bad & 1) why += "; a lookup index is >= the witness length";
+            throw Error(H2B_ERR_ARG, "create_proof" + why);
+        }
         res.theta = tr.squeeze();
         ctx.check(h2b_ctx_side_join(c));  // the random polynomial arrived while phase 0 ran
         side_transforms(cs.adv_names);
@@ -706,6 +755,17 @@ private:
         owned.push_back(std::make_unique<Poly>(ctx, m));
         return owned.back().get();
     }
+    // a buffer of the halo2-base witness form: reallocated only when a proof needs more than any proof before it
+    Poly* grown(PolyPtr& p, size_t m) {
+        if (!p || p->len() < m) p = std::make_unique<Poly>(ctx, std::max<size_t>(m, 1));
+        return p.get();
+    }
+    void upload_u64(PolyPtr& p, const std::vector<uint64_t>& words, Proof& res) {
+        std::vector<Fr> packed((words.size() + 3) / 4, Fr{});
+        if (!words.empty()) std::memcpy(packed[0].data(), words.data(), words.size() * 8);
+        grown(p, packed.size())->upload(packed.data(), packed.size());
+        res.h2d_bytes += words.size() * 8;
+    }
     // the arrays an h2b_graph points to live in `hold` until the next bind()
     h2b_graph bind(const GraphEvaluator& ev, ValueSource result, const std::vector<const void*>& fixed, const std::vector<const void*>& advice,
                    const Challenges& ch) {
@@ -737,6 +797,7 @@ private:
     const ProverCircuit& cs;
     std::vector<PolyPtr> owned;
     PolyPtr v, lkv, adv_block;
+    PolyPtr rat_den, rat_idx, lk_idx;  // the halo2-base witness form
     std::map<std::string, ColRef> lagr;
     std::map<std::string, Poly*> coef, ext;
     Poly *inp = nullptr, *rnd = nullptr, *h = nullptr, *d_out = nullptr, *d_status = nullptr, *zero = nullptr;

@@ -3,6 +3,7 @@
 //! `G1 {x, y, z}` are plain structs of those, so slices are passed as `*const u64` without copying — the `[u64; 4]`
 //! little-endian limb contract halo2-base itself relies on (halo2-base/src/utils/mod.rs:332-377).
 use crate::ffi::*;
+use crate::plonk::Assigned;  // the fork's own `Assigned` (halo2-axiom 0.5.3 plonk/assigned.rs), outside this directory
 use halo2curves::bn256::{Fr, G1Affine, G1};
 use once_cell::sync::OnceCell;
 use std::ffi::CStr;
@@ -113,6 +114,31 @@ impl Backend {
         cols
     }
 
+    /// halo2-base's own witness form for the resident prover (`h2b_apply_rational_dev`, `h2b_assign_lookups_indexed_dev`),
+    /// built in one walk with no inversion: `threads` = (context_id, `ctx.advice`) of every thread in order (their
+    /// concatenation is the virtual column); `lookups` = (context_id, offset) of every `ContextCell` that
+    /// `LookupAnyManager::assign_raw` copies (virtual_region/lookups.rs:130-155), in its order.
+    pub fn assigned_witness(&self, threads: &[(usize, &[Assigned<Fr>])], lookups: &[(usize, usize)]) -> AssignedWitness {
+        let mut start = std::collections::HashMap::new();
+        let mut w = AssignedWitness::default();
+        for (id, advice) in threads {
+            start.insert(*id, w.values.len() as u64);
+            for a in advice.iter() {
+                match a {
+                    Assigned::Zero => w.values.push(Fr::zero()),
+                    Assigned::Trivial(x) => w.values.push(*x),
+                    Assigned::Rational(n, d) => {
+                        w.rational_index.push(w.values.len() as u64);
+                        w.rational_den.push(*d);
+                        w.values.push(*n);
+                    }
+                }
+            }
+        }
+        w.lookup_index = lookups.iter().map(|(id, off)| start[id] + *off as u64).collect();
+        w
+    }
+
     pub fn poly(&self, len: usize) -> Poly {
         let mut h = std::ptr::null_mut();
         check(self.ctx, unsafe { h2b_poly_alloc(self.ctx, len, &mut h) });
@@ -127,6 +153,13 @@ impl Backend {
 #[repr(C)]
 #[derive(Clone, Copy)]
 pub struct AssignedCell { pub tag: u64, pub num: [u64; 4], pub den: [u64; 4] }
+
+/// halo2-base's own witness form (include/h2b200.h): `values` holds n for every `Rational(n, d)` cell;
+/// (`rational_index[i]`, `rational_den[i]`) are those cells, indices strictly increasing; `lookup_index` names the
+/// looked-up cells in the virtual column.  Upload the three arrays to `h2b_poly` buffers and call
+/// `h2b_apply_rational_dev`, `h2b_assign_columns_dev`, `h2b_assign_lookups_indexed_dev` (INTEGRATION.md §3b).
+#[derive(Default)]
+pub struct AssignedWitness { pub values: Vec<Fr>, pub rational_index: Vec<u64>, pub rational_den: Vec<Fr>, pub lookup_index: Vec<u64> }
 
 impl Poly {
     pub fn device_ptr(&self) -> *mut std::os::raw::c_void { unsafe { h2b_poly_device_ptr(self.h) } }
