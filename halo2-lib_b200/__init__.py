@@ -1,7 +1,7 @@
 """halo2-lib_b200 — host-side mirror (Python, for tests / bench plumbing) of the prover interfaces that the
 H100 back end implements behind the C ABI of include/h2b200.h.  The C++ mirror for a compiled host is
 include/h2b200.hpp; the Rust binding a maintainer adds is shown in INTEGRATION.md."""
-from ._capi import lib, LIB_PATH, SIGNATURES, header_symbols  # noqa: F401
+from ._capi import lib, LIB_PATH, SIGNATURES, header_symbols, H2B_ERR_ARG, CHECK_MAX_REPORT  # noqa: F401
 from .parallel import shard_range, ntt_owner, ntt_owners_balanced, all_gather_points, connect_peers, allreduce_points  # noqa: F401
 from .host import (  # noqa: F401
     H2BError,

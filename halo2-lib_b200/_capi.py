@@ -13,6 +13,7 @@ HEADER_PATH = os.path.join(os.path.dirname(HERE), "include", "h2b200.h")
 
 H2B_OK, H2B_ERR_ARG, H2B_ERR_CUDA, H2B_ERR_OOM, H2B_ERR_LAYOUT, H2B_ERR_UNSATISFIED = 0, -1, -2, -3, -4, -5
 BASIS_MONOMIAL, BASIS_LAGRANGE = 0, 1
+CHECK_MAX_REPORT = 65536  # H2B_CHECK_MAX_REPORT
 
 _vp, _sz, _u32, _int = C.c_void_p, C.c_size_t, C.c_uint32, C.c_int
 _u64p = C.POINTER(C.c_uint64)
@@ -126,6 +127,10 @@ SIGNATURES = {
     "h2b_permutation_fold_dev": (_int, [_vp, _vpp, _sz, _vpp, _vpp, _sz, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _u32, _vp]),
     "h2b_lookup_fold": (_int, [_vp, _gp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
     "h2b_lookup_fold_dev": (_int, [_vp, _gp, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _u32, _vp]),
+    "h2b_check_graph_dev": (_int, [_vp, _gp, _u32, _sz, _sz, _vp]),
+    "h2b_check_lookup_dev": (_int, [_vp, _vp, _vp, _u32, _sz, _sz, _vp]),
+    "h2b_permutation_decode_dev": (_int, [_vp, _vpp, _sz, _u32, _vp, _sz, _vp]),
+    "h2b_check_copies_dev": (_int, [_vp, _vpp, _vp, _sz, _u32, _sz, _vp]),
     "h2b_divide_by_vanishing_poly": (_int, [_vp, _vp, _u32, _u32]),
     "h2b_divide_by_vanishing_poly_dev": (_int, [_vp, _vp, _u32, _u32]),
     "h2b_eval_polynomial": (_int, [_vp, _vp, _sz, _vp, _vp]),

@@ -1362,6 +1362,35 @@ int h2b_divide_by_vanishing_poly(h2b_ctx* ctx, uint64_t* values, uint32_t k, uin
     });
 }
 
+// ------------------------------------------------------------------------------------------------ constraint check
+int h2b_check_graph_dev(h2b_ctx* ctx, const h2b_graph* g, uint32_t k, size_t rows, size_t max_report, void* d_report) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(g && d_report, "check_graph: null pointer");
+        check_graph_run(ctx, g, k, rows, max_report, d_report);
+    });
+}
+int h2b_check_lookup_dev(h2b_ctx* ctx, const void* d_input, const void* d_table, uint32_t k, size_t rows, size_t max_report,
+                         void* d_report) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_input && d_table && d_report, "check_lookup: null pointer");
+        check_lookup_run(ctx, d_input, d_table, k, rows, max_report, d_report);
+    });
+}
+int h2b_permutation_decode_dev(h2b_ctx* ctx, const void* const* d_sigma, size_t n_cols, uint32_t k, void* d_map, size_t max_report,
+                               void* d_reports) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_sigma && d_map && d_reports, "permutation_decode: null pointer");
+        permutation_decode_run(ctx, d_sigma, n_cols, k, d_map, max_report, d_reports);
+    });
+}
+int h2b_check_copies_dev(h2b_ctx* ctx, const void* const* d_columns, const void* d_map, size_t n_cols, uint32_t k, size_t max_report,
+                         void* d_reports) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_columns && d_map && d_reports, "check_copies: null pointer");
+        check_copies_run(ctx, d_columns, d_map, n_cols, k, max_report, d_reports);
+    });
+}
+
 // ------------------------------------------------------------------------------------------------ opening arithmetic
 int h2b_eval_polynomial_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n, const uint64_t x[4], uint64_t out[4]) {
     return guarded(ctx, [&] {

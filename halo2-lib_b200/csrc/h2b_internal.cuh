@@ -62,6 +62,8 @@ enum WsSlot {
     WS_MISC,
     WS_MISC2,
     WS_PROD,          // product-column scratch (numerators, denominators, power tables)
+    WS_CHECK_FLAGS,   // constraint check: one flag byte per checked cell, then the tile counts of the reports
+    WS_CHECK_TABLES,  // constraint check: omega powers and the hash table of the sigma decode
     WS_COUNT
 };
 
@@ -224,6 +226,18 @@ uint32_t* permute_expression_pair_enqueue(h2b_ctx* ctx, const void* d_input, con
                                           void* d_permuted_input, void* d_permuted_table);  // enqueue only; returns the device verdict word
 bool permute_expression_pair_run(h2b_ctx* ctx, const void* d_input, const void* d_table, uint32_t k, uint32_t blinding_factors,
                                  void* d_permuted_input, void* d_permuted_table);
+// the canonical sort of one column of n elements: out = src sorted by canonical value, out_canon = those canonical values;
+// scratch holds sort_column_scratch(n, sort_ctas) bytes, sort_ctas = sort_column_ctas(ctx, n) (the cooperative grid)
+int sort_column_ctas(h2b_ctx* ctx, uint32_t n);
+size_t sort_column_scratch(uint32_t n, int sort_ctas);
+void sort_column(h2b_ctx* ctx, const uint64_t* d_src, uint32_t n, uint64_t* d_out, uint64_t* d_out_canon, char* scratch, int sort_ctas);
+// ---- check.cu (MockProver::verify's checks; reports of max_report + 1 words per item, see include/h2b200.h)
+void check_graph_run(h2b_ctx* ctx, const h2b_graph* g, uint32_t k, size_t rows, size_t max_report, void* d_report);
+void check_lookup_run(h2b_ctx* ctx, const void* d_input, const void* d_table, uint32_t k, size_t rows, size_t max_report, void* d_report);
+void permutation_decode_run(h2b_ctx* ctx, const void* const* d_sigma, size_t n_cols, uint32_t k, void* d_map, size_t max_report,
+                            void* d_reports);
+void check_copies_run(h2b_ctx* ctx, const void* const* d_columns, const void* d_map, size_t n_cols, uint32_t k, size_t max_report,
+                      void* d_reports);
 // ---- srs.cu
 void g_to_lagrange_run(h2b_ctx* ctx, const void* d_g, uint32_t k, void* d_g_lagrange);
 void srs_setup_run(h2b_ctx* ctx, const uint64_t tau[4], const uint64_t base_xy[8], uint32_t k, void* d_g, void* d_g_lagrange);

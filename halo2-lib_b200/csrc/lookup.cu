@@ -27,27 +27,11 @@
 
 #include "h2b_internal.cuh"
 #include "field.cuh"
+#include "keys.cuh"
 
 namespace cg = cooperative_groups;
 
 namespace h2b {
-
-struct Key256 {
-    uint64_t l[4];
-};
-__device__ __forceinline__ int key_cmp(const Key256& a, const Key256& b) {
-#pragma unroll
-    for (int i = 3; i >= 0; i--) {
-        if (a.l[i] < b.l[i]) return -1;
-        if (a.l[i] > b.l[i]) return 1;
-    }
-    return 0;
-}
-__device__ __forceinline__ Key256 key_load(const uint64_t* p, size_t i) {
-    const ulonglong2* q = reinterpret_cast<const ulonglong2*>(p + 4 * i);
-    ulonglong2 a = q[0], b = q[1];
-    return Key256{{a.x, a.y, b.x, b.y}};
-}
 
 // canonical (non-Montgomery) values, the identity permutation, and diff[0..8) |= value XOR first value (a byte position
 // whose bits are all zero there is constant over the column: its sort pass is the identity)
@@ -184,17 +168,6 @@ __global__ void __launch_bounds__(256) k_gather_rows(const uint64_t* __restrict_
     Fr::load_nc(canon + 4 * j).store(out_canon + 4 * (size_t)i);
 }
 
-// is `key` present in the sorted column `col` (n canonical keys)?
-__device__ __forceinline__ bool sorted_contains(const uint64_t* col, u32 n, const Key256& key) {
-    u32 lo = 0, hi = n;
-    while (lo < hi) {
-        const u32 mid = (lo + hi) >> 1;
-        if (key_cmp(key_load(col, mid), key) < 0) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo < n && key_cmp(key_load(col, lo), key) == 0;
-}
-
 // rep[i] = 1 where A'[i] repeats A'[i-1]; left[j] = 1 where table value j is NOT consumed by a first occurrence;
 // *missing |= 1 when a first occurrence is absent from the table
 __global__ void __launch_bounds__(256) k_lookup_flags(const uint64_t* __restrict__ a_canon, const uint64_t* __restrict__ t_canon, u32 n,
@@ -281,8 +254,22 @@ __global__ void __launch_bounds__(256) k_xscan_apply(u32 n, const uint2* __restr
         if (base + e < n) { pa[base + e] += aa; pb[base + e] += ab; }
 }
 
+// cooperative grid of the sort: every CTA resident, no more CTAs than tiles
+int sort_column_ctas(h2b_ctx* ctx, u32 n) {
+    int per_sm = 0;
+    H2B_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_radix_sort, RS_T, 0));
+    H2B_REQUIRE(per_sm >= 1, "sort_column: the sort kernel does not fit on an SM");
+    int sort_ctas = ctx->sm_count * (per_sm < 4 ? per_sm : 4);
+    const int tiles = (int)((n + RS_T - 1) / RS_T);
+    if (sort_ctas > tiles) sort_ctas = tiles;
+    return sort_ctas;
+}
+size_t sort_column_scratch(u32 n, int sort_ctas) {
+    return ((size_t)n * (32 + 4 + 4) + (256 * (size_t)sort_ctas + 256 + 16) * 4 + 255) & ~(size_t)255;
+}
+
 // sorts one column: out = src sorted by canonical value, out_canon = the canonical values in that order
-static void sort_column(h2b_ctx* ctx, const uint64_t* d_src, u32 n, uint64_t* d_out, uint64_t* d_out_canon, char* scratch, int sort_ctas) {
+void sort_column(h2b_ctx* ctx, const uint64_t* d_src, u32 n, uint64_t* d_out, uint64_t* d_out_canon, char* scratch, int sort_ctas) {
     // scratch: canon (32 n) | idx_a (4 n) | idx_b (4 n) | table (256 x CTAs) | totals (256) | diff (8) | which (1)
     uint64_t* canon = (uint64_t*)scratch;
     u32* idx_a = (u32*)(canon + 4 * (size_t)n);
@@ -310,15 +297,9 @@ u32* permute_expression_pair_enqueue(h2b_ctx* ctx, const void* d_input, const vo
     const size_t rows = (size_t)1 << k;
     H2B_REQUIRE((size_t)blinding_factors + 1 < rows, "permute_expression_pair: no usable rows");
     const u32 n = (u32)(rows - (blinding_factors + 1));
-    // cooperative grid of the sort: every CTA resident, no more CTAs than tiles
-    int per_sm = 0;
-    H2B_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_radix_sort, RS_T, 0));
-    H2B_REQUIRE(per_sm >= 1, "permute_expression_pair: the sort kernel does not fit on an SM");
-    int sort_ctas = ctx->sm_count * (per_sm < 4 ? per_sm : 4);
-    const int tiles = (int)((n + RS_T - 1) / RS_T);
-    if (sort_ctas > tiles) sort_ctas = tiles;
+    const int sort_ctas = sort_column_ctas(ctx, n);
     const u32 ntiles = (n + XS_TILE - 1) / XS_TILE;
-    const size_t sort_scratch = ((size_t)n * (32 + 4 + 4) + (256 * (size_t)sort_ctas + 256 + 16) * 4 + 255) & ~(size_t)255;
+    const size_t sort_scratch = sort_column_scratch(n, sort_ctas);
     // workspace: sort scratch | a_canon | t_sorted | t_canon | rep, rep_pos, left, left_pos, rep_rows | tile sums | missing
     const size_t total = sort_scratch + 3 * (size_t)n * 32 + 5 * (size_t)n * 4 + (size_t)ntiles * 8 + 256;
     char* w = (char*)ctx->get(WS_SORT_TMP, total);

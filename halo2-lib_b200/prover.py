@@ -22,7 +22,7 @@ from __future__ import annotations
 import ctypes as C
 import hashlib
 import numpy as np
-from ._capi import lib, BASIS_MONOMIAL, BASIS_LAGRANGE, H2B_ERR_ARG
+from ._capi import lib, BASIS_MONOMIAL, BASIS_LAGRANGE, H2B_ERR_ARG, CHECK_MAX_REPORT
 from .host import Context, ParamsKZG, H2BError
 from . import evaluation as ev
 
@@ -207,11 +207,42 @@ class Circuit:
             self.lk_graph, self.lk_res = g2, g2.add_lookup([("product", ("fixed", 0, 0), ("advice", 0, 0))], [("fixed", 1, 0)])
         else:        # fixed slot [table], advice slot [l{t}]
             self.lk_graph, self.lk_res = g2, g2.add_lookup([("advice", 0, 0)], [("fixed", 0, 0)])
+        self._check = None  # what ProverSession.check needs beyond a proof, built by its first call (check_state)
+
+    def check_state(self):
+        """(gate program, its result, sigma map) for the constraint check, built on the first call: the vertical gate
+        q * (a + b c - d) as one program on fixed slot 0 / advice slot 0 (bound to q{j}, a{j} for every gate column), and the
+        sigma columns decoded into map[c][r] = c' << k | r' (u32, perm_cols order).  Raises H2BError naming the first
+        (column, row) whose sigma entry is not delta^c' omega^r' for a permutation column c'."""
+        if self._check is None:
+            ctx, npc = self.ctx, len(self.perm_cols)
+            g = ev.GraphEvaluator()
+            a = lambda r: ("advice", 0, r)
+            res = g.add_expression(("product", ("fixed", 0, 0), ("sum", ("sum", a(0), ("product", a(1), a(2))), ("negated", a(3)))))
+            smap = Poly(ctx, (npc * self.n + 7) // 8)
+            rep = Poly(ctx, (2 * npc + 3) // 4)  # max_report = 1: count and first row per column
+            sig = (C.c_void_p * npc)(*[self.lagr[nm].ptr for nm in self.sigma_names])
+            try:
+                ctx.check(lib.h2b_permutation_decode_dev(ctx.h, sig, npc, self.k, C.c_void_p(smap.ptr), 1, C.c_void_p(rep.ptr)))
+                words = rep.download().reshape(-1)
+            finally:
+                rep.free()
+            bad = [c for c in range(npc) if words[2 * c]]
+            if bad:
+                smap.free()
+                c = bad[0]
+                raise H2BError(H2B_ERR_ARG, "Circuit: the sigma entry of permutation column %d (%s) at row %d is not delta^c omega^r "
+                                            "for any of the %d permutation columns" % (c, self.perm_cols[c], int(words[2 * c + 1]), npc))
+            self._check = (g, res, smap)
+        return self._check
 
     def free(self):
         for d in (self.lagr, self.coeff, self.ext):
             for p in d.values():
                 p.free()
+        if self._check is not None:
+            self._check[2].free()
+            self._check = None
 
 
 def synthetic_circuit(ctx: Context, k: int, rng: np.random.Generator, lookup_bits: int = 8, A: int = 1, L: int = 0,
@@ -457,6 +488,119 @@ class ProverSession:
             ctx.check(lib.h2b_poly_lincomb_dev(ctx.h, arr, vp(lim.ctypes.data), len(pp), n, vp(out.ptr)))
             first = False
 
+    @staticmethod
+    def _check_witness_args(lookup_ptr, lookup_index_ptr, n_rational, rational_index_ptr, rational_den_ptr, who):
+        if lookup_ptr and lookup_index_ptr:
+            raise ValueError(who + ": pass the looked-up cells either as values (lookup_ptr) or as indices (lookup_index_ptr)")
+        if n_rational and not (rational_index_ptr and rational_den_ptr):
+            raise ValueError(who + ": n_rational > 0 needs rational_index_ptr and rational_den_ptr")
+
+    @staticmethod
+    def _witness_error(rat: int, lk: int, who: str):
+        """the verdict words of the halo2-base witness form (rat: h2b_apply_rational_dev, lk: the indexed gather) -> H2BError"""
+        why = (["a Rational index is >= the witness length"] if rat & 1 else []) + \
+              (["the Rational indices do not strictly increase"] if rat & 2 else []) + \
+              (["a lookup index is >= the witness length"] if lk & 1 else [])
+        raise H2BError(H2B_ERR_ARG, who + ": " + "; ".join(why))
+
+    def _assign_witness(self, witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr, n_rational,
+                        lookup_index_ptr, random_poly_ptr=0):
+        """phase 0 up to the advice columns in self.adv_block (what `prove` and `check` share): the witness, the halo2-base
+        form's Rational pairs and lookup indices or the looked-up values go up, the Rational cells become n * d^-1 and the
+        assignment lays out the gate and lookup-advice columns (all 2^k rows written).  With the halo2-base form the two
+        verdict words land in element 48 of d_out.  random_poly_ptr != 0: the random polynomial goes up on the side queue,
+        beside the assignment."""
+        ctx, cs, vp = self.ctx, self.cs, C.c_void_p
+        k, n, A, L = cs.k, cs.n, cs.A, cs.L
+        hb_form = bool(n_rational or lookup_index_ptr)
+        self.v.upload_ptr(witness_ptr, n_cells)
+        self.h2d_bytes += n_cells * 32
+        if n_rational:
+            den = self._grown("rational_den", n_rational)
+            den.upload_ptr(rational_den_ptr, n_rational)
+            self.h2d_bytes += n_rational * 32
+            rat_idx = self._upload_u64("rational_index", rational_index_ptr, n_rational)
+        if L and lookup_index_ptr:
+            lk_idx = self._upload_u64("lookup_index", lookup_index_ptr, n_lookup)
+        elif L:
+            self.lkv.upload_ptr(lookup_ptr, n_lookup)
+            self.h2d_bytes += n_lookup * 32
+        if random_poly_ptr:
+            ctx.check(lib.h2b_ctx_side_begin(ctx.h))
+            ctx.check(lib.h2b_poly_upload_async(ctx.h, self.rnd.h, 0, vp(random_poly_ptr), n))
+            ctx.check(lib.h2b_ctx_side_end(ctx.h))
+            self.h2d_bytes += n * 32
+        verdict = self.d_out.at(48)
+        if hb_form:  # zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
+            ctx.check(lib.h2b_apply_rational_dev(ctx.h, vp(self.v.ptr), n_cells, vp(rat_idx.ptr if n_rational else 0),
+                                                 vp(den.ptr if n_rational else 0), n_rational, vp(verdict)))
+        nbp = 0 if break_points is None else len(break_points)
+        bp_arr = (C.c_uint64 * max(1, nbp))(*[int(b) for b in (break_points if nbp else [])])
+        ctx.check(lib.h2b_assign_columns_dev(ctx.h, vp(self.v.ptr), n_cells, bp_arr if nbp else None, nbp, k, A, vp(self.adv_block.ptr)))
+        if L and lookup_index_ptr:
+            ctx.check(lib.h2b_assign_lookups_indexed_dev(ctx.h, vp(self.v.ptr), n_cells, vp(lk_idx.ptr), n_lookup, k, L,
+                                                         vp(self.adv_block.at(A * n)), vp(verdict + 4)))
+        elif L:
+            ctx.check(lib.h2b_assign_lookups_dev(ctx.h, vp(self.lkv.ptr), n_lookup, k, L, vp(self.adv_block.at(A * n))))
+
+    def check(self, witness_ptr: int, n_cells: int, break_points=None, lookup_ptr: int = 0, n_lookup: int = 0, rational_index_ptr: int = 0,
+              rational_den_ptr: int = 0, n_rational: int = 0, lookup_index_ptr: int = 0, max_report: int = 16) -> dict:
+        """MockProver::verify for this circuit: which gates, lookups and copy constraints the witness breaks, and where.
+        Takes the witness exactly as `prove` does and runs the same assignment; no blinding, no random polynomial, no transcript.
+        The values checked are the ones a proof would commit before blinding, with rows >= u read as 0:
+          gates[j]    rows r < u with q{j}(r) (a{j}(r) + a{j}(r+1) a{j}(r+2) - a{j}(r+3)) != 0 (rotations mod n);
+          lookups[t]  rows r < u whose input (q_lookup * a0, or l{t}) is not among the table's rows [0, u);
+          copies[c]   rows r < n of permutation column c (perm_cols order) whose value differs from the cell sigma_c(r) names.
+        Each entry is (failure count, the first min(count, max_report) failing rows ascending).  Every report comes down in one
+        copy.  A bad halo2-base index raises H2BError; so does a sigma entry that names no cell (on the circuit's first check)."""
+        ctx, cs, vp = self.ctx, self.cs, C.c_void_p
+        k, n, u, A, L = cs.k, cs.n, cs.u, cs.A, cs.L
+        self._check_witness_args(lookup_ptr, lookup_index_ptr, n_rational, rational_index_ptr, rational_den_ptr, "check")
+        if not 1 <= max_report <= CHECK_MAX_REPORT:
+            raise ValueError("check: max_report must be in 1..%d" % CHECK_MAX_REPORT)
+        gate, gate_res, smap = cs.check_state()
+        hb_form = bool(n_rational or lookup_index_ptr)
+        self.h2d_bytes = self.d2h_bytes = 0
+        self._assign_witness(witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr, n_rational,
+                             lookup_index_ptr)
+        zero_rows = self._grown("zero_rows", n - u)  # zero-filled, never written
+        for nm in cs.adv_names:
+            ctx.check(lib.h2b_poly_copy_dev(ctx.h, vp(self.lagr[nm].at(u)), vp(zero_rows.ptr), n - u))
+        # report block: element 0 = the witness-form verdict words, then max_report + 1 words per gate, lookup, permutation column
+        W, npc = max_report + 1, len(cs.perm_cols)
+        n_items = A + cs.n_lookups + npc
+        rep = self._grown("check_report", 1 + (n_items * W + 3) // 4)
+        at = lambda i: vp(rep.ptr + 32 + 8 * W * i)
+        if hb_form:
+            ctx.check(lib.h2b_poly_copy_dev(ctx.h, vp(rep.ptr), vp(self.d_out.at(48)), 1))
+        for j in range(A):
+            bg = ev.BoundGraph(gate, gate_res, fixed=[cs.lagr["q%d" % j].ptr], advice=[self.lagr["a%d" % j].ptr])
+            ctx.check(lib.h2b_check_graph_dev(ctx.h, C.byref(bg.struct), k, u, max_report, at(j)))
+        for t in range(cs.n_lookups):
+            if L == 0:
+                ctx.check(lib.h2b_fr_mul_elementwise_dev(ctx.h, vp(cs.lagr["q_lookup"].ptr), vp(self.lagr["a0"].ptr), n, vp(self.inp.ptr)))
+                inp = self.inp.ptr
+            else:
+                inp = self.lagr["l%d" % t].ptr
+            ctx.check(lib.h2b_check_lookup_dev(ctx.h, vp(inp), vp(cs.lagr["table"].ptr), k, u, max_report, at(A + t)))
+        cols = [cs.lagr["c"].ptr] + [self.lagr[nm].ptr for nm in cs.adv_names]
+        ctx.check(lib.h2b_check_copies_dev(ctx.h, (C.c_void_p * npc)(*cols), vp(smap.ptr), npc, k, max_report, at(A + cs.n_lookups)))
+        words = rep.download(0, 1 + (n_items * W + 3) // 4).reshape(-1)
+        self.d2h_bytes = 8 * len(words)
+        if hb_form:
+            rat, lk = int(words[0]) & 0xFFFFFFFF, int(words[0]) >> 32
+            lk = lk if L and lookup_index_ptr else 0  # the lookup word is only written by the indexed gather
+            if rat or lk:
+                self._witness_error(rat, lk, "check")
+        reports = []
+        for i in range(n_items):
+            w = words[4 + W * i: 4 + W * (i + 1)]
+            cnt = int(w[0])
+            reports.append((cnt, [int(r) for r in w[1:1 + min(cnt, max_report)]]))
+        res = {"gates": reports[:A], "lookups": reports[A:A + cs.n_lookups], "copies": reports[A + cs.n_lookups:]}
+        res["satisfied"] = not any(c for c, _ in reports)
+        return res
+
     def prove(self, witness_ptr: int, n_cells: int, random_poly_ptr: int, seed: int = 0, break_points=None,
               lookup_ptr: int = 0, n_lookup: int = 0, rational_index_ptr: int = 0, rational_den_ptr: int = 0, n_rational: int = 0,
               lookup_index_ptr: int = 0) -> dict:
@@ -470,10 +614,7 @@ class ProverSession:
         assign_raw make (d = 0 -> 0).  A bad index raises H2BError once phase 0's commitments are down; no proof is returned."""
         ctx, cs, vp = self.ctx, self.cs, C.c_void_p
         k, n, ext_k, bf, u, A, L = cs.k, cs.n, cs.ext_k, cs.bf, cs.u, cs.A, cs.L
-        if lookup_ptr and lookup_index_ptr:
-            raise ValueError("prove: pass the looked-up cells either as values (lookup_ptr) or as indices (lookup_index_ptr)")
-        if n_rational and not (rational_index_ptr and rational_den_ptr):
-            raise ValueError("prove: n_rational > 0 needs rational_index_ptr and rational_den_ptr")
+        self._check_witness_args(lookup_ptr, lookup_index_ptr, n_rational, rational_index_ptr, rational_den_ptr, "prove")
         hb_form = bool(n_rational or lookup_index_ptr)
         rng = np.random.default_rng(seed)
         tr = Transcript()
@@ -505,47 +646,16 @@ class ProverSession:
             tr.absorb(cm)
 
         # ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside it)
-        self.v.upload_ptr(witness_ptr, n_cells)
-        self.h2d_bytes += n_cells * 32
-        if n_rational:
-            den = self._grown("rational_den", n_rational)
-            den.upload_ptr(rational_den_ptr, n_rational)
-            self.h2d_bytes += n_rational * 32
-            rat_idx = self._upload_u64("rational_index", rational_index_ptr, n_rational)
-        if L and lookup_index_ptr:
-            lk_idx = self._upload_u64("lookup_index", lookup_index_ptr, n_lookup)
-        elif L:
-            self.lkv.upload_ptr(lookup_ptr, n_lookup)
-            self.h2d_bytes += n_lookup * 32
-        ctx.check(lib.h2b_ctx_side_begin(ctx.h))
-        ctx.check(lib.h2b_poly_upload_async(ctx.h, self.rnd.h, 0, vp(random_poly_ptr), n))
-        ctx.check(lib.h2b_ctx_side_end(ctx.h))
-        self.h2d_bytes += n * 32
-        verdict = self.d_out.at(48)
-        if hb_form:  # zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
-            ctx.check(lib.h2b_apply_rational_dev(ctx.h, vp(self.v.ptr), n_cells, vp(rat_idx.ptr if n_rational else 0),
-                                                 vp(den.ptr if n_rational else 0), n_rational, vp(verdict)))
-        nbp = 0 if break_points is None else len(break_points)
-        bp_arr = (C.c_uint64 * max(1, nbp))(*[int(b) for b in (break_points if nbp else [])])
-        ctx.check(lib.h2b_assign_columns_dev(ctx.h, vp(self.v.ptr), n_cells, bp_arr if nbp else None, nbp, k, A, vp(self.adv_block.ptr)))
-        if L and lookup_index_ptr:
-            ctx.check(lib.h2b_assign_lookups_indexed_dev(ctx.h, vp(self.v.ptr), n_cells, vp(lk_idx.ptr), n_lookup, k, L,
-                                                         vp(self.adv_block.at(A * n)), vp(verdict + 4)))
-        elif L:
-            ctx.check(lib.h2b_assign_lookups_dev(ctx.h, vp(self.lkv.ptr), n_lookup, k, L, vp(self.adv_block.at(A * n))))
+        self._assign_witness(witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr, n_rational,
+                             lookup_index_ptr, random_poly_ptr)
         for nm in cs.adv_names:
             self._blind(self.lagr[nm], u, rng)
         commit([(BASIS_LAGRANGE, self.lagr[nm].ptr) for nm in cs.adv_names], verdict=hb_form)
         rat, lk = self.verdict if hb_form else (0, 0)
-        if not (L and lookup_index_ptr):
-            lk = 0  # the lookup word is only written by the indexed gather
-        if rat or lk:
+        if rat or (L and lookup_index_ptr and lk):
             ctx.check(lib.h2b_ctx_side_join(ctx.h))  # nothing of this proof stays in flight behind the error
             ctx.synchronize()
-            why = (["a Rational index is >= the witness length"] if rat & 1 else []) + \
-                  (["the Rational indices do not strictly increase"] if rat & 2 else []) + \
-                  (["a lookup index is >= the witness length"] if lk & 1 else [])
-            raise H2BError(H2B_ERR_ARG, "prove: " + "; ".join(why))
+            self._witness_error(rat, lk if L and lookup_index_ptr else 0, "prove")
         theta = tr.squeeze()
         mark("phase0 advice")
         ctx.check(lib.h2b_ctx_side_join(ctx.h))  # the random polynomial arrived while phase 0 ran

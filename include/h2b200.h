@@ -394,6 +394,30 @@ int h2b_lookup_fold_dev(h2b_ctx* ctx, const h2b_graph* graph, const void* d_z, c
 int h2b_divide_by_vanishing_poly(h2b_ctx* ctx, uint64_t* values, uint32_t k, uint32_t ext_k);
 int h2b_divide_by_vanishing_poly_dev(h2b_ctx* ctx, void* d_values, uint32_t k, uint32_t ext_k);
 
+/* ---- constraint check: `MockProver::verify` for halo2-base's constraint system (which gate, lookup or copy constraint a
+ * witness breaks, and at which rows) on Lagrange columns of 2^k rows, asynchronous on the context's stream.
+ * A report is max_report + 1 uint64 words per checked item, in device memory: the failure count, then the first
+ * min(count, max_report) failing rows in ascending order, the remaining words zero.  The same inputs give the same bytes.
+ * 1 <= k <= 28 and 1 <= max_report <= H2B_CHECK_MAX_REPORT.  Scratch comes from the context's workspaces.
+ *   h2b_check_graph_dev       rows r < `rows` (<= 2^k) where the program's result is not zero; the graph runs on columns of 2^k
+ *                             rows with rotations mod 2^k (validated as h2b_quotient_graph_dev validates it; PREVIOUS reads 0).
+ *   h2b_check_lookup_dev      rows r < `rows` whose input value is not among table rows [0, rows).
+ *   h2b_permutation_decode_dev  n_cols sigma columns (the permutation's column order) -> d_map, n_cols x 2^k uint32:
+ *                             map[c][r] = c' << k | r' where sigma_c(r) = delta^c' omega^r', c' < n_cols.  An entry of no such
+ *                             form is reported in column c's report (d_reports: n_cols reports) and maps to (c, r) itself.
+ *                             Needs k + ceil(log2 n_cols) <= 32 and n_cols <= 65535.
+ *   h2b_check_copies_dev      cells (c, r), r < 2^k, whose value differs from the value of cell map[c][r] (a map entry naming a
+ *                             column >= n_cols counts as a failure); d_columns: host array of n_cols device pointers in the
+ *                             permutation's column order; d_reports: n_cols reports. */
+#define H2B_CHECK_MAX_REPORT 65536
+int h2b_check_graph_dev(h2b_ctx* ctx, const h2b_graph* g, uint32_t k, size_t rows, size_t max_report, void* d_report);
+int h2b_check_lookup_dev(h2b_ctx* ctx, const void* d_input, const void* d_table, uint32_t k, size_t rows, size_t max_report,
+                         void* d_report);
+int h2b_permutation_decode_dev(h2b_ctx* ctx, const void* const* d_sigma, size_t n_cols, uint32_t k, void* d_map,
+                               size_t max_report, void* d_reports /* n_cols reports: malformed entries */);
+int h2b_check_copies_dev(h2b_ctx* ctx, const void* const* d_columns, const void* d_map, size_t n_cols, uint32_t k,
+                         size_t max_report, void* d_reports /* n_cols reports */);
+
 /* ---- opening arithmetic (SURVEY.md §8(f) rank 4): halo2-axiom 0.5.3 `arithmetic::{eval_polynomial, kate_division}`
  * and the polynomial linear combinations of `poly/kzg/multiopen/shplonk/prover.rs` ------------------------------- */
 /* out = sum_i coeffs[i] * x^i */

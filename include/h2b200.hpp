@@ -225,6 +225,23 @@ inline void assign_lookups_indexed_dev(const Context& ctx, const void* d_values,
     ctx.check(h2b_assign_lookups_indexed_dev(ctx.raw(), d_values, N, d_index, n_lookup, k, L, d_cols, d_status));
 }
 
+// the constraint check (asynchronous, device pointers; see h2b200.h): reports of max_report + 1 u64 words per checked item
+inline void check_graph_dev(const Context& ctx, const h2b_graph& g, uint32_t k, size_t rows, size_t max_report, void* d_report) {
+    ctx.check(h2b_check_graph_dev(ctx.raw(), &g, k, rows, max_report, d_report));
+}
+inline void check_lookup_dev(const Context& ctx, const void* d_input, const void* d_table, uint32_t k, size_t rows, size_t max_report,
+                             void* d_report) {
+    ctx.check(h2b_check_lookup_dev(ctx.raw(), d_input, d_table, k, rows, max_report, d_report));
+}
+inline void permutation_decode_dev(const Context& ctx, const std::vector<const void*>& d_sigma, uint32_t k, void* d_map, size_t max_report,
+                                   void* d_reports) {
+    ctx.check(h2b_permutation_decode_dev(ctx.raw(), d_sigma.data(), d_sigma.size(), k, d_map, max_report, d_reports));
+}
+inline void check_copies_dev(const Context& ctx, const std::vector<const void*>& d_columns, const void* d_map, uint32_t k, size_t max_report,
+                             void* d_reports) {
+    ctx.check(h2b_check_copies_dev(ctx.raw(), d_columns.data(), d_map, d_columns.size(), k, max_report, d_reports));
+}
+
 // arithmetic::eval_polynomial(poly, point)
 inline Fr eval_polynomial(const Context& ctx, const std::vector<Fr>& poly, const Fr& point) {
     Fr out{};

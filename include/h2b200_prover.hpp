@@ -358,6 +358,36 @@ public:
         }
     }
 
+    // what ProverSession::check needs beyond a proof, built on the first check: the vertical gate as one program on fixed slot 0 /
+    // advice slot 0 (bound to q{j}, a{j} per gate column) and the sigma columns decoded into map[c][r] = c' << k | r' (u32);
+    // throws H2B_ERR_ARG naming the first (column, row) whose sigma entry names no cell.  A circuit never checked allocates nothing.
+    void prepare_check() const {
+        if (check_map) return;
+        GraphEvaluator ev;
+        const uint32_t r0 = ev.add_rotation(0), r1 = ev.add_rotation(1), r2 = ev.add_rotation(2), r3 = ev.add_rotation(3);
+        auto adv = [&](uint32_t rot) { return ev.add_calculation(Calculation::Store(ValueSource::Advice(0, rot))); };
+        const ValueSource q = ev.add_calculation(Calculation::Store(ValueSource::Fixed(0, r0)));
+        const ValueSource a0 = adv(r0), a1 = adv(r1), a2 = adv(r2), a3 = adv(r3);
+        const ValueSource sum = ev.add_calculation(Calculation::Add(a0, ev.add_calculation(Calculation::Mul(a1, a2))));
+        const ValueSource res = ev.add_calculation(Calculation::Mul(q, ev.add_calculation(Calculation::Sub(sum, a3))));
+        const size_t npc = perm_cols.size();
+        auto map = std::make_unique<Poly>(ctx, (npc * n + 7) / 8);
+        Poly rep(ctx, (2 * npc + 3) / 4);  // max_report = 1: count and first row per column
+        std::vector<const void*> sig;
+        for (auto& nm : sigma_names) sig.push_back(lagr.at(nm)->at());
+        permutation_decode_dev(ctx, sig, k, map->at(), 1, rep.at());
+        const std::vector<Fr> raw = rep.download(0, rep.len());
+        const uint64_t* w = raw[0].data();
+        for (size_t c = 0; c < npc; c++)
+            if (w[2 * c])
+                throw Error(H2B_ERR_ARG, "ProverCircuit: the sigma entry of permutation column " + std::to_string(c) + " (" + perm_cols[c] +
+                                             ") at row " + std::to_string(w[2 * c + 1]) + " is not delta^c omega^r for any of the " +
+                                             std::to_string(npc) + " permutation columns");
+        check_ev = std::move(ev);
+        check_result = res;
+        check_map = std::move(map);
+    }
+
     static constexpr size_t GATES_PER_PROGRAM = 5;
     struct GateProgram {
         GraphEvaluator ev;
@@ -375,6 +405,9 @@ public:
     std::vector<GateProgram> gate_programs;
     GraphEvaluator lookup_ev;
     ValueSource lookup_result{};
+    mutable GraphEvaluator check_ev;  // prepare_check()
+    mutable ValueSource check_result{};
+    mutable PolyPtr check_map;
 };
 
 // ------------------------------------------------------------------------------------------------ one proof
@@ -385,6 +418,13 @@ struct AssignedWitness {
     std::vector<uint64_t> rational_index;
     std::vector<Fr> rational_den;
     std::vector<uint64_t> lookup_index;
+};
+
+// ProverSession::check: per gate column, lookup and permutation column (perm_cols order) the failure count and the first
+// min(count, max_report) failing rows, ascending
+struct CheckReport {
+    bool satisfied = true;
+    std::vector<std::pair<uint64_t, std::vector<uint64_t>>> gates, lookups, copies;
 };
 
 struct Proof {
@@ -435,10 +475,7 @@ public:
         h2b_ctx* c = ctx.raw();
         Transcript tr;
         Proof res;
-        if (form && !lookup_cells.empty() && !form->lookup_index.empty())
-            throw Error(H2B_ERR_ARG, "create_proof: pass the looked-up cells either as values or as indices");
-        if (form && form->rational_index.size() != form->rational_den.size())
-            throw Error(H2B_ERR_ARG, "create_proof: rational_index and rational_den differ in length");
+        check_form(lookup_cells, form, "create_proof");
         const bool lk_indexed = form && L && !form->lookup_index.empty();
         uint64_t verdict = 0;  // phase 0: the verdict words, read with the first download of its commitments
         auto commit = [&](const std::vector<std::pair<int, void*>>& items, bool absorb, bool with_verdict = false) {
@@ -495,34 +532,7 @@ public:
         };
 
         // ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside it)
-        v->upload(witness.data(), witness.size());
-        res.h2d_bytes += witness.size() * 32;
-        const size_t R = form ? form->rational_index.size() : 0;
-        if (R) {
-            grown(rat_den, R)->upload(form->rational_den.data(), R);
-            res.h2d_bytes += R * 32;
-            upload_u64(rat_idx, form->rational_index, res);
-        }
-        if (lk_indexed) {
-            upload_u64(lk_idx, form->lookup_index, res);
-        } else if (L) {
-            lkv->upload(lookup_cells.data(), lookup_cells.size());
-            res.h2d_bytes += lookup_cells.size() * 32;
-        }
-        ctx.check(h2b_ctx_side_begin(c));
-        rnd->upload_async(random_poly.data(), n);
-        ctx.check(h2b_ctx_side_end(c));
-        res.h2d_bytes += n * 32;
-        uint32_t* d_verdict = static_cast<uint32_t*>(d_out->at(48));
-        if (form)  // zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
-            ctx.check(h2b_apply_rational_dev(c, v->at(), witness.size(), R ? rat_idx->at() : nullptr, R ? rat_den->at() : nullptr, R, d_verdict));
-        ctx.check(h2b_assign_columns_dev(c, v->at(), witness.size(), break_points.empty() ? nullptr : break_points.data(), break_points.size(), k, A,
-                                         adv_block->at()));
-        if (lk_indexed)
-            ctx.check(h2b_assign_lookups_indexed_dev(c, v->at(), witness.size(), lk_idx->at(), form->lookup_index.size(), k, L, adv_block->at(A * n),
-                                                     d_verdict + 1));
-        else if (L)
-            ctx.check(h2b_assign_lookups_dev(c, lkv->at(), lookup_cells.size(), k, L, adv_block->at(A * n)));
+        assign_witness(witness, break_points, lookup_cells, form, &random_poly, res.h2d_bytes);
         std::vector<std::pair<int, void*>> items;
         for (auto& nm : cs.adv_names) {
             blind_col(lagr[nm], u);
@@ -533,11 +543,7 @@ public:
         if (rat_bad || lk_bad) {
             h2b_ctx_side_join(c);  // nothing of this proof stays in flight behind the error
             h2b_ctx_synchronize(c);
-            std::string why;
-            if (rat_bad & 1) why += "; a Rational index is >= the witness length";
-            if (rat_bad & 2) why += "; the Rational indices do not strictly increase";
-            if (lk_bad & 1) why += "; a lookup index is >= the witness length";
-            throw Error(H2B_ERR_ARG, "create_proof" + why);
+            witness_error(rat_bad, lk_bad, "create_proof");
         }
         res.theta = tr.squeeze();
         ctx.check(h2b_ctx_side_join(c));  // the random polynomial arrived while phase 0 ran
@@ -750,7 +756,112 @@ public:
         return res;
     }
 
+    // MockProver::verify for this circuit (ProverSession.check of halo2-lib_b200/prover.py, same result): the witness as for
+    // create_proof, the same assignment, no blinding, no random polynomial, no transcript; rows >= u read as 0.  Every report
+    // comes down in one copy; a bad index of the halo2-base form throws H2B_ERR_ARG.
+    CheckReport check(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
+                      const AssignedWitness* form = nullptr, size_t max_report = 16) {
+        const uint32_t k = cs.k;
+        const size_t n = cs.n, u = cs.u, A = cs.A, L = cs.L;
+        h2b_ctx* c = ctx.raw();
+        check_form(lookup_cells, form, "check");
+        if (max_report < 1 || max_report > H2B_CHECK_MAX_REPORT) throw Error(H2B_ERR_ARG, "check: max_report out of range");
+        cs.prepare_check();
+        size_t h2d = 0;
+        assign_witness(witness, break_points, lookup_cells, form, nullptr, h2d);
+        Poly* zero_rows = grown(check_zero, n - u);  // zero-filled, never written
+        for (auto& nm : cs.adv_names) ctx.check(h2b_poly_copy_dev(c, lagr[nm].ptr(u), zero_rows->at(), n - u));
+        // report block: element 0 = the witness-form verdict words, then max_report + 1 words per gate, lookup, permutation column
+        const size_t W = max_report + 1, npc = cs.perm_cols.size(), n_items = A + cs.n_lookups + npc, elems = 1 + (n_items * W + 3) / 4;
+        Poly* rep = grown(check_rep, elems);
+        auto at = [&](size_t i) { return static_cast<char*>(rep->at(1)) + 8 * W * i; };
+        if (form) ctx.check(h2b_poly_copy_dev(c, rep->at(), d_out->at(48), 1));
+        for (size_t j = 0; j < A; j++) {
+            const h2b_graph g = bind(cs.check_ev, cs.check_result, {cs.lagr.at("q" + std::to_string(j))->at()}, {lagr["a" + std::to_string(j)].ptr()},
+                                     Challenges{});
+            check_graph_dev(ctx, g, k, u, max_report, at(j));
+        }
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const void* in = lagr[L ? "l" + std::to_string(t) : "a0"].ptr();
+            if (L == 0) {
+                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at("q_lookup")->at(), in, n, inp->at()));
+                in = inp->at();
+            }
+            check_lookup_dev(ctx, in, cs.lagr.at("table")->at(), k, u, max_report, at(A + t));
+        }
+        std::vector<const void*> cols{cs.lagr.at("c")->at()};
+        for (auto& nm : cs.adv_names) cols.push_back(lagr[nm].ptr());
+        check_copies_dev(ctx, cols, cs.check_map->at(), k, max_report, at(A + cs.n_lookups));
+        const std::vector<Fr> raw = rep->download(0, elems);
+        const uint64_t* w = raw[0].data();
+        if (form) {
+            const uint32_t rat_bad = uint32_t(w[0]), lk_bad = (L && !form->lookup_index.empty()) ? uint32_t(w[0] >> 32) : 0;
+            if (rat_bad || lk_bad) witness_error(rat_bad, lk_bad, "check");
+        }
+        CheckReport out;
+        for (size_t i = 0; i < n_items; i++) {
+            const uint64_t* r = w + 4 + W * i;
+            std::pair<uint64_t, std::vector<uint64_t>> e{r[0], std::vector<uint64_t>(r + 1, r + 1 + std::min<uint64_t>(r[0], max_report))};
+            out.satisfied = out.satisfied && r[0] == 0;
+            (i < A ? out.gates : i < A + cs.n_lookups ? out.lookups : out.copies).push_back(std::move(e));
+        }
+        return out;
+    }
+
 private:
+    static void check_form(const std::vector<Fr>& lookup_cells, const AssignedWitness* form, const std::string& who) {
+        if (form && !lookup_cells.empty() && !form->lookup_index.empty())
+            throw Error(H2B_ERR_ARG, who + ": pass the looked-up cells either as values or as indices");
+        if (form && form->rational_index.size() != form->rational_den.size())
+            throw Error(H2B_ERR_ARG, who + ": rational_index and rational_den differ in length");
+    }
+    [[noreturn]] static void witness_error(uint32_t rat_bad, uint32_t lk_bad, const std::string& who) {
+        std::string why;
+        if (rat_bad & 1) why += "; a Rational index is >= the witness length";
+        if (rat_bad & 2) why += "; the Rational indices do not strictly increase";
+        if (lk_bad & 1) why += "; a lookup index is >= the witness length";
+        throw Error(H2B_ERR_ARG, who + why);
+    }
+    // phase 0 up to the advice columns in adv_block (what create_proof and check share): witness, Rational pairs and lookup
+    // indices or looked-up values up, Rational cells -> n * d^-1, the assignment; with the halo2-base form the verdict words
+    // land in element 48 of d_out.  random_poly != nullptr: it goes up on the side queue, beside the assignment.
+    void assign_witness(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
+                        const AssignedWitness* form, const std::vector<Fr>* random_poly, size_t& h2d_bytes) {
+        const uint32_t k = cs.k;
+        const size_t n = cs.n, A = cs.A, L = cs.L;
+        h2b_ctx* c = ctx.raw();
+        const bool lk_indexed = form && L && !form->lookup_index.empty();
+        v->upload(witness.data(), witness.size());
+        h2d_bytes += witness.size() * 32;
+        const size_t R = form ? form->rational_index.size() : 0;
+        if (R) {
+            grown(rat_den, R)->upload(form->rational_den.data(), R);
+            h2d_bytes += R * 32;
+            upload_u64(rat_idx, form->rational_index, h2d_bytes);
+        }
+        if (lk_indexed) {
+            upload_u64(lk_idx, form->lookup_index, h2d_bytes);
+        } else if (L) {
+            lkv->upload(lookup_cells.data(), lookup_cells.size());
+            h2d_bytes += lookup_cells.size() * 32;
+        }
+        if (random_poly) {
+            ctx.check(h2b_ctx_side_begin(c));
+            rnd->upload_async(random_poly->data(), n);
+            ctx.check(h2b_ctx_side_end(c));
+            h2d_bytes += n * 32;
+        }
+        uint32_t* d_verdict = static_cast<uint32_t*>(d_out->at(48));
+        if (form)  // zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
+            ctx.check(h2b_apply_rational_dev(c, v->at(), witness.size(), R ? rat_idx->at() : nullptr, R ? rat_den->at() : nullptr, R, d_verdict));
+        ctx.check(h2b_assign_columns_dev(c, v->at(), witness.size(), break_points.empty() ? nullptr : break_points.data(), break_points.size(), k, A,
+                                         adv_block->at()));
+        if (lk_indexed)
+            ctx.check(h2b_assign_lookups_indexed_dev(c, v->at(), witness.size(), lk_idx->at(), form->lookup_index.size(), k, L, adv_block->at(A * n),
+                                                     d_verdict + 1));
+        else if (L)
+            ctx.check(h2b_assign_lookups_dev(c, lkv->at(), lookup_cells.size(), k, L, adv_block->at(A * n)));
+    }
     Poly* own(size_t m) {
         owned.push_back(std::make_unique<Poly>(ctx, m));
         return owned.back().get();
@@ -760,11 +871,11 @@ private:
         if (!p || p->len() < m) p = std::make_unique<Poly>(ctx, std::max<size_t>(m, 1));
         return p.get();
     }
-    void upload_u64(PolyPtr& p, const std::vector<uint64_t>& words, Proof& res) {
+    void upload_u64(PolyPtr& p, const std::vector<uint64_t>& words, size_t& h2d_bytes) {
         std::vector<Fr> packed((words.size() + 3) / 4, Fr{});
         if (!words.empty()) std::memcpy(packed[0].data(), words.data(), words.size() * 8);
         grown(p, packed.size())->upload(packed.data(), packed.size());
-        res.h2d_bytes += words.size() * 8;
+        h2d_bytes += words.size() * 8;
     }
     // the arrays an h2b_graph points to live in `hold` until the next bind()
     h2b_graph bind(const GraphEvaluator& ev, ValueSource result, const std::vector<const void*>& fixed, const std::vector<const void*>& advice,
@@ -798,6 +909,7 @@ private:
     std::vector<PolyPtr> owned;
     PolyPtr v, lkv, adv_block;
     PolyPtr rat_den, rat_idx, lk_idx;  // the halo2-base witness form
+    PolyPtr check_zero, check_rep;     // check(): zero rows, the report block
     std::map<std::string, ColRef> lagr;
     std::map<std::string, Poly*> coef, ext;
     Poly *inp = nullptr, *rnd = nullptr, *h = nullptr, *d_out = nullptr, *d_status = nullptr, *zero = nullptr;
