@@ -1,4 +1,5 @@
-"""ctypes binding of libh2b200.so — exactly the symbols include/h2b200.h declares.
+"""ctypes binding of libh2b200.so: the symbols include/h2b200.h declares (SIGNATURES), and the private calls through
+which prover.py drives the compiled resident prover (PROVER_SIGNATURES, halo2-lib_b200/csrc/prover_binding.cu).
 
 There is no fallback: if the shared library is missing the import fails, and if no CUDA device is present
 `Context()` raises (h2b_ctx_create returns H2B_ERR_CUDA)."""
@@ -156,6 +157,37 @@ SIGNATURES = {
 }
 
 
+class Witness(C.Structure):
+    """h2b::WitnessView (include/h2b200_prover.hpp): the witness of one proof or check, host pointers + counts"""
+    _fields_ = [
+        ("cells", _vp), ("n_cells", _sz), ("break_points", _vp), ("n_break_points", _sz),
+        ("lookup_cells", _vp), ("lookup_index", _vp), ("n_lookup", _sz),
+        ("rational_index", _vp), ("rational_den", _vp), ("n_rational", _sz),
+    ]
+
+
+# callbacks of the compiled prover (first argument: the `user` pointer); 0 = success, anything else stops the proof
+BLIND_FN = C.CFUNCTYPE(_int, _vp, _sz, _vp)             # (rows, out: rows x 4 limbs)
+ALLREDUCE_FN = C.CFUNCTYPE(_int, _vp, _vp, _sz)         # (device pointer of the m partial commitments, m)
+COMMIT_FN = C.CFUNCTYPE(_int, _vp, _int, _vp, _sz)      # (basis, host rows of the committed polynomial, n)
+_witp = C.POINTER(Witness)
+_u64s = C.POINTER(C.c_uint64)
+
+PROVER_SIGNATURES = {
+    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp)]),
+    "h2bp_circuit_free": (None, [_vp]),
+    "h2bp_circuit_info": (_int, [_vp, _u64s, C.c_char_p, _sz]),
+    "h2bp_circuit_column": (_int, [_vp, C.c_char_p, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
+    "h2bp_session_create": (_int, [_vp, _vp, _u32, _sz, _vp, C.POINTER(_vp)]),
+    "h2bp_session_free": (None, [_vp]),
+    "h2bp_session_info": (_int, [_vp, _u64s, C.c_char_p, _sz]),
+    "h2bp_session_column": (_int, [_vp, C.c_char_p, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
+    "h2bp_session_shard": (_int, [_vp, _sz, _sz, ALLREDUCE_FN, _vp]),
+    "h2bp_prove": (_int, [_vp, _witp, _vp, BLIND_FN, _vp, COMMIT_FN, _vp, _vp, _vp, _vp, _vp]),
+    "h2bp_check": (_int, [_vp, _witp, _sz, _vp]),
+}
+
+
 def header_symbols() -> list[str]:
     """Function names declared in include/h2b200.h (used by the CPU test that every symbol is exported)."""
     txt = open(HEADER_PATH).read()
@@ -169,7 +201,7 @@ def load() -> C.CDLL:
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(there is no CPU fallback)")
     lib = C.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in {**SIGNATURES, **PROVER_SIGNATURES}.items():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args

@@ -1,0 +1,207 @@
+// prover_binding.cu — the private C binding of the resident prover (include/h2b200_prover.hpp) that halo2-lib_b200/prover.py
+// calls through ctypes.  The calls are the Python package's binding, not product ABI: include/h2b200.h does not declare them.
+// Host code only.  No exception leaves this file: every call maps failures to a status code + h2b_last_error().
+#include <algorithm>
+#include <array>
+#include <cstdint>
+#include <cstring>
+#include <functional>
+#include <map>
+#include <memory>
+#include <stdexcept>
+#include <string>
+#include <utility>
+#include <vector>
+
+#include "h2b_internal.cuh"
+
+// the header's inline code stays private to the library: programs that include the header never bind to this copy
+#pragma GCC visibility push(hidden)
+#include "../../include/h2b200_prover.hpp"
+
+namespace h2bp {
+using namespace h2b;
+
+struct BoundCircuit {
+    Context ctx;
+    ProverCircuit cs;
+    BoundCircuit(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, const std::map<std::string, const Fr*>& fixed,
+                 const std::vector<const Fr*>& sigma)
+        : ctx(c), cs(ctx, k, A, L, sel, fixed, sigma) {}
+};
+struct BoundSession {
+    Context ctx;
+    ParamsKZG params;
+    ProverSession sess;
+    BoundSession(h2b_ctx* c, h2b_srs* srs, uint32_t k, size_t srs_count, const ProverCircuit& cs)
+        : ctx(c), params(ctx, k, srs, srs_count), sess(ctx, params, cs) {}
+};
+
+// Runs `body` and translates every failure.  The context lock is taken only to store the message: the prover calls the public
+// entry points, which take that (non-recursive) lock themselves.
+template <class Fn>
+int run(h2b_ctx* ctx, Fn&& body) {
+    if (!ctx) return H2B_ERR_ARG;
+    int code;
+    std::string msg;
+    try {
+        body();
+        return H2B_OK;
+    } catch (const Error& e) {
+        code = e.code;
+        msg = e.what();
+        const std::string prefix = "h2b200 error " + std::to_string(e.code) + ": ";
+        if (msg.compare(0, prefix.size(), prefix) == 0) msg.erase(0, prefix.size());
+    } catch (const std::bad_alloc&) {
+        code = H2B_ERR_OOM;
+        msg = "host allocation failed";
+    } catch (const std::exception& e) {
+        code = H2B_ERR_CUDA;
+        msg = e.what();
+    } catch (...) {
+        code = H2B_ERR_CUDA;
+        msg = "unknown failure";
+    }
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    ctx->err = msg;
+    return code;
+}
+
+std::string join(const std::vector<std::string>& v) {
+    std::string s;
+    for (auto& x : v) s += (s.empty() ? "" : ",") + x;
+    return s;
+}
+void write_text(const std::string& s, char* out, size_t cap) {
+    if (!out || s.size() + 1 > cap) throw Error(H2B_ERR_ARG, "name buffer too small");
+    std::memcpy(out, s.c_str(), s.size() + 1);
+}
+void write_column(const NamedColumn& c, h2b_poly** poly, size_t* offset, size_t* rows) {
+    if (!poly || !offset || !rows) throw Error(H2B_ERR_ARG, "null output");
+    *poly = c.col.poly->raw();
+    *offset = c.col.offset;
+    *rows = c.rows;
+}
+}  // namespace h2bp
+using namespace h2b;
+using namespace h2bp;
+
+// callbacks: 0 = success; anything else aborts the proof with H2B_ERR_ARG
+typedef int (*h2bp_blind_fn)(void* user, size_t rows, uint64_t* out);              // rows x 4 limbs of blinding scalars
+typedef int (*h2bp_allreduce_fn)(void* user, void* d_points, size_t m);             // see ProverSession::shard
+typedef int (*h2bp_commit_fn)(void* user, int basis, const uint64_t* rows, size_t n);  // see ProverSession::observer
+
+#define H2BP_API extern "C" __attribute__((visibility("default")))
+
+// fixed: n_fixed named columns (at least the circuit's fixed_names), sigma: one per permutation column; 2^k rows each
+H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, const char* const* fixed_names,
+                                 const uint64_t* const* fixed, size_t n_fixed, const uint64_t* const* sigma, size_t n_sigma,
+                                 BoundCircuit** out) {
+    return run(ctx, [&] {
+        if (!out || (n_fixed && (!fixed_names || !fixed)) || (n_sigma && !sigma)) throw Error(H2B_ERR_ARG, "circuit_create: null argument");
+        std::map<std::string, const Fr*> f;
+        for (size_t i = 0; i < n_fixed; i++) f[fixed_names[i]] = reinterpret_cast<const Fr*>(fixed[i]);
+        std::vector<const Fr*> s;
+        for (size_t i = 0; i < n_sigma; i++) s.push_back(reinterpret_cast<const Fr*>(sigma[i]));
+        *out = new BoundCircuit(ctx, k, A, L, selector_lookup != 0, f, s);
+    });
+}
+H2BP_API void h2bp_circuit_free(BoundCircuit* b) { delete b; }
+
+// shape: degree, chunk, ext_k, bf, u, n_sets, n_lookups, selector_lookup; names: "adv=..\nperm=..\nfixed=..\nsigma=.." (comma-separated)
+H2BP_API int h2bp_circuit_info(BoundCircuit* b, uint64_t* shape, char* names, size_t cap) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        const ProverCircuit& cs = b->cs;
+        const uint64_t v[8] = {cs.degree, cs.chunk, cs.ext_k, cs.bf, cs.u, cs.n_sets, cs.n_lookups, cs.selector_lookup};
+        if (!shape) throw Error(H2B_ERR_ARG, "circuit_info: null shape");
+        std::copy(v, v + 8, shape);
+        write_text("adv=" + join(cs.adv_names) + "\nperm=" + join(cs.perm_cols) + "\nfixed=" + join(cs.fixed_names) + "\nsigma=" +
+                       join(cs.sigma_names),
+                   names, cap);
+    });
+}
+H2BP_API int h2bp_circuit_column(BoundCircuit* b, const char* table, const char* name, h2b_poly** poly, size_t* offset, size_t* rows) {
+    return run(b ? b->ctx.raw() : nullptr, [&] { write_column(b->cs.column(table ? table : "", name ? name : ""), poly, offset, rows); });
+}
+
+// srs: the caller's SRS handle (its shard holds srs_count points); both handles must outlive the session
+H2BP_API int h2bp_session_create(h2b_ctx* ctx, h2b_srs* srs, uint32_t k, size_t srs_count, BoundCircuit* cs, BoundSession** out) {
+    return run(ctx, [&] {
+        if (!srs || !cs || !out) throw Error(H2B_ERR_ARG, "session_create: null argument");
+        *out = new BoundSession(ctx, srs, k, srs_count, cs->cs);
+    });
+}
+H2BP_API void h2bp_session_free(BoundSession* b) { delete b; }
+
+// counts: commitments per proof, evaluations per proof; names: the evaluations' "column:rotation", comma-separated, in order
+H2BP_API int h2bp_session_info(BoundSession* b, uint64_t* counts, char* names, size_t cap) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        const auto q = b->sess.queries();
+        std::vector<std::string> nm;
+        for (auto& e : q) nm.push_back(e.name + ":" + std::to_string(e.rot));
+        if (!counts) throw Error(H2B_ERR_ARG, "session_info: null counts");
+        counts[0] = b->sess.commitments_per_proof();
+        counts[1] = q.size();
+        write_text(join(nm), names, cap);
+    });
+}
+H2BP_API int h2bp_session_column(BoundSession* b, const char* table, const char* name, h2b_poly** poly, size_t* offset, size_t* rows) {
+    return run(b ? b->ctx.raw() : nullptr, [&] { write_column(b->sess.column(table ? table : "", name ? name : ""), poly, offset, rows); });
+}
+H2BP_API int h2bp_session_shard(BoundSession* b, size_t begin, size_t n_loc, h2bp_allreduce_fn fn, void* user) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        ProverSession::AllReduce ar;
+        if (fn)
+            ar = [fn, user](void* d, size_t m) {
+                if (fn(user, d, m)) throw Error(H2B_ERR_ARG, "the all-reduce callback failed");
+            };
+        b->sess.shard(begin, n_loc, std::move(ar));
+    });
+}
+
+// one proof.  random_poly: 2^k elements (pinned); observer may be null.  Out: commitments (affine, 12 limbs each),
+// evaluations (4 limbs each), the challenges theta beta gamma y x (Montgomery, 4 limbs each), bytes = [h2d, d2h]
+H2BP_API int h2bp_prove(BoundSession* b, const WitnessView* w, const uint64_t* random_poly, h2bp_blind_fn blind, void* blind_user,
+                        h2bp_commit_fn observer, void* observer_user, uint64_t* commitments, uint64_t* evals, uint64_t* challenges,
+                        uint64_t* bytes) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        if (!w || !blind || !commitments || !evals || !challenges || !bytes) throw Error(H2B_ERR_ARG, "prove: null argument");
+        ProverSession& s = b->sess;
+        s.observer = nullptr;
+        if (observer)
+            s.observer = [observer, observer_user](int basis, const std::vector<Fr>& rows) {
+                if (observer(observer_user, basis, rows[0].data(), rows.size())) throw Error(H2B_ERR_ARG, "the commit observer failed");
+            };
+        auto source = [&](size_t rows) {
+            std::vector<Fr> out(rows);
+            if (blind(blind_user, rows, out[0].data())) throw Error(H2B_ERR_ARG, "the blinding callback failed");
+            return out;
+        };
+        const Proof pr = s.create_proof(*w, reinterpret_cast<const Fr*>(random_poly), source);
+        std::memcpy(commitments, pr.commitments.data(), pr.commitments.size() * sizeof(G1));
+        for (size_t i = 0; i < pr.evals.size(); i++) std::memcpy(evals + 4 * i, pr.evals[i].second.data(), 32);
+        const Fr* ch[5] = {&pr.theta, &pr.beta, &pr.gamma, &pr.y, &pr.x};
+        for (int i = 0; i < 5; i++) std::memcpy(challenges + 4 * i, ch[i]->data(), 32);
+        bytes[0] = pr.h2d_bytes;
+        bytes[1] = pr.d2h_bytes;
+    });
+}
+
+// the constraint check.  report: max_report + 1 words per gate column, lookup and permutation column (in that order): the
+// failure count, then the first min(count, max_report) failing rows ascending
+H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report, uint64_t* report) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        if (!w || !report) throw Error(H2B_ERR_ARG, "check: null argument");
+        const CheckReport r = b->sess.check(*w, max_report);
+        uint64_t* p = report;
+        for (auto* part : {&r.gates, &r.lookups, &r.copies})
+            for (auto& [count, rows] : *part) {
+                std::fill(p, p + max_report + 1, 0);
+                p[0] = count;
+                std::copy(rows.begin(), rows.end(), p + 1);
+                p += max_report + 1;
+            }
+    });
+}
+
+#pragma GCC visibility pop

@@ -59,8 +59,12 @@ public:
         int rc = h2b_ctx_create_multi(devices.data(), (int)devices.size(), &ctx_);
         if (rc != H2B_OK) throw Error(rc, h2b_last_error(nullptr));
     }
+    // a view of a context the caller owns and destroys (a binding that already holds the handle)
+    explicit Context(h2b_ctx* borrowed) : ctx_(borrowed), owned_(false) {}
     int device_count() const { return h2b_ctx_device_count(ctx_); }
-    ~Context() { h2b_ctx_destroy(ctx_); }
+    ~Context() {
+        if (owned_) h2b_ctx_destroy(ctx_);
+    }
     Context(const Context&) = delete;
     Context& operator=(const Context&) = delete;
     h2b_ctx* raw() const { return ctx_; }
@@ -82,6 +86,7 @@ public:
 
 private:
     h2b_ctx* ctx_ = nullptr;
+    bool owned_ = true;
 };
 
 // best_multiexp(coeffs, bases): ad-hoc bases.  Rust asserts coeffs.len() == bases.len().
@@ -112,7 +117,12 @@ public:
                                  g_lagrange.empty() ? nullptr : reinterpret_cast<const uint64_t*>(g_lagrange.data()), k,
                                  begin, count_, &srs_));
     }
-    ~ParamsKZG() { h2b_srs_destroy(ctx_.raw(), srs_); }
+    // a view of an SRS handle the caller owns and destroys (its shard holds `count` points)
+    ParamsKZG(const Context& ctx, uint32_t k, h2b_srs* borrowed, size_t count)
+        : ctx_(ctx), k_(k), count_(count), srs_(borrowed), owned_(false) {}
+    ~ParamsKZG() {
+        if (owned_) h2b_srs_destroy(ctx_.raw(), srs_);
+    }
     ParamsKZG(const ParamsKZG&) = delete;
     ParamsKZG& operator=(const ParamsKZG&) = delete;
     uint32_t k() const { return k_; }
@@ -144,6 +154,7 @@ private:
     uint32_t k_;
     size_t count_;
     h2b_srs* srs_ = nullptr;
+    bool owned_ = true;
 };
 
 // EvaluationDomain::new(j, k): j = cs.degree(); quotient_poly_degree = j - 1; extended_k = least e >= k with

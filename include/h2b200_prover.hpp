@@ -1,9 +1,8 @@
 // h2b200_prover.hpp — C++ host side of the RESIDENT prover: the data flow of halo2-axiom 0.5.3 `create_proof`
 // (sole halo2-lib call site: halo2-base/src/utils/testing.rs:40-48) for the constraint system halo2-base builds, with
-// every column kept in HBM behind `h2b_poly` handles between the phases.  It is the compiled twin of
-// halo2-lib_b200/prover.py (same phases, same transcript, same order of commitments, evaluations and opening sets: the two
-// produce identical bytes for the same inputs — tests/test_gpu_prover.py::test_cpp_prover_matches_python) and the shape a
-// Rust `create_proof` over include/h2b200.h would take (INTEGRATION.md §3b).
+// every column kept in HBM behind `h2b_poly` handles between the phases.  It is the one implementation of the proof
+// sequence: halo2-lib_b200/prover.py binds it through halo2-lib_b200/csrc/prover_binding.cu, and it is the shape a Rust
+// `create_proof` over include/h2b200.h would take (INTEGRATION.md §3b).
 //
 // Circuit shape (halo2-base `BaseCircuitParams`): A gate-advice columns a0..a{A-1} with selectors q{j} and the vertical
 // gate q (a0 + a1 a2 - a3) (flex_gate/mod.rs:80-91); L lookup-advice columns l0..l{L-1} looked up in `table` as they are
@@ -25,7 +24,8 @@ namespace h2b {
 
 // ------------------------------------------------------------------------------------------------ host-side fields (Montgomery)
 // a few dozen multiplications per proof: challenges, rotations of the evaluation point, powers of v and mu (Fr); one
-// inversion per commitment to bring it to affine form before it enters the transcript (Fq) — what the Rust side does on the CPU
+// inversion per downloaded batch of commitments to bring them to affine form before they enter the transcript (Fq) — what
+// the Rust side does on the CPU
 struct FrHostParams {
     static constexpr uint64_t MOD[4] = {0x43e1f593f0000001ULL, 0x2833e84879b97091ULL, 0xb85045b68181585dULL, 0x30644e72e131a029ULL};
     static constexpr uint64_t R1[4] = {0xac96341c4ffffffbULL, 0x36fc76959f60cd29ULL, 0x666ea36f7879462eULL, 0x0e0a77c19a07df2fULL};
@@ -138,11 +138,32 @@ struct HostFr : HostField<FrHostParams> {
     }
 };
 // Jacobian (X, Y, Z) -> (X / Z^2, Y / Z^3, 1), the identity -> all zero: the form in which a commitment enters the transcript
-// and the proof (the accumulation order inside an MSM is not deterministic, the Jacobian representative therefore is not either)
+// and the proof (the accumulation order inside an MSM is not deterministic, the Jacobian representative therefore is not either).
+// In place over the m commitments of one download with ONE inversion (Montgomery's trick): the host does this between phases
+// while the GPU waits.
+inline void g1_normalize_host_batch(G1* pts, size_t m) {
+    std::vector<Fq> pref(m);  // prefix products over the non-zero z
+    Fq acc = HostFq::one();
+    for (size_t i = 0; i < m; i++) {
+        pref[i] = acc;
+        if (!HostFq::is_zero(pts[i].z)) acc = HostFq::mul(acc, pts[i].z);
+    }
+    Fq inv = HostFq::inv(acc);
+    for (size_t i = m; i-- > 0;) {
+        G1& p = pts[i];
+        if (HostFq::is_zero(p.z)) {
+            p = G1{};
+            continue;
+        }
+        const Fq zi = HostFq::mul(inv, pref[i]), zi2 = HostFq::mul(zi, zi);
+        inv = HostFq::mul(inv, p.z);
+        p = G1{HostFq::mul(p.x, zi2), HostFq::mul(p.y, HostFq::mul(zi2, zi)), HostFq::one()};
+    }
+}
 inline G1 g1_normalize_host(const G1& p) {
-    if (HostFq::is_zero(p.z)) return G1{{0, 0, 0, 0}, {0, 0, 0, 0}, {0, 0, 0, 0}};
-    const Fq zi = HostFq::inv(p.z), zi2 = HostFq::mul(zi, zi);
-    return G1{HostFq::mul(p.x, zi2), HostFq::mul(p.y, HostFq::mul(zi2, zi)), HostFq::one()};
+    G1 q = p;
+    g1_normalize_host_batch(&q, 1);
+    return q;
 }
 
 // ------------------------------------------------------------------------------------------------ Blake2b-512 (RFC 7693)
@@ -244,8 +265,12 @@ public:
     void* at(size_t elem = 0) const { return ptr_ + 32 * elem; }
     size_t len() const { return n_; }
     h2b_poly* raw() const { return h_; }
-    void upload(const Fr* host, size_t n, size_t offset = 0) const { ctx_->check(h2b_poly_upload(ctx_->raw(), h_, offset, host->data(), n)); }
-    void upload_async(const Fr* pinned, size_t n, size_t offset = 0) const { ctx_->check(h2b_poly_upload_async(ctx_->raw(), h_, offset, pinned->data(), n)); }
+    void upload(const Fr* host, size_t n, size_t offset = 0) const {
+        ctx_->check(h2b_poly_upload(ctx_->raw(), h_, offset, reinterpret_cast<const uint64_t*>(host), n));
+    }
+    void upload_async(const Fr* pinned, size_t n, size_t offset = 0) const {
+        ctx_->check(h2b_poly_upload_async(ctx_->raw(), h_, offset, reinterpret_cast<const uint64_t*>(pinned), n));
+    }
     std::vector<Fr> download(size_t offset, size_t n) const {
         std::vector<Fr> out(n);
         if (n) ctx_->check(h2b_poly_download(ctx_->raw(), h_, offset, out[0].data(), n));
@@ -260,11 +285,16 @@ private:
 };
 using PolyPtr = std::unique_ptr<Poly>;
 
-// a column: n rows of a device polynomial (an advice column is a slice of the block the assignment kernels write)
+// a column: rows of a device polynomial from `offset` on (an advice column is a slice of the block the assignment kernels write)
 struct ColRef {
     const Poly* poly = nullptr;
     size_t offset = 0;
     void* ptr(size_t row = 0) const { return poly->at(offset + row); }
+};
+// a named device column (tests read them back): where it is and how many rows it has
+struct NamedColumn {
+    ColRef col;
+    size_t rows = 0;
 };
 
 // ------------------------------------------------------------------------------------------------ the fixed side of a circuit
@@ -274,6 +304,10 @@ public:
     // in the order [c, a0.., l0..]
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, std::vector<Fr>>& fixed,
                   const std::vector<std::vector<Fr>>& sigma)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k)) {}
+    // the same with every column as a pointer to its 2^k rows (nothing is copied on the host)
+    ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
+                  const std::vector<const Fr*>& sigma)
         : ctx(ctx), k(k), n(size_t(1) << k), A(A), L(L), selector_lookup(selector_lookup && L == 0) {
         degree = L ? 4 : (this->selector_lookup ? 5 : 3);
         chunk = degree - 2;
@@ -295,11 +329,11 @@ public:
         l0[0] = HostFr::one();
         ll[u] = HostFr::one();
         for (size_t i = 0; i < u; i++) la[i] = HostFr::one();
-        auto add = [&](const std::string& name, const std::vector<Fr>& arr) {
-            if (arr.size() != n) throw Error(H2B_ERR_ARG, "ProverCircuit: column " + name + " must hold 2^k rows");
+        auto add = [&](const std::string& name, const Fr* arr) {
+            if (!arr) throw Error(H2B_ERR_ARG, "ProverCircuit: column " + name + " is null");
             auto lg = std::make_unique<Poly>(ctx, n), cf = std::make_unique<Poly>(ctx, n), ex = std::make_unique<Poly>(ctx, size_t(1) << ext_k);
-            lg->upload(arr.data(), n);
-            cf->upload(arr.data(), n);
+            lg->upload(arr, n);
+            cf->upload(arr, n);
             ctx.check(h2b_lagrange_to_coeff_dev(ctx.raw(), cf->at(), k));
             ctx.check(h2b_coeff_to_extended_dev(ctx.raw(), cf->at(), n, ext_k, ex->at()));
             lagr[name] = std::move(lg);
@@ -315,9 +349,9 @@ public:
             sigma_names.push_back("sigma_" + perm_cols[i]);
             add(sigma_names.back(), sigma[i]);
         }
-        add("l0", l0);
-        add("l_last", ll);
-        add("l_active", la);
+        add("l0", l0.data());
+        add("l_last", ll.data());
+        add("l_active", la.data());
         h2b_ctx_synchronize(ctx.raw());
         // gate programs: GATES_PER_PROGRAM vertical gates each (a program holds at most 64 calculations); every program continues
         // the Horner fold in y from the previous value, so the chain of programs is the one fold evaluate_h does
@@ -388,6 +422,18 @@ public:
         check_map = std::move(map);
     }
 
+    // a fixed-side column by name, for tests: "lagr" / "coeff" / "ext" (fixed, sigma and the l0 / l_last / l_active columns)
+    // and "sigma_map" (the decoded sigma of the check, built here on first use)
+    NamedColumn column(const std::string& table, const std::string& name) const {
+        if (table == "sigma_map") {
+            prepare_check();
+            return {{check_map.get(), 0}, check_map->len()};
+        }
+        const std::map<std::string, PolyPtr>* t = table == "lagr" ? &lagr : table == "coeff" ? &coeff : table == "ext" ? &ext : nullptr;
+        if (!t || !t->count(name)) throw Error(H2B_ERR_ARG, "ProverCircuit: no column " + table + " " + name);
+        return {{t->at(name).get(), 0}, t->at(name)->len()};
+    }
+
     static constexpr size_t GATES_PER_PROGRAM = 5;
     struct GateProgram {
         GraphEvaluator ev;
@@ -408,6 +454,24 @@ public:
     mutable GraphEvaluator check_ev;  // prepare_check()
     mutable ValueSource check_result{};
     mutable PolyPtr check_map;
+
+private:
+    static std::map<std::string, const Fr*> rows_of(const std::map<std::string, std::vector<Fr>>& cols, uint32_t k) {
+        std::map<std::string, const Fr*> out;
+        for (auto& [name, v] : cols) {
+            if (v.size() != size_t(1) << k) throw Error(H2B_ERR_ARG, "ProverCircuit: column " + name + " must hold 2^k rows");
+            out[name] = v.data();
+        }
+        return out;
+    }
+    static std::vector<const Fr*> rows_of(const std::vector<std::vector<Fr>>& cols, uint32_t k) {
+        std::vector<const Fr*> out;
+        for (auto& v : cols) {
+            if (v.size() != size_t(1) << k) throw Error(H2B_ERR_ARG, "ProverCircuit: every sigma column must hold 2^k rows");
+            out.push_back(v.data());
+        }
+        return out;
+    }
 };
 
 // ------------------------------------------------------------------------------------------------ one proof
@@ -418,6 +482,24 @@ struct AssignedWitness {
     std::vector<uint64_t> rational_index;
     std::vector<Fr> rational_den;
     std::vector<uint64_t> lookup_index;
+};
+
+// The witness of one proof or check as the caller holds it, pointer + count (nothing is copied on the host): the virtual
+// column of the gate cells (Montgomery), break_points as keygen pinned them, and the looked-up cells in assign_raw order (L > 0)
+// either as values (lookup_cells) or, in the halo2-base form, as virtual-column indices (lookup_index) — together with the
+// (index, d) pairs of its Rational cells (see AssignedWitness).
+struct WitnessView {
+    const Fr* cells = nullptr;
+    size_t n_cells = 0;
+    const uint64_t* break_points = nullptr;
+    size_t n_break_points = 0;
+    const Fr* lookup_cells = nullptr;
+    const uint64_t* lookup_index = nullptr;
+    size_t n_lookup = 0;
+    const uint64_t* rational_index = nullptr;
+    const Fr* rational_den = nullptr;
+    size_t n_rational = 0;
+    bool assigned_form() const { return n_rational || lookup_index; }
 };
 
 // ProverSession::check: per gate column, lookup and permutation column (perm_cols order) the failure count and the first
@@ -438,8 +520,12 @@ class ProverSession {
 public:
     // `blind(rows)`: the caller's source of blinding scalars (Montgomery limbs), called in the order the prover blinds its columns
     using BlindSource = std::function<std::vector<Fr>(size_t)>;
+    // `allreduce(d_points, m)`: combines the m partial commitments (Jacobian, on the device) of all ranks in place
+    using AllReduce = std::function<void(void*, size_t)>;
+    // `observer(basis, rows)`: the n rows of every committed polynomial, in commit order (verification runs; synchronises)
+    using CommitObserver = std::function<void(int, const std::vector<Fr>&)>;
 
-    ProverSession(const Context& ctx, const ParamsKZG& params, const ProverCircuit& cs) : ctx(ctx), params(params), cs(cs) {
+    ProverSession(const Context& ctx, const ParamsKZG& params, const ProverCircuit& cs) : ctx(ctx), params(params), cs(cs), n_loc(cs.n) {
         const size_t n = cs.n, ne = size_t(1) << cs.ext_k;
         v = std::make_unique<Poly>(ctx, n * cs.A);
         if (cs.L) lkv = std::make_unique<Poly>(ctx, n * cs.L);
@@ -464,27 +550,47 @@ public:
         zero = own(1);  // one zero element (never written)
     }
 
+    // multi-GPU: this rank commits rows [begin, begin + n_loc) of every polynomial (its shard of the SRS) and `allreduce`
+    // combines the partial commitments of all ranks after every batched MSM, before they come down; everything else is replicated
+    void shard(size_t begin, size_t n_loc, AllReduce allreduce) {
+        if (begin + n_loc > cs.n) throw Error(H2B_ERR_ARG, "shard: rows past 2^k");
+        shard_begin = begin;
+        this->n_loc = n_loc;
+        this->allreduce = std::move(allreduce);
+    }
+    CommitObserver observer;  // empty: proofs download nothing but commitments and evaluations
+
     // witness: the virtual column of the gate cells (Montgomery), break_points as keygen pinned them, lookup_cells in
     // assign_raw order (L > 0), random_poly: the vanishing argument's random polynomial (n coefficients).
     // form: the halo2-base witness form (see AssignedWitness; then lookup_cells stays empty); a bad index throws once phase 0's
     // commitments are down
     Proof create_proof(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
                        const std::vector<Fr>& random_poly, const BlindSource& blind, const AssignedWitness* form = nullptr) {
+        if (random_poly.size() != cs.n) throw Error(H2B_ERR_ARG, "create_proof: the random polynomial must hold 2^k coefficients");
+        return create_proof(view(witness, break_points, lookup_cells, form, "create_proof"), random_poly.data(), blind);
+    }
+    // random_poly: n coefficients in pinned host memory (uploaded asynchronously beside phase 0)
+    Proof create_proof(const WitnessView& wit, const Fr* random_poly, const BlindSource& blind) {
         const uint32_t k = cs.k, ext_k = cs.ext_k, bf = cs.bf;
-        const size_t n = cs.n, u = cs.u, A = cs.A, L = cs.L;
+        const size_t n = cs.n, u = cs.u, L = cs.L;
         h2b_ctx* c = ctx.raw();
         Transcript tr;
         Proof res;
-        check_form(lookup_cells, form, "create_proof");
-        const bool lk_indexed = form && L && !form->lookup_index.empty();
+        check_inputs(wit, "create_proof");
+        if (!random_poly) throw Error(H2B_ERR_ARG, "create_proof: null random polynomial");
         uint64_t verdict = 0;  // phase 0: the verdict words, read with the first download of its commitments
-        auto commit = [&](const std::vector<std::pair<int, void*>>& items, bool absorb, bool with_verdict = false) {
+        auto commit = [&](const std::vector<std::pair<int, ColRef>>& items, bool absorb, bool with_verdict = false) {
             for (size_t lo = 0; lo < items.size(); lo += 16) {
                 const size_t m = std::min<size_t>(16, items.size() - lo);
                 std::vector<const void*> ptrs(m);
                 std::vector<int> bs(m);
-                for (size_t i = 0; i < m; i++) { bs[i] = items[lo + i].first; ptrs[i] = items[lo + i].second; }
-                ctx.check(h2b_msm_g1_batch_dev(c, params.raw(), bs.data(), ptrs.data(), m, n, d_out->at()));
+                for (size_t i = 0; i < m; i++) { bs[i] = items[lo + i].first; ptrs[i] = items[lo + i].second.ptr(shard_begin); }
+                ctx.check(h2b_msm_g1_batch_dev(c, params.raw(), bs.data(), ptrs.data(), m, n_loc, d_out->at()));
+                if (allreduce) allreduce(d_out->at(), m);
+                if (observer) {
+                    ctx.check(h2b_ctx_synchronize(c));
+                    for (size_t i = 0; i < m; i++) observer(bs[i], items[lo + i].second.poly->download(items[lo + i].second.offset, n));
+                }
                 const size_t cnt = with_verdict && lo == 0 ? 49 : m * 3;
                 std::vector<G1> out(m);
                 if (cnt == 49) {
@@ -495,7 +601,7 @@ public:
                     ctx.check(h2b_poly_download(c, d_out->raw(), 0, out[0].x.data(), m * 3));
                 }
                 res.d2h_bytes += cnt * 32;
-                for (auto& pt : out) pt = g1_normalize_host(pt);  // affine form: what the transcript and the proof hold
+                g1_normalize_host_batch(out.data(), m);  // affine form: what the transcript and the proof hold
                 if (absorb) tr.absorb(out.data(), m * sizeof(G1));
                 res.commitments.insert(res.commitments.end(), out.begin(), out.end());
             }
@@ -532,14 +638,14 @@ public:
         };
 
         // ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside it)
-        assign_witness(witness, break_points, lookup_cells, form, &random_poly, res.h2d_bytes);
-        std::vector<std::pair<int, void*>> items;
+        assign_witness(wit, random_poly, res.h2d_bytes);
+        std::vector<std::pair<int, ColRef>> items;
         for (auto& nm : cs.adv_names) {
             blind_col(lagr[nm], u);
-            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm].ptr()});
+            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm]});
         }
-        commit(items, true, form != nullptr);
-        const uint32_t rat_bad = uint32_t(verdict), lk_bad = lk_indexed ? uint32_t(verdict >> 32) : 0;
+        commit(items, true, wit.assigned_form());
+        const uint32_t rat_bad = uint32_t(verdict), lk_bad = L && wit.lookup_index ? uint32_t(verdict >> 32) : 0;
         if (rat_bad || lk_bad) {
             h2b_ctx_side_join(c);  // nothing of this proof stays in flight behind the error
             h2b_ctx_synchronize(c);
@@ -565,8 +671,8 @@ public:
                                                             static_cast<uint32_t*>(d_status->at(t))));
             blind_col(pa, u);
             blind_col(ps, u);
-            items.push_back({H2B_BASIS_LAGRANGE, pa.ptr()});
-            items.push_back({H2B_BASIS_LAGRANGE, ps.ptr()});
+            items.push_back({H2B_BASIS_LAGRANGE, pa});
+            items.push_back({H2B_BASIS_LAGRANGE, ps});
             perm_names.push_back("pa" + ts);
             perm_names.push_back("ps" + ts);
         }
@@ -602,10 +708,10 @@ public:
         items.clear();
         for (auto& nm : prod_names) {
             blind_col(lagr[nm], u + 1);
-            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm].ptr()});
+            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm]});
         }
         side_transforms(prod_names);  // beside the commitments below
-        items.push_back({H2B_BASIS_MONOMIAL, rnd->at()});
+        items.push_back({H2B_BASIS_MONOMIAL, ColRef{rnd, 0}});
         commit(items, true);
         res.y = tr.squeeze();
         ctx.check(h2b_ctx_side_join(c));  // every column is now in coefficient and extended form
@@ -651,36 +757,13 @@ public:
         ctx.check(h2b_extended_to_coeff_dev(c, h->at(), ext_k));
         const size_t pieces = cs.degree - 1;
         items.clear();
-        for (size_t j = 0; j < pieces; j++) items.push_back({H2B_BASIS_MONOMIAL, h->at(j * n)});
+        for (size_t j = 0; j < pieces; j++) items.push_back({H2B_BASIS_MONOMIAL, ColRef{h, j * n}});
         commit(items, true);
         res.x = tr.squeeze();
         // ---- evaluations at x and its rotations
         const Fr w = HostFr::omega(k);
         auto rot = [&](int r) { return HostFr::mul(res.x, HostFr::pow(w, uint64_t(((r % (long long)n) + (long long)n) % (long long)n))); };
-        const int last = -int(bf + 1);
-        struct Query { std::string name; const void* ptr; int rot; };
-        std::vector<Query> queries;
-        for (size_t j = 0; j < A; j++)
-            for (int r : {0, 1, 2, 3}) queries.push_back({"a" + std::to_string(j), coef["a" + std::to_string(j)]->at(), r});
-        for (size_t t = 0; t < L; t++) queries.push_back({"l" + std::to_string(t), coef["l" + std::to_string(t)]->at(), 0});
-        for (auto& nm : cs.fixed_names) queries.push_back({nm, cs.coeff.at(nm)->at(), 0});
-        for (auto& nm : cs.sigma_names) queries.push_back({nm, cs.coeff.at(nm)->at(), 0});
-        for (size_t s = 0; s < cs.n_sets; s++) {  // every set at x and omega x; all but the last one also at omega^last x
-            const std::string nm = "zp" + std::to_string(s);
-            queries.push_back({nm, coef[nm]->at(), 0});
-            queries.push_back({nm, coef[nm]->at(), 1});
-            if (s + 1 < cs.n_sets) queries.push_back({nm, coef[nm]->at(), last});
-        }
-        for (size_t t = 0; t < cs.n_lookups; t++) {
-            const std::string ts = std::to_string(t);
-            queries.push_back({"pa" + ts, coef["pa" + ts]->at(), 0});
-            queries.push_back({"pa" + ts, coef["pa" + ts]->at(), -1});
-            queries.push_back({"ps" + ts, coef["ps" + ts]->at(), 0});
-            queries.push_back({"zl" + ts, coef["zl" + ts]->at(), 0});
-            queries.push_back({"zl" + ts, coef["zl" + ts]->at(), 1});
-        }
-        for (size_t j = 0; j < pieces; j++) queries.push_back({"h" + std::to_string(j), h->at(j * n), 0});
-        queries.push_back({"rnd", rnd->at(), 0});
+        const std::vector<Query> queries = this->queries();
         {
             const size_t m = queries.size();
             std::vector<const void*> polys(m);
@@ -747,35 +830,75 @@ public:
         ctx.check(h2b_ctx_side_join(c));
         if (have_main) lincomb({tmp[2]->at(), tmp_side[2]->at()}, {HostFr::one(), HostFr::one()}, tmp[2]);
         else ctx.check(h2b_poly_copy_dev(c, tmp[2]->at(), tmp_side[2]->at(), n));
-        commit({{H2B_BASIS_MONOMIAL, tmp[2]->at()}}, true);
+        commit({{H2B_BASIS_MONOMIAL, ColRef{tmp[2], 0}}}, true);
         const Fr u_ch = tr.squeeze();
         // final quotient: W' = L / (X - u) (the remainder is dropped by kate_division)
         ctx.check(h2b_kate_division_dev(c, tmp[2]->at(), n, u_ch.data(), tmp[3]->at()));
         ctx.check(h2b_poly_copy_dev(c, tmp[3]->at(n - 1), zero->at(), 1));
-        commit({{H2B_BASIS_MONOMIAL, tmp[3]->at()}}, false);
+        commit({{H2B_BASIS_MONOMIAL, ColRef{tmp[3], 0}}}, false);
         return res;
     }
+    // commitments per proof, in commit order: advice | permuted pairs | product columns + random | h pieces | two openings
+    size_t commitments_per_proof() const {
+        return cs.adv_names.size() + 2 * cs.n_lookups + (cs.n_sets + cs.n_lookups + 1) + (cs.degree - 1) + 2;
+    }
+    // the evaluations of a proof, in the order they enter the transcript: (column, rotation) and the coefficients evaluated
+    struct Query {
+        std::string name;
+        const void* ptr;
+        int rot;
+    };
+    std::vector<Query> queries() const {
+        const int last = -int(cs.bf + 1);
+        std::vector<Query> q;
+        auto add = [&](const std::string& nm, int r) { q.push_back({nm, coef.at(nm)->at(), r}); };
+        for (size_t j = 0; j < cs.A; j++)
+            for (int r : {0, 1, 2, 3}) add("a" + std::to_string(j), r);
+        for (size_t t = 0; t < cs.L; t++) add("l" + std::to_string(t), 0);
+        for (auto& nm : cs.fixed_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (auto& nm : cs.sigma_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (size_t s = 0; s < cs.n_sets; s++) {  // every set at x and omega x; all but the last one also at omega^last x
+            const std::string nm = "zp" + std::to_string(s);
+            add(nm, 0);
+            add(nm, 1);
+            if (s + 1 < cs.n_sets) add(nm, last);
+        }
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const std::string ts = std::to_string(t);
+            add("pa" + ts, 0);
+            add("pa" + ts, -1);
+            add("ps" + ts, 0);
+            add("zl" + ts, 0);
+            add("zl" + ts, 1);
+        }
+        for (size_t j = 0; j + 1 < cs.degree; j++) q.push_back({"h" + std::to_string(j), h->at(j * cs.n), 0});
+        q.push_back({"rnd", rnd->at(), 0});
+        return q;
+    }
 
-    // MockProver::verify for this circuit (ProverSession.check of halo2-lib_b200/prover.py, same result): the witness as for
-    // create_proof, the same assignment, no blinding, no random polynomial, no transcript; rows >= u read as 0.  Every report
-    // comes down in one copy; a bad index of the halo2-base form throws H2B_ERR_ARG.
+    // MockProver::verify for this circuit: the witness as for create_proof, the same assignment, no blinding, no random
+    // polynomial, no transcript; rows >= u read as 0.  Every report comes down in one copy; a bad index of the halo2-base form
+    // throws H2B_ERR_ARG.
     CheckReport check(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
                       const AssignedWitness* form = nullptr, size_t max_report = 16) {
+        return check(view(witness, break_points, lookup_cells, form, "check"), max_report);
+    }
+    CheckReport check(const WitnessView& wit, size_t max_report = 16) {
         const uint32_t k = cs.k;
         const size_t n = cs.n, u = cs.u, A = cs.A, L = cs.L;
         h2b_ctx* c = ctx.raw();
-        check_form(lookup_cells, form, "check");
+        check_inputs(wit, "check");
         if (max_report < 1 || max_report > H2B_CHECK_MAX_REPORT) throw Error(H2B_ERR_ARG, "check: max_report out of range");
         cs.prepare_check();
         size_t h2d = 0;
-        assign_witness(witness, break_points, lookup_cells, form, nullptr, h2d);
+        assign_witness(wit, nullptr, h2d);
         Poly* zero_rows = grown(check_zero, n - u);  // zero-filled, never written
         for (auto& nm : cs.adv_names) ctx.check(h2b_poly_copy_dev(c, lagr[nm].ptr(u), zero_rows->at(), n - u));
         // report block: element 0 = the witness-form verdict words, then max_report + 1 words per gate, lookup, permutation column
         const size_t W = max_report + 1, npc = cs.perm_cols.size(), n_items = A + cs.n_lookups + npc, elems = 1 + (n_items * W + 3) / 4;
         Poly* rep = grown(check_rep, elems);
         auto at = [&](size_t i) { return static_cast<char*>(rep->at(1)) + 8 * W * i; };
-        if (form) ctx.check(h2b_poly_copy_dev(c, rep->at(), d_out->at(48), 1));
+        if (wit.assigned_form()) ctx.check(h2b_poly_copy_dev(c, rep->at(), d_out->at(48), 1));
         for (size_t j = 0; j < A; j++) {
             const h2b_graph g = bind(cs.check_ev, cs.check_result, {cs.lagr.at("q" + std::to_string(j))->at()}, {lagr["a" + std::to_string(j)].ptr()},
                                      Challenges{});
@@ -794,8 +917,8 @@ public:
         check_copies_dev(ctx, cols, cs.check_map->at(), k, max_report, at(A + cs.n_lookups));
         const std::vector<Fr> raw = rep->download(0, elems);
         const uint64_t* w = raw[0].data();
-        if (form) {
-            const uint32_t rat_bad = uint32_t(w[0]), lk_bad = (L && !form->lookup_index.empty()) ? uint32_t(w[0] >> 32) : 0;
+        if (wit.assigned_form()) {
+            const uint32_t rat_bad = uint32_t(w[0]), lk_bad = L && wit.lookup_index ? uint32_t(w[0] >> 32) : 0;
             if (rat_bad || lk_bad) witness_error(rat_bad, lk_bad, "check");
         }
         CheckReport out;
@@ -808,12 +931,46 @@ public:
         return out;
     }
 
+    // a session column by name, for tests: "lagr" / "coef" / "ext" by column name, "h" (the quotient: values on the extended
+    // coset, then the coefficients of its pieces) and "check_report" (the report block of the last check)
+    NamedColumn column(const std::string& table, const std::string& name) const {
+        if (table == "lagr" && lagr.count(name)) return {lagr.at(name), cs.n};
+        if (table == "coef" && coef.count(name)) return {{coef.at(name), 0}, cs.n};
+        if (table == "ext" && ext.count(name)) return {{ext.at(name), 0}, ext.at(name)->len()};
+        if (table == "h") return {{h, 0}, h->len()};
+        if (table == "check_report" && check_rep) return {{check_rep.get(), 0}, check_rep->len()};
+        throw Error(H2B_ERR_ARG, "ProverSession: no column " + table + " " + name);
+    }
+
 private:
-    static void check_form(const std::vector<Fr>& lookup_cells, const AssignedWitness* form, const std::string& who) {
-        if (form && !lookup_cells.empty() && !form->lookup_index.empty())
-            throw Error(H2B_ERR_ARG, who + ": pass the looked-up cells either as values or as indices");
-        if (form && form->rational_index.size() != form->rational_den.size())
-            throw Error(H2B_ERR_ARG, who + ": rational_index and rational_den differ in length");
+    static WitnessView view(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
+                            const AssignedWitness* form, const std::string& who) {
+        WitnessView w;
+        w.cells = witness.data();
+        w.n_cells = witness.size();
+        w.break_points = break_points.empty() ? nullptr : break_points.data();
+        w.n_break_points = break_points.size();
+        w.lookup_cells = lookup_cells.data();
+        w.n_lookup = lookup_cells.size();
+        if (form) {
+            if (form->rational_index.size() != form->rational_den.size())
+                throw Error(H2B_ERR_ARG, who + ": rational_index and rational_den differ in length");
+            w.rational_index = form->rational_index.data();
+            w.rational_den = form->rational_den.data();
+            w.n_rational = form->rational_index.size();
+            if (!form->lookup_index.empty()) {
+                if (!lookup_cells.empty()) throw Error(H2B_ERR_ARG, who + ": pass the looked-up cells either as values or as indices");
+                w.lookup_cells = nullptr;
+                w.lookup_index = form->lookup_index.data();
+                w.n_lookup = form->lookup_index.size();
+            }
+        }
+        return w;
+    }
+    static void check_inputs(const WitnessView& w, const std::string& who) {
+        if (w.lookup_cells && w.lookup_index) throw Error(H2B_ERR_ARG, who + ": pass the looked-up cells either as values or as indices");
+        if (w.n_rational && !(w.rational_index && w.rational_den))
+            throw Error(H2B_ERR_ARG, who + ": n_rational > 0 needs rational_index and rational_den");
     }
     [[noreturn]] static void witness_error(uint32_t rat_bad, uint32_t lk_bad, const std::string& who) {
         std::string why;
@@ -825,42 +982,38 @@ private:
     // phase 0 up to the advice columns in adv_block (what create_proof and check share): witness, Rational pairs and lookup
     // indices or looked-up values up, Rational cells -> n * d^-1, the assignment; with the halo2-base form the verdict words
     // land in element 48 of d_out.  random_poly != nullptr: it goes up on the side queue, beside the assignment.
-    void assign_witness(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
-                        const AssignedWitness* form, const std::vector<Fr>* random_poly, size_t& h2d_bytes) {
+    void assign_witness(const WitnessView& w, const Fr* random_poly, size_t& h2d_bytes) {
         const uint32_t k = cs.k;
-        const size_t n = cs.n, A = cs.A, L = cs.L;
+        const size_t n = cs.n, A = cs.A, L = cs.L, R = w.n_rational;
         h2b_ctx* c = ctx.raw();
-        const bool lk_indexed = form && L && !form->lookup_index.empty();
-        v->upload(witness.data(), witness.size());
-        h2d_bytes += witness.size() * 32;
-        const size_t R = form ? form->rational_index.size() : 0;
+        const bool lk_indexed = L && w.lookup_index;
+        v->upload(w.cells, w.n_cells);
+        h2d_bytes += w.n_cells * 32;
         if (R) {
-            grown(rat_den, R)->upload(form->rational_den.data(), R);
+            grown(rat_den, R)->upload(w.rational_den, R);
             h2d_bytes += R * 32;
-            upload_u64(rat_idx, form->rational_index, h2d_bytes);
+            upload_u64(rat_idx, w.rational_index, R, h2d_bytes);
         }
         if (lk_indexed) {
-            upload_u64(lk_idx, form->lookup_index, h2d_bytes);
+            upload_u64(lk_idx, w.lookup_index, w.n_lookup, h2d_bytes);
         } else if (L) {
-            lkv->upload(lookup_cells.data(), lookup_cells.size());
-            h2d_bytes += lookup_cells.size() * 32;
+            lkv->upload(w.lookup_cells, w.n_lookup);
+            h2d_bytes += w.n_lookup * 32;
         }
         if (random_poly) {
             ctx.check(h2b_ctx_side_begin(c));
-            rnd->upload_async(random_poly->data(), n);
+            rnd->upload_async(random_poly, n);
             ctx.check(h2b_ctx_side_end(c));
             h2d_bytes += n * 32;
         }
         uint32_t* d_verdict = static_cast<uint32_t*>(d_out->at(48));
-        if (form)  // zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
-            ctx.check(h2b_apply_rational_dev(c, v->at(), witness.size(), R ? rat_idx->at() : nullptr, R ? rat_den->at() : nullptr, R, d_verdict));
-        ctx.check(h2b_assign_columns_dev(c, v->at(), witness.size(), break_points.empty() ? nullptr : break_points.data(), break_points.size(), k, A,
-                                         adv_block->at()));
+        if (w.assigned_form())  // zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
+            ctx.check(h2b_apply_rational_dev(c, v->at(), w.n_cells, R ? rat_idx->at() : nullptr, R ? rat_den->at() : nullptr, R, d_verdict));
+        ctx.check(h2b_assign_columns_dev(c, v->at(), w.n_cells, w.n_break_points ? w.break_points : nullptr, w.n_break_points, k, A, adv_block->at()));
         if (lk_indexed)
-            ctx.check(h2b_assign_lookups_indexed_dev(c, v->at(), witness.size(), lk_idx->at(), form->lookup_index.size(), k, L, adv_block->at(A * n),
-                                                     d_verdict + 1));
+            ctx.check(h2b_assign_lookups_indexed_dev(c, v->at(), w.n_cells, lk_idx->at(), w.n_lookup, k, L, adv_block->at(A * n), d_verdict + 1));
         else if (L)
-            ctx.check(h2b_assign_lookups_dev(c, lkv->at(), lookup_cells.size(), k, L, adv_block->at(A * n)));
+            ctx.check(h2b_assign_lookups_dev(c, lkv->at(), w.n_lookup, k, L, adv_block->at(A * n)));
     }
     Poly* own(size_t m) {
         owned.push_back(std::make_unique<Poly>(ctx, m));
@@ -871,11 +1024,18 @@ private:
         if (!p || p->len() < m) p = std::make_unique<Poly>(ctx, std::max<size_t>(m, 1));
         return p.get();
     }
-    void upload_u64(PolyPtr& p, const std::vector<uint64_t>& words, size_t& h2d_bytes) {
-        std::vector<Fr> packed((words.size() + 3) / 4, Fr{});
-        if (!words.empty()) std::memcpy(packed[0].data(), words.data(), words.size() * 8);
-        grown(p, packed.size())->upload(packed.data(), packed.size());
-        h2d_bytes += words.size() * 8;
+    // count uint64 words: whole 32-byte elements straight from the caller's array, the last 1..3 words through a zero-padded
+    // element (nothing past the end of the caller's array is read)
+    void upload_u64(PolyPtr& p, const uint64_t* words, size_t count, size_t& h2d_bytes) {
+        Poly* d = grown(p, (count + 3) / 4);
+        const size_t full = count / 4;
+        if (full) d->upload(reinterpret_cast<const Fr*>(words), full);
+        if (count % 4) {
+            Fr tail{};
+            std::memcpy(tail.data(), words + 4 * full, 8 * (count % 4));
+            d->upload(&tail, 1, full);
+        }
+        h2d_bytes += count * 8;
     }
     // the arrays an h2b_graph points to live in `hold` until the next bind()
     h2b_graph bind(const GraphEvaluator& ev, ValueSource result, const std::vector<const void*>& fixed, const std::vector<const void*>& advice,
@@ -906,6 +1066,8 @@ private:
     const Context& ctx;
     const ParamsKZG& params;
     const ProverCircuit& cs;
+    size_t shard_begin = 0, n_loc;  // shard()
+    AllReduce allreduce;
     std::vector<PolyPtr> owned;
     PolyPtr v, lkv, adv_block;
     PolyPtr rat_den, rat_idx, lk_idx;  // the halo2-base witness form

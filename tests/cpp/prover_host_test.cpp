@@ -1,4 +1,5 @@
-// CPU-only checks of the host pieces of include/h2b200_prover.hpp (Blake2b transcript, 254-bit host arithmetic): prints
+// CPU-only checks of the host pieces of include/h2b200_prover.hpp (Blake2b transcript, 254-bit host arithmetic, the
+// normalisation of commitments): prints
 // values that tests/test_cpp_mirror.py recomputes with hashlib and Python integers.
 #include <cstdio>
 
@@ -48,5 +49,8 @@ int main() {
     const G1 pt{c1, c2, c3}, nz = g1_normalize_host(pt), id = g1_normalize_host(G1{c1, c2, Fq{0, 0, 0, 0}});
     hex("normalize", &nz, 96);
     hex("normalize_identity", &id, 96);
+    G1 batch[3] = {pt, G1{c2, c3, Fq{0, 0, 0, 0}}, G1{c3, c1, c2}};  // one inversion for the batch, the identity in the middle
+    g1_normalize_host_batch(batch, 3);
+    for (int i = 0; i < 3; i++) hex(("batch" + std::to_string(i)).c_str(), &batch[i], 96);
     return 0;
 }

@@ -34,7 +34,8 @@ PROVER_HOST_EXE = os.path.join(ROOT, "build", "prover_host_test")
 
 def test_cpp_prover_host_side_matches_python_integers():
     """the host pieces of include/h2b200_prover.hpp — Blake2b-512, the transcript's challenge (64 bytes mod r), the 254-bit
-    Montgomery arithmetic used for rotations and powers of challenges — against hashlib and plain Python integers"""
+    Montgomery arithmetic used for rotations and powers of challenges, the normalisation of commitments — against hashlib and
+    plain Python integers"""
     import hashlib
     os.makedirs(os.path.dirname(PROVER_HOST_EXE), exist_ok=True)
     libdir = os.path.join(ROOT, "halo2-lib_b200")
@@ -67,6 +68,10 @@ def test_cpp_prover_host_side_matches_python_integers():
     assert np.array_equal(g1_normalize_host(pt), limbs(out["normalize"]))
     pt0 = pt.copy(); pt0[8:] = 0
     assert not limbs(out["normalize_identity"]).any() and not g1_normalize_host(pt0).any()
+    # a batch with one inversion (the identity in the middle): each point as alone
+    pt2 = np.concatenate([limbs(out["squeeze3"]), limbs(out["squeeze1"]), limbs(out["squeeze2"])])
+    assert np.array_equal(limbs(out["batch0"]), g1_normalize_host(pt)) and not limbs(out["batch1"]).any()
+    assert np.array_equal(limbs(out["batch2"]), g1_normalize_host(pt2))
 
 
 def test_cpp_prover_mirror_compiles_and_links():

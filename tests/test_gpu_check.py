@@ -167,7 +167,7 @@ def test_more_failures_than_max_report(ctx, h2b):
     raw = []
     for _ in range(2):
         _check(sess, inst, V, max_report=7)
-        raw.append(sess._grown("check_report", 1).download().tobytes())
+        raw.append(sess.check_report.download().tobytes())
     assert raw[0] == raw[1]
     sess.free(); cs.free(); params.close()
 
@@ -239,7 +239,10 @@ def test_argument_errors_leave_the_session_usable(ctx, h2b):
     buf = torch.zeros((4 * n * 4,), dtype=torch.int64, device="cuda")
     p = buf.data_ptr()
     col = vp(cs.lagr["table"].ptr)
-    g, res, smap = cs.check_state()
+    g = h2b.GraphEvaluator()  # the vertical gate q (a0 + a1 a2 - a3) on fixed slot 0 / advice slot 0
+    a = lambda r: ("advice", 0, r)
+    res = g.add_expression(("product", ("fixed", 0, 0), ("sum", ("sum", a(0), ("product", a(1), a(2))), ("negated", a(3)))))
+    smap = cs.sigma_map
     bg = h2b.BoundGraph(g, res, fixed=[cs.lagr["q0"].ptr], advice=[sess.lagr["a0"].ptr])
     bad_bg = h2b.BoundGraph(g, res, fixed=[cs.lagr["q0"].ptr], advice=[sess.lagr["a0"].ptr])
     bad_bg.struct.n_calculations = 65

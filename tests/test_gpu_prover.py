@@ -167,10 +167,10 @@ def test_resident_prover_reproduces_the_committed_golden_proof(ctx, h2b):
 
 @pytest.mark.parametrize("k,A,L,sel", [(8, 1, 0, True), (8, 1, 0, False), (9, 7, 2, True)])
 def test_cpp_prover_matches_python(ctx, h2b, k, A, L, sel, tmp_path):
-    """the compiled host side (include/h2b200_prover.hpp: ProverCircuit + ProverSession::create_proof, Blake2b transcript,
-    host-side 254-bit arithmetic) drives the C ABI to the SAME BYTES as halo2-lib_b200/prover.py for the same instance,
-    SRS, random polynomial and blinding rows: commitments, evaluations and challenges are compared byte for byte.  The
-    Python proof is the one the protocol-level checks above run on."""
+    """the two front ends of the compiled prover pass identical inputs: a C++ program (include/h2b200_prover.hpp over
+    std::vector inputs and its own Context / ParamsKZG) and halo2-lib_b200/prover.py (the library's binding, host pointers)
+    give the SAME BYTES for the same instance, SRS, random polynomial and blinding rows: commitments, evaluations and
+    challenges are compared byte for byte.  The Python proof is the one the protocol-level checks above run on."""
     import os, subprocess
     rng, params, cs, sess, inst, bases = _setup(ctx, h2b, k, 3500 + k + 10 * A, A, L, sel)
     n = 1 << k
@@ -207,6 +207,28 @@ def test_cpp_prover_matches_python(ctx, h2b, k, A, L, sel, tmp_path):
     want = [res["challenges"][c] for c in ("theta", "beta", "gamma", "y", "x")]
     assert [pc.fr(c) for c in chal] == want
     sess.free(); cs.free(); params.close()
+
+
+def test_shard_over_the_whole_range_matches_the_unsharded_proof(ctx, h2b):
+    """the multi-GPU path on one GPU: shard(0, n, allreduce) with a callback that records its calls and leaves the points as
+    they are.  It must be called once per batched MSM (at most 16 commitments; 17 advice columns make phase 0 two batches)
+    with that batch's size, and the proof must be the same bytes as an unsharded one."""
+    k, A, L = 8, 15, 2
+    rng, params, cs, sess, inst, bases = _setup(ctx, h2b, k, 3900, A, L, True)
+    rnd = mont(rand_ints(rng, 1 << k, R), R)
+    want = _prove(sess, inst, rnd)
+    calls = []
+    sharded = h2b.ProverSession(ctx, params, cs)
+    sharded.shard(0, 1 << k, lambda ptr, m: calls.append((ptr, m)))
+    got = _prove(sharded, inst, rnd)
+    nlk = cs.n_lookups
+    assert [m for _, m in calls] == [16, A + L - 16, 2 * nlk, cs.n_sets + nlk + 1, cs.degree - 1, 1, 1]
+    assert calls[0][0] and len(set(p for p, _ in calls)) == 1
+    assert [c.tobytes() for c in got["commitments"]] == [c.tobytes() for c in want["commitments"]]
+    assert [(q, v.tobytes()) for q, v in got["evals"].items()] == [(q, v.tobytes()) for q, v in want["evals"].items()]
+    assert got["challenges"] == want["challenges"]
+    assert (got["h2d_bytes"], got["d2h_bytes"]) == (want["h2d_bytes"], want["d2h_bytes"])
+    sharded.free(); sess.free(); cs.free(); params.close()
 
 
 def test_product_columns_vs_integer_recurrence(ctx, h2b):
