@@ -132,6 +132,11 @@ SIGNATURES = {
     "h2b_check_lookup_dev": (_int, [_vp, _vp, _vp, _u32, _sz, _sz, _vp]),
     "h2b_permutation_decode_dev": (_int, [_vp, _vpp, _sz, _u32, _vp, _sz, _vp]),
     "h2b_check_copies_dev": (_int, [_vp, _vpp, _vp, _sz, _u32, _sz, _vp]),
+    "h2b_mock_selectors_dev": (_int, [_vp, _vp, _sz, _vp, _sz, _u32, _sz, _vp]),
+    "h2b_mock_lookup_selector_dev": (_int, [_vp, _vp, _sz, _sz, _sz, _u32, _vp, _vp]),
+    "h2b_check_equalities_dev": (_int, [_vp, _vp, _sz, _vp, _sz, _sz, _vp, _vp]),
+    "h2b_check_constants_dev": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp, _vp]),
+    "h2b_count_distinct_dev": (_int, [_vp, _vp, _sz, _vp]),
     "h2b_divide_by_vanishing_poly": (_int, [_vp, _vp, _u32, _u32]),
     "h2b_divide_by_vanishing_poly_dev": (_int, [_vp, _vp, _u32, _u32]),
     "h2b_eval_polynomial": (_int, [_vp, _vp, _sz, _vp, _vp]),
@@ -166,6 +171,15 @@ class Witness(C.Structure):
     ]
 
 
+class BuilderView(C.Structure):
+    """h2b::BuilderView (include/h2b200_mock.hpp): a halo2-base builder in its keygen form, host pointers + counts"""
+    _fields_ = [
+        ("cells", _vp), ("n_cells", _sz), ("rational_index", _vp), ("rational_den", _vp), ("n_rational", _sz),
+        ("selectors", _vp), ("advice_equalities", _vp), ("n_advice_equalities", _sz),
+        ("constants", _vp), ("constant_index", _vp), ("n_constant_equalities", _sz), ("lookup_index", _vp), ("n_lookup", _sz),
+    ]
+
+
 # callbacks of the compiled prover (first argument: the `user` pointer); 0 = success, anything else stops the proof
 BLIND_FN = C.CFUNCTYPE(_int, _vp, _sz, _vp)             # (rows, out: rows x 4 limbs)
 ALLREDUCE_FN = C.CFUNCTYPE(_int, _vp, _vp, _sz)         # (device pointer of the m partial commitments, m)
@@ -185,6 +199,10 @@ PROVER_SIGNATURES = {
     "h2bp_session_shard": (_int, [_vp, _sz, _sz, ALLREDUCE_FN, _vp]),
     "h2bp_prove": (_int, [_vp, _witp, _vp, BLIND_FN, _vp, COMMIT_FN, _vp, _vp, _vp, _vp, _vp]),
     "h2bp_check": (_int, [_vp, _witp, _sz, _vp]),
+    "h2bp_mock_create": (_int, [_vp, _u32, _sz, _sz, _int, _u32, _sz, C.POINTER(_vp), _u64s]),
+    "h2bp_mock_free": (None, [_vp]),
+    "h2bp_mock_column": (_int, [_vp, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
+    "h2bp_mock_run": (_int, [_vp, C.POINTER(BuilderView), _sz, _vp, _u64s, _vp, _vp]),
 }
 
 

@@ -149,15 +149,8 @@ __global__ void __launch_bounds__(128) k_eval_rational(const uint64_t* __restric
     (Fr::load_nc(num + 4 * (size_t)i) * d).store(out + 4 * (size_t)i);
 }
 
-void assign_columns_run(h2b_ctx* ctx, const void* d_vcol, size_t N, const uint64_t* break_points, size_t nbp,
-                        uint32_t k, size_t ncols, void* d_cols) {
-    H2B_REQUIRE(k <= 28, "assign: k out of range");
-    const size_t rows = (size_t)1 << k;
-    if (ncols == 0) {
-        // single_phase.rs:279-286: "Trying to assign threads in a phase with no columns"
-        if (N != 0) throw StatusError{H2B_ERR_LAYOUT, "assign_witnesses: cells present but the phase has no advice columns"};
-        return;
-    }
+// the spans of the ncols columns the walk fills: column c holds V[s_c .. s_c + len_c); columns the walk does not reach are empty
+static std::vector<ColSpan> column_spans(size_t N, const uint64_t* break_points, size_t nbp, size_t rows, size_t ncols) {
     std::vector<ColSpan> spans(ncols, ColSpan{0, 0});
     size_t s = 0, c = 0, bpi = 0;
     size_t rem = N;
@@ -183,6 +176,19 @@ void assign_columns_run(h2b_ctx* ctx, const void* d_vcol, size_t N, const uint64
             rem = 0;
         }
     }
+    return spans;
+}
+
+void assign_columns_run(h2b_ctx* ctx, const void* d_vcol, size_t N, const uint64_t* break_points, size_t nbp,
+                        uint32_t k, size_t ncols, void* d_cols) {
+    H2B_REQUIRE(k <= 28, "assign: k out of range");
+    const size_t rows = (size_t)1 << k;
+    if (ncols == 0) {
+        // single_phase.rs:279-286: "Trying to assign threads in a phase with no columns"
+        if (N != 0) throw StatusError{H2B_ERR_LAYOUT, "assign_witnesses: cells present but the phase has no advice columns"};
+        return;
+    }
+    const std::vector<ColSpan> spans = column_spans(N, break_points, nbp, rows, ncols);
     size_t total = ncols * rows * 2;
     if (ncols <= 64) {  // the usual case: spans travel as a kernel argument, the call stays asynchronous
         ColSpans64 sv;
@@ -197,6 +203,66 @@ void assign_columns_run(h2b_ctx* ctx, const void* d_vcol, size_t N, const uint64
     memcpy(h_spans, spans.data(), ncols * sizeof(ColSpan));
     H2B_CUDA(cudaMemcpyAsync(d_spans, h_spans, ncols * sizeof(ColSpan), cudaMemcpyHostToDevice, ctx->stream));
     H2B_LAUNCH(ctx, k_assign_columns, ceil_div(total, 256), 256, 0, (const uint4*)d_vcol, d_spans, k, (u32)ncols, (uint4*)d_cols);
+}
+
+// MockProver's selector columns: q_c[r] = selector[s_c + r] for r < sel_len_c, zero elsewhere.  A column the walk left at a break
+// has sel_len = len - 1: the break cell's selector is enabled at row 0 of the next column only (single_phase.rs:229-257 enable
+// after the break), while the cell itself sits in both.
+struct SelSpan {
+    uint64_t start;
+    uint64_t sel_len;
+};
+__global__ void __launch_bounds__(256) k_mock_selectors(const uint8_t* __restrict__ sel, const SelSpan* __restrict__ spans, u32 rows_log,
+                                                        u32 ncols, uint64_t* __restrict__ q) {
+    const size_t cell = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (cell >= ((size_t)ncols << rows_log)) return;
+    const u32 c = (u32)(cell >> rows_log);
+    const size_t r = cell & (((size_t)1 << rows_log) - 1);
+    const SelSpan sp = spans[c];
+    const bool on = r < sp.sel_len && __ldg(sel + sp.start + r) != 0;
+    (on ? Fr::one() : Fr::zero()).store(q + 4 * cell);
+}
+
+// q_lookup[index[i]] = 1 (one gate column: the raw row of a virtual cell is its index).  bit 0 of *status: an index >= N;
+// bit 1: an index >= max_rows (the row is not usable)
+__global__ void __launch_bounds__(256) k_mock_lookup_selector(const uint64_t* __restrict__ index, size_t m, uint64_t N, uint64_t max_rows,
+                                                              uint64_t* __restrict__ q, u32* __restrict__ status) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint64_t idx = __ldg(index + i);
+    const u32 bad = (idx < N ? 0u : 1u) | (idx < max_rows ? 0u : 2u);
+    if (bad) {
+        atomicOr(status, bad);
+        return;
+    }
+    Fr::one().store(q + 4 * idx);
+}
+
+void mock_selectors_run(h2b_ctx* ctx, const void* d_selectors, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t ncols,
+                        void* d_q) {
+    H2B_REQUIRE(k <= 28, "mock_selectors: k out of range");
+    H2B_REQUIRE(ncols >= 1, "mock_selectors: no gate columns");
+    const size_t rows = (size_t)1 << k;
+    const std::vector<ColSpan> spans = column_spans(N, break_points, nbp, rows, ncols);
+    std::vector<SelSpan> sel(ncols);
+    for (size_t c = 0; c < ncols; c++) {
+        const bool broke = c + 1 < ncols && spans[c + 1].len > 0;
+        sel[c] = SelSpan{spans[c].start, broke ? spans[c].len - 1 : spans[c].len};
+    }
+    SelSpan* d_spans = (SelSpan*)ctx->get(WS_MISC, ncols * sizeof(SelSpan));
+    H2B_CUDA(cudaMemcpyAsync(d_spans, sel.data(), ncols * sizeof(SelSpan), cudaMemcpyHostToDevice, ctx->stream));  // pageable: staged now
+    H2B_LAUNCH(ctx, k_mock_selectors, ceil_div(ncols * rows, 256), 256, 0, (const uint8_t*)d_selectors, (const SelSpan*)d_spans, k, (u32)ncols,
+               (uint64_t*)d_q);
+}
+
+void mock_lookup_selector_run(h2b_ctx* ctx, const uint64_t* d_index, size_t m, size_t N, size_t max_rows, uint32_t k, void* d_q,
+                              uint32_t* d_status) {
+    H2B_REQUIRE(k <= 28, "mock_lookup_selector: k out of range");
+    H2B_REQUIRE(max_rows <= ((size_t)1 << k), "mock_lookup_selector: max_rows > 2^k");
+    H2B_CUDA(cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+    H2B_CUDA(cudaMemsetAsync(d_q, 0, ((size_t)1 << k) * 32, ctx->stream));
+    if (m == 0) return;
+    H2B_LAUNCH(ctx, k_mock_lookup_selector, ceil_div(m, 256), 256, 0, d_index, m, (uint64_t)N, (uint64_t)max_rows, (uint64_t*)d_q, d_status);
 }
 
 // d_recs: N staging records of 72 bytes.  d_values (N x 32 B) receives what the prover's `batch_invert_assigned` yields:

@@ -1391,6 +1391,42 @@ int h2b_check_copies_dev(h2b_ctx* ctx, const void* const* d_columns, const void*
     });
 }
 
+// ------------------------------------------------------------------------------------------------ MockProver of a builder
+int h2b_mock_selectors_dev(h2b_ctx* ctx, const void* d_selectors, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t ncols,
+                           void* d_q) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_selectors || N == 0) && (break_points || nbp == 0) && d_q, "mock_selectors: null pointer");
+        mock_selectors_run(ctx, d_selectors, N, break_points, nbp, k, ncols, d_q);
+    });
+}
+int h2b_mock_lookup_selector_dev(h2b_ctx* ctx, const void* d_index, size_t m, size_t N, size_t max_rows, uint32_t k, void* d_q,
+                                 uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_index || m == 0) && d_q && d_status, "mock_lookup_selector: null pointer");
+        mock_lookup_selector_run(ctx, (const uint64_t*)d_index, m, N, max_rows, k, d_q, d_status);
+    });
+}
+int h2b_check_equalities_dev(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_pairs, size_t m, size_t max_report, void* d_report,
+                             uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_cells || N == 0) && (d_pairs || m == 0) && d_report && d_status, "check_equalities: null pointer");
+        check_equalities_run(ctx, d_cells, N, (const uint64_t*)d_pairs, m, max_report, d_report, d_status);
+    });
+}
+int h2b_check_constants_dev(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_consts, const void* d_index, size_t m,
+                            size_t max_report, void* d_report, uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_cells || N == 0) && ((d_consts && d_index) || m == 0) && d_report && d_status, "check_constants: null pointer");
+        check_constants_run(ctx, d_cells, N, d_consts, (const uint64_t*)d_index, m, max_report, d_report, d_status);
+    });
+}
+int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_values || m == 0) && d_count, "count_distinct: null pointer");
+        count_distinct_run(ctx, d_values, m, d_count);
+    });
+}
+
 // ------------------------------------------------------------------------------------------------ opening arithmetic
 int h2b_eval_polynomial_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n, const uint64_t x[4], uint64_t out[4]) {
     return guarded(ctx, [&] {

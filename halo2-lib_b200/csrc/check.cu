@@ -9,7 +9,9 @@
 //   sigma:   an entry v = delta^c' omega^r' is decoded by v^n = delta^(c' n) (omega^n = 1: k squarings, matched against
 //            delta^(c n) for c < n_cols) and w = v delta^-c' = omega^r', found in an open-addressing table of the omega
 //            powers (u32 row slots, full-value compare, so the answer does not depend on the insertion order);
-//   copies:  value(c, r) against value(map(c, r)), one thread per cell.
+//   copies:  value(c, r) against value(map(c, r)), one thread per cell;
+//   equalities of a builder (MockProver, include/h2b200_mock.hpp): value(a) against value(b), value(cell) against its
+//            constant, one thread per equality; the distinct constants counted as runs of the sorted column.
 #include "h2b_internal.cuh"
 #include "field.cuh"
 #include "graph.cuh"
@@ -319,6 +321,96 @@ void check_copies_run(h2b_ctx* ctx, const void* const* d_columns, const void* d_
     uint8_t* flags = flags_workspace(ctx, n_cols, (u32)n, &counts);
     H2B_LAUNCH(ctx, k_check_copies, dim3(ceil_div(n, 256), (unsigned)n_cols), 256, 0, cols, (const u32*)d_map, (u32)n_cols, k, flags);
     report_run(ctx, flags, n_cols, (u32)n, max_report, d_reports, counts);
+}
+
+// ------------------------------------------------------------------------------------------ equalities of the builder
+// halo2-base's copy manager as pairs of virtual-column cells: advice_equalities (a, b) and constant_equalities (c, i).  One
+// thread per equality; an index >= N is not read, flags its equality and sets bit 0 of *status.
+__global__ void __launch_bounds__(256) k_check_equalities(const uint64_t* __restrict__ cells, uint64_t N, const uint64_t* __restrict__ pairs,
+                                                          u32 m, uint8_t* __restrict__ flags, u32* __restrict__ status) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint64_t a = __ldg(pairs + 2 * (size_t)i), b = __ldg(pairs + 2 * (size_t)i + 1);
+    bool bad = true;
+    if (a < N && b < N)
+        bad = !(Fr::load_nc(cells + 4 * a) - Fr::load_nc(cells + 4 * b)).is_zero();
+    else
+        atomicOr(status, 1u);
+    flags[i] = bad ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(256) k_check_constants(const uint64_t* __restrict__ cells, uint64_t N, const uint64_t* __restrict__ consts,
+                                                         const uint64_t* __restrict__ index, u32 m, uint8_t* __restrict__ flags,
+                                                         u32* __restrict__ status) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint64_t a = __ldg(index + i);
+    bool bad = true;
+    if (a < N)
+        bad = !(Fr::load_nc(cells + 4 * a) - Fr::load_nc(consts + 4 * (size_t)i)).is_zero();
+    else
+        atomicOr(status, 1u);
+    flags[i] = bad ? 1 : 0;
+}
+
+// runs of equal values in a column of canonical values sorted ascending
+__global__ void __launch_bounds__(256) k_count_runs(const uint64_t* __restrict__ canon, u32 m, u32* __restrict__ count) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    bool head = false;
+    if (i < m) {
+        head = i == 0;
+        for (int j = 0; j < 4 && !head; j++) head = __ldg(canon + 4 * (size_t)i + j) != __ldg(canon + 4 * (size_t)i - 4 + j);
+    }
+    const u32 c = __popc(__ballot_sync(0xffffffffu, head));
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);
+}
+
+static void check_pairs_common(size_t m, size_t max_report) {
+    H2B_REQUIRE(max_report >= 1 && max_report <= H2B_CHECK_MAX_REPORT, "check: max_report must be in 1..H2B_CHECK_MAX_REPORT");
+    H2B_REQUIRE(m < ((size_t)1 << 32), "check: at most 2^32 - 1 equalities per call");
+}
+
+void check_equalities_run(h2b_ctx* ctx, const void* d_cells, size_t N, const uint64_t* d_pairs, size_t m, size_t max_report, void* d_report,
+                          uint32_t* d_status) {
+    check_pairs_common(m, max_report);
+    H2B_CUDA(cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+    if (m == 0) {
+        H2B_CUDA(cudaMemsetAsync(d_report, 0, (max_report + 1) * 8, ctx->stream));
+        return;
+    }
+    u32* counts;
+    uint8_t* flags = flags_workspace(ctx, 1, (u32)m, &counts);
+    H2B_LAUNCH(ctx, k_check_equalities, ceil_div(m, 256), 256, 0, (const uint64_t*)d_cells, (uint64_t)N, d_pairs, (u32)m, flags, d_status);
+    report_run(ctx, flags, 1, (u32)m, max_report, d_report, counts);
+}
+
+void check_constants_run(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_consts, const uint64_t* d_index, size_t m,
+                         size_t max_report, void* d_report, uint32_t* d_status) {
+    check_pairs_common(m, max_report);
+    H2B_CUDA(cudaMemsetAsync(d_status, 0, 4, ctx->stream));
+    if (m == 0) {
+        H2B_CUDA(cudaMemsetAsync(d_report, 0, (max_report + 1) * 8, ctx->stream));
+        return;
+    }
+    u32* counts;
+    uint8_t* flags = flags_workspace(ctx, 1, (u32)m, &counts);
+    H2B_LAUNCH(ctx, k_check_constants, ceil_div(m, 256), 256, 0, (const uint64_t*)d_cells, (uint64_t)N, (const uint64_t*)d_consts, d_index,
+               (u32)m, flags, d_status);
+    report_run(ctx, flags, 1, (u32)m, max_report, d_report, counts);
+}
+
+void count_distinct_run(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count) {
+    H2B_REQUIRE(m < ((size_t)1 << 32), "count_distinct: at most 2^32 - 1 values");
+    H2B_CUDA(cudaMemsetAsync(d_count, 0, 4, ctx->stream));
+    if (m == 0) return;
+    const u32 n = (u32)m;
+    const int sort_ctas = sort_column_ctas(ctx, n);
+    const size_t scratch = sort_column_scratch(n, sort_ctas);
+    char* w = (char*)ctx->get(WS_SORT_TMP, scratch + 2 * (size_t)n * 32);
+    uint64_t* sorted = (uint64_t*)(w + scratch);
+    uint64_t* canon = sorted + 4 * (size_t)n;
+    sort_column(ctx, (const uint64_t*)d_values, n, sorted, canon, w, sort_ctas);
+    H2B_LAUNCH(ctx, k_count_runs, ceil_div(n, 256), 256, 0, (const uint64_t*)canon, n, d_count);
 }
 
 }  // namespace h2b

@@ -201,6 +201,11 @@ void assign_lookups_run(h2b_ctx* ctx, const void* d_vals, size_t N, uint32_t k, 
 void eval_rational_run(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out);
 // halo2-base form of the witness (asynchronous; violations land in *d_status, which both zero first)
 void apply_rational_run(h2b_ctx* ctx, void* d_values, size_t N, const uint64_t* d_index, void* d_den, size_t R, uint32_t* d_status);
+// MockProver on halo2-base's keygen data (include/h2b200.h, "MockProver for a halo2-base builder")
+void mock_selectors_run(h2b_ctx* ctx, const void* d_selectors, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t ncols,
+                        void* d_q);
+void mock_lookup_selector_run(h2b_ctx* ctx, const uint64_t* d_index, size_t m, size_t N, size_t max_rows, uint32_t k, void* d_q,
+                              uint32_t* d_status);
 void assign_lookups_indexed_run(h2b_ctx* ctx, const void* d_vals, size_t N, const uint64_t* d_index, size_t n_lookup, uint32_t k, size_t L,
                                 void* d_cols, uint32_t* d_status);
 // ---- peer.cu
@@ -238,6 +243,11 @@ void permutation_decode_run(h2b_ctx* ctx, const void* const* d_sigma, size_t n_c
                             void* d_reports);
 void check_copies_run(h2b_ctx* ctx, const void* const* d_columns, const void* d_map, size_t n_cols, uint32_t k, size_t max_report,
                       void* d_reports);
+void check_equalities_run(h2b_ctx* ctx, const void* d_cells, size_t N, const uint64_t* d_pairs, size_t m, size_t max_report, void* d_report,
+                          uint32_t* d_status);
+void check_constants_run(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_consts, const uint64_t* d_index, size_t m,
+                         size_t max_report, void* d_report, uint32_t* d_status);
+void count_distinct_run(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count);
 // ---- srs.cu
 void g_to_lagrange_run(h2b_ctx* ctx, const void* d_g, uint32_t k, void* d_g_lagrange);
 void srs_setup_run(h2b_ctx* ctx, const uint64_t tau[4], const uint64_t base_xy[8], uint32_t k, void* d_g, void* d_g_lagrange);

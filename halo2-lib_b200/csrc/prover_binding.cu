@@ -18,6 +18,7 @@
 // the header's inline code stays private to the library: programs that include the header never bind to this copy
 #pragma GCC visibility push(hidden)
 #include "../../include/h2b200_prover.hpp"
+#include "../../include/h2b200_mock.hpp"
 
 namespace h2bp {
 using namespace h2b;
@@ -28,6 +29,12 @@ struct BoundCircuit {
     BoundCircuit(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, const std::map<std::string, const Fr*>& fixed,
                  const std::vector<const Fr*>& sigma)
         : ctx(c), cs(ctx, k, A, L, sel, fixed, sigma) {}
+};
+struct BoundMock {
+    Context ctx;
+    MockProver mock;
+    BoundMock(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, uint32_t lookup_bits, size_t max_rows)
+        : ctx(c), mock(ctx, k, A, L, sel, lookup_bits, max_rows) {}
 };
 struct BoundSession {
     Context ctx;
@@ -201,6 +208,54 @@ H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report
                 std::copy(rows.begin(), rows.end(), p + 1);
                 p += max_report + 1;
             }
+    });
+}
+
+// MockProver of a builder (include/h2b200_mock.hpp).  n_lookups: the number of lookup reports (L, 1 for the selector lookup, or 0)
+H2BP_API int h2bp_mock_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits, size_t max_rows,
+                              BoundMock** out, uint64_t* n_lookups) {
+    return run(ctx, [&] {
+        if (!out || !n_lookups) throw Error(H2B_ERR_ARG, "mock_create: null argument");
+        *out = new BoundMock(ctx, k, A, L, selector_lookup != 0, lookup_bits, max_rows);
+        *n_lookups = (*out)->mock.n_lookups;
+    });
+}
+H2BP_API void h2bp_mock_free(BoundMock* b) { delete b; }
+H2BP_API int h2bp_mock_column(BoundMock* b, const char* name, h2b_poly** poly, size_t* offset, size_t* rows) {
+    return run(b ? b->ctx.raw() : nullptr, [&] { write_column(b->mock.column(name ? name : ""), poly, offset, rows); });
+}
+
+// one run.  break_points: A - 1 words (the count in *n_break_points); report: max_report + 1 words per gate column, lookup, then
+// the advice equalities and the constant equalities (as h2bp_check); cells: max_report x (column, row, column, row) of the
+// reported advice equalities, then max_report x (column, row) of the reported constant equalities
+H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report, uint64_t* break_points, uint64_t* n_break_points,
+                           uint64_t* report, uint64_t* cells) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        if (!v || !n_break_points || !report || !cells || (b->mock.A > 1 && !break_points)) throw Error(H2B_ERR_ARG, "mock_run: null argument");
+        const MockReport r = b->mock.run(*v, max_report);
+        *n_break_points = r.break_points.size();
+        std::copy(r.break_points.begin(), r.break_points.end(), break_points);
+        uint64_t* p = report;
+        auto put = [&](const std::pair<uint64_t, std::vector<uint64_t>>& e) {
+            std::fill(p, p + max_report + 1, 0);
+            p[0] = e.first;
+            std::copy(e.second.begin(), e.second.end(), p + 1);
+            p += max_report + 1;
+        };
+        for (auto& e : r.gates) put(e);
+        for (auto& e : r.lookups) put(e);
+        put(r.equalities);
+        put(r.constants);
+        std::fill(cells, cells + 6 * max_report, 0);
+        for (size_t i = 0; i < r.equality_cells.size(); i++) {
+            const auto& [x, y] = r.equality_cells[i];
+            const uint64_t w[4] = {x.column, x.row, y.column, y.row};
+            std::copy(w, w + 4, cells + 4 * i);
+        }
+        for (size_t i = 0; i < r.constant_cells.size(); i++) {
+            cells[4 * max_report + 2 * i] = r.constant_cells[i].column;
+            cells[4 * max_report + 2 * i + 1] = r.constant_cells[i].row;
+        }
     });
 }
 

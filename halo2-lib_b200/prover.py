@@ -11,7 +11,7 @@ polynomials; the transcript, the challenges and every device call stay in the co
 from __future__ import annotations
 import ctypes as C
 import numpy as np
-from ._capi import lib, CHECK_MAX_REPORT, Witness, BLIND_FN, ALLREDUCE_FN, COMMIT_FN
+from ._capi import lib, CHECK_MAX_REPORT, Witness, BuilderView, BLIND_FN, ALLREDUCE_FN, COMMIT_FN
 from .host import Context, ParamsKZG
 
 R_MOD = 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001
@@ -415,4 +415,78 @@ class ProverSession:
     def free(self):
         if self._h:
             lib.h2bp_session_free(self._h)
+            self._h = None
+
+
+class MockProver:
+    """MockProver::run + verify for a halo2-base builder in its keygen form, with no SRS, sigma or proving key
+    (h2b::MockProver, include/h2b200_mock.hpp): what BaseTester::run_builder asks of halo2's MockProver.
+
+    Shape as `Circuit`: A gate-advice columns, L lookup-advice columns (or the selector lookup when L = 0, or no lookup), one
+    constants column, the table 0 .. 2^lookup_bits - 1, and max_rows = 2^k - unusable_rows as calculate_params gets it
+    (at most 2^k - 7; default 2^k - 9, BaseTester's unusable_rows).  `lagr[name]` (a{j}, l{t}, q{j}, q_lookup, table) views the columns of the last run."""
+
+    def __init__(self, ctx: Context, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
+                 max_rows: int | None = None):
+        self.ctx, self.k, self.A, self.L = ctx, k, A, L
+        self.max_rows = (1 << k) - 9 if max_rows is None else max_rows
+        h, nl = C.c_void_p(), C.c_uint64()
+        ctx.check(lib.h2bp_mock_create(ctx.h, k, A, L, int(selector_lookup), lookup_bits, self.max_rows, C.byref(h), C.byref(nl)))
+        self._h, self.n_lookups = h, int(nl.value)
+        self.lagr = _Columns(self, "lagr")
+
+    def column(self, table: str, name: str) -> Column:
+        if table != "lagr":
+            raise KeyError(table)
+        poly, off, rows = C.c_void_p(), C.c_size_t(), C.c_size_t()
+        self.ctx.check(lib.h2bp_mock_column(self._h, name.encode(), C.byref(poly), C.byref(off), C.byref(rows)))
+        return Column(self.ctx, poly, off.value, rows.value)
+
+    def run(self, cells, selectors, advice_equalities=(), constant_equalities=None, lookups=(), rational_index=None, rational_den=None,
+            max_report: int = 16) -> dict:
+        """cells: the virtual column (n x 4 Montgomery limbs), in either witness form (rational_index / rational_den: the
+        (uint64 index, Montgomery d) pairs of the Rational cells, indices strictly increasing); selectors: one bool per cell;
+        advice_equalities: (a, b) index pairs; constant_equalities: (constants (m x 4 Montgomery limbs), indices); lookups:
+        indices of the looked-up cells in assign_raw order (L > 0) or of the cells whose raw row gets q_lookup (L = 0).
+
+        Returns gates[j], lookups[t] (failing rows < u), equalities and constants (failing equality indices), each as
+        (count, the first min(count, max_report) ascending); equality_cells / constant_cells: the raw cells ((column, row)) of
+        every reported equality; break_points; satisfied.  halo2-base's panics raise H2BError with its message."""
+        if not 1 <= max_report <= CHECK_MAX_REPORT:
+            raise ValueError("MockProver: max_report must be in 1..%d" % CHECK_MAX_REPORT)
+        u64 = lambda a: np.ascontiguousarray(a, dtype=np.uint64)
+        V = u64(cells).reshape(-1, 4)
+        S = np.ascontiguousarray(selectors, dtype=np.uint8).reshape(-1)
+        if len(S) != len(V):
+            raise ValueError("MockProver: one selector per cell")
+        E = u64(advice_equalities).reshape(-1, 2)
+        ce, ci = (np.zeros((0, 4)), []) if constant_equalities is None else constant_equalities
+        Kc, Ki = u64(ce).reshape(-1, 4), u64(ci).reshape(-1)
+        if len(Kc) != len(Ki):
+            raise ValueError("MockProver: one index per constant")
+        LK = u64(lookups).reshape(-1)
+        RI = u64([] if rational_index is None else rational_index).reshape(-1)
+        RD = u64(np.zeros((0, 4)) if rational_den is None else rational_den).reshape(-1, 4)
+        if len(RI) != len(RD):
+            raise ValueError("MockProver: rational_index and rational_den differ in length")
+        p = lambda a: a.ctypes.data if a.size else None
+        view = BuilderView(p(V), len(V), p(RI), p(RD), len(RI), p(S), p(E), len(E), p(Kc), p(Ki), len(Ki), p(LK), len(LK))
+        A, nl = self.A, self.n_lookups
+        bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
+        words = np.empty((A + nl + 2, max_report + 1), dtype=np.uint64)
+        cells_out = np.empty(6 * max_report, dtype=np.uint64)
+        self.ctx.check(lib.h2bp_mock_run(self._h, C.byref(view), max_report, C.c_void_p(bps.ctypes.data), C.byref(nbp),
+                                         C.c_void_p(words.ctypes.data), C.c_void_p(cells_out.ctypes.data)))
+        reports = [(int(r[0]), [int(x) for x in r[1:1 + min(int(r[0]), max_report)]]) for r in words]
+        eq, co = reports[A + nl], reports[A + nl + 1]
+        ec = cells_out[:4 * max_report].reshape(-1, 4)
+        cc = cells_out[4 * max_report:].reshape(-1, 2)
+        return {"gates": reports[:A], "lookups": reports[A:A + nl], "equalities": eq, "constants": co,
+                "equality_cells": [((int(c[0]), int(c[1])), (int(c[2]), int(c[3]))) for c in ec[:len(eq[1])]],
+                "constant_cells": [(int(c[0]), int(c[1])) for c in cc[:len(co[1])]],
+                "break_points": [int(b) for b in bps[:nbp.value]], "satisfied": not any(c for c, _ in reports)}
+
+    def free(self):
+        if self._h:
+            lib.h2bp_mock_free(self._h)
             self._h = None

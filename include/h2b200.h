@@ -418,6 +418,30 @@ int h2b_permutation_decode_dev(h2b_ctx* ctx, const void* const* d_sigma, size_t 
 int h2b_check_copies_dev(h2b_ctx* ctx, const void* const* d_columns, const void* d_map, size_t n_cols, uint32_t k,
                          size_t max_report, void* d_reports /* n_cols reports */);
 
+/* ---- MockProver for a halo2-base builder in its keygen form (no SRS, no sigma, no proving key; see h2b200_mock.hpp).
+ * Indices are uint64 positions in the virtual column (ctx.advice concatenated over the threads).  All asynchronous.
+ *   h2b_mock_selectors_dev        the selector columns of the gate-advice columns: d_q (ncols x 2^k) gets q_c[r] = 1 where the
+ *                                 walk of h2b_assign_columns_dev places virtual cell s_c + r in column c and its selector byte
+ *                                 (d_selectors, N bytes) is set, 0 elsewhere; a break cell's selector goes to row 0 of the next
+ *                                 column only (the walk enables it after the break).  Same H2B_ERR_LAYOUT rules.
+ *   h2b_mock_lookup_selector_dev  q_lookup of one gate column (2^k, zeroed first): q[index[i]] = 1.  *d_status (zeroed first):
+ *                                 bit 0 an index >= N, bit 1 an index >= max_rows (an unusable row).
+ *   h2b_check_equalities_dev      m pairs (a, b) (2 x uint64 each): the equalities whose cells differ -> one report over the pair
+ *                                 indices (form of the constraint check reports).  *d_status (zeroed first): bit 0 for an index
+ *                                 >= N (its equality is flagged, nothing is read through it).
+ *   h2b_check_constants_dev       m pairs (d_consts[i] Montgomery, d_index[i]): cells differing from their constant; the same report
+ *                                 and status rules.
+ *   h2b_count_distinct_dev        *d_count (device uint32) = the number of distinct values among m Montgomery elements. */
+int h2b_mock_selectors_dev(h2b_ctx* ctx, const void* d_selectors, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k,
+                           size_t ncols, void* d_q);
+int h2b_mock_lookup_selector_dev(h2b_ctx* ctx, const void* d_index, size_t m, size_t N, size_t max_rows, uint32_t k, void* d_q,
+                                 uint32_t* d_status);
+int h2b_check_equalities_dev(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_pairs, size_t m, size_t max_report,
+                             void* d_report, uint32_t* d_status);
+int h2b_check_constants_dev(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_consts, const void* d_index, size_t m,
+                            size_t max_report, void* d_report, uint32_t* d_status);
+int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count);
+
 /* ---- opening arithmetic (SURVEY.md §8(f) rank 4): halo2-axiom 0.5.3 `arithmetic::{eval_polynomial, kate_division}`
  * and the polynomial linear combinations of `poly/kzg/multiopen/shplonk/prover.rs` ------------------------------- */
 /* out = sum_i coeffs[i] * x^i */
