@@ -31,4 +31,4 @@ from .evaluation import (  # noqa: F401,E402
     poly_lincomb,
     permute_expression_pair,
 )
-from .prover import Poly, Circuit, ProverSession, MockProver, synthetic_circuit  # noqa: F401,E402
+from .prover import Poly, Circuit, ProverSession, MockProver, keygen, synthetic_circuit  # noqa: F401,E402

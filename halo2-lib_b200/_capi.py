@@ -137,6 +137,9 @@ SIGNATURES = {
     "h2b_check_equalities_dev": (_int, [_vp, _vp, _sz, _vp, _sz, _sz, _vp, _vp]),
     "h2b_check_constants_dev": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp, _vp]),
     "h2b_count_distinct_dev": (_int, [_vp, _vp, _sz, _vp]),
+    "h2b_keygen_copies_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "h2b_keygen_sigma_map_dev": (_int, [_vp, _vp, _sz, _sz, _u32, _vp]),
+    "h2b_keygen_sigma_values_dev": (_int, [_vp, _vp, _sz, _u32, _vp]),
     "h2b_divide_by_vanishing_poly": (_int, [_vp, _vp, _u32, _u32]),
     "h2b_divide_by_vanishing_poly_dev": (_int, [_vp, _vp, _u32, _u32]),
     "h2b_eval_polynomial": (_int, [_vp, _vp, _sz, _vp, _vp]),
@@ -203,6 +206,7 @@ PROVER_SIGNATURES = {
     "h2bp_mock_free": (None, [_vp]),
     "h2bp_mock_column": (_int, [_vp, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
     "h2bp_mock_run": (_int, [_vp, C.POINTER(BuilderView), _sz, _vp, _u64s, _vp, _vp]),
+    "h2bp_keygen": (_int, [_vp, _vp, _u32, _sz, _sz, _sz, _int, _u32, _sz, C.POINTER(BuilderView), C.POINTER(_vp), _vp, _u64s, _vp, _vp]),
 }
 
 

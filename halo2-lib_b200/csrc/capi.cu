@@ -1427,6 +1427,31 @@ int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_
     });
 }
 
+// ------------------------------------------------------------------------------------------------ keygen of a builder
+int h2b_keygen_copies_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
+                          const void* d_lookup_index, size_t n_lookup, const void* d_pairs, size_t M, const void* d_consts,
+                          const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((break_points || nbp == 0) && (d_lookup_index || n_lookup == 0) && (d_pairs || M == 0) &&
+                        ((d_consts && d_const_index) || Mc == 0) && d_c && (d_edges || nbp + n_lookup + M + Mc == 0) && d_status,
+                    "keygen_copies: null pointer");
+        keygen_copies_run(ctx, N, break_points, nbp, k, A, L, (const uint64_t*)d_lookup_index, n_lookup, (const uint64_t*)d_pairs, M, d_consts,
+                          (const uint64_t*)d_const_index, Mc, d_c, d_edges, d_status);
+    });
+}
+int h2b_keygen_sigma_map_dev(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_edges || E == 0) && d_map, "keygen_sigma_map: null pointer");
+        keygen_sigma_map_run(ctx, d_edges, E, n_cols, k, d_map);
+    });
+}
+int h2b_keygen_sigma_values_dev(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_map && d_sigma, "keygen_sigma_values: null pointer");
+        keygen_sigma_values_run(ctx, d_map, n_cols, k, d_sigma);
+    });
+}
+
 // ------------------------------------------------------------------------------------------------ opening arithmetic
 int h2b_eval_polynomial_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n, const uint64_t x[4], uint64_t out[4]) {
     return guarded(ctx, [&] {

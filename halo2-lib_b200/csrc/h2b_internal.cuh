@@ -236,6 +236,21 @@ bool permute_expression_pair_run(h2b_ctx* ctx, const void* d_input, const void* 
 int sort_column_ctas(h2b_ctx* ctx, uint32_t n);
 size_t sort_column_scratch(uint32_t n, int sort_ctas);
 void sort_column(h2b_ctx* ctx, const uint64_t* d_src, uint32_t n, uint64_t* d_out, uint64_t* d_out_canon, char* scratch, int sort_ctas);
+// the same stable sort on n 256-bit integer keys (4 little-endian uint64 each, not field elements): d_perm[i] = the id of the
+// i-th smallest key, ties in the order of d_init (the identity when null); scratch holds sort_keys_scratch(n, sort_ctas) bytes
+size_t sort_keys_scratch(uint32_t n, int sort_ctas);
+void sort_keys(h2b_ctx* ctx, const uint64_t* d_keys, uint32_t n, const uint32_t* d_init, uint32_t* d_perm, char* scratch, int sort_ctas);
+// d_out[i] = d_in[0] + .. + d_in[i - 1] (uint32); scratch holds exclusive_scan_scratch(n) bytes
+size_t exclusive_scan_scratch(uint32_t n);
+void exclusive_scan(h2b_ctx* ctx, const uint32_t* d_in, uint32_t n, uint32_t* d_out, char* scratch);
+// ---- ntt.cu: omega^r = lo[r mod 2^h] * hi[r >> h] for the 2^k domain root (the power tables of its NTT plan)
+void domain_power_tables(h2b_ctx* ctx, uint32_t k, const void** lo, const void** hi, int* h);
+// ---- keygen.cu (include/h2b200.h, "keygen of a halo2-base builder")
+void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, const uint64_t* d_lookup_index,
+                       size_t n_lookup, const uint64_t* d_pairs, size_t M, const void* d_consts, const uint64_t* d_const_index, size_t Mc,
+                       void* d_c, void* d_edges, uint32_t* status);
+void keygen_sigma_map_run(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map);
+void keygen_sigma_values_run(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma);
 // ---- check.cu (MockProver::verify's checks; reports of max_report + 1 words per item, see include/h2b200.h)
 void check_graph_run(h2b_ctx* ctx, const h2b_graph* g, uint32_t k, size_t rows, size_t max_report, void* d_report);
 void check_lookup_run(h2b_ctx* ctx, const void* d_input, const void* d_table, uint32_t k, size_t rows, size_t max_report, void* d_report);

@@ -289,6 +289,66 @@ void sort_column(h2b_ctx* ctx, const uint64_t* d_src, u32 n, uint64_t* d_out, ui
                d_out_canon);
 }
 
+// ---------------------------------------------------------------------- the same sort and scan on integer keys (keygen.cu)
+// idx = init (or the identity) and diff[0..8) |= key XOR first key: the byte positions k_radix_sort has to pass over
+__global__ void __launch_bounds__(256) k_key_init(const uint64_t* __restrict__ keys, u32 n, const u32* __restrict__ init, u32* __restrict__ idx,
+                                                  u32* __restrict__ diff) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    u32 mine[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (i < n) {
+        idx[i] = init ? init[i] : i;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const uint64_t x = __ldg(keys + 4 * (size_t)i + j) ^ __ldg(keys + j);
+            mine[2 * j] = (u32)x;
+            mine[2 * j + 1] = (u32)(x >> 32);
+        }
+    }
+#pragma unroll
+    for (int l = 0; l < 8; l++) {
+        const u32 m = __reduce_or_sync(0xffffffffu, mine[l]);
+        if ((threadIdx.x & 31) == 0 && m) atomicOr(diff + l, m);
+    }
+}
+__global__ void __launch_bounds__(256) k_pick_perm(const u32* __restrict__ idx_a, const u32* __restrict__ idx_b, const u32* __restrict__ which, u32 n,
+                                                   u32* __restrict__ perm) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) perm[i] = (__ldg(which) ? idx_b : idx_a)[i];
+}
+
+size_t sort_keys_scratch(u32 n, int sort_ctas) {
+    return ((size_t)n * 8 + (256 * (size_t)sort_ctas + 256 + 16) * 4 + 255) & ~(size_t)255;
+}
+
+void sort_keys(h2b_ctx* ctx, const uint64_t* d_keys, u32 n, const u32* d_init, u32* d_perm, char* scratch, int sort_ctas) {
+    if (n == 0) return;
+    // scratch: idx_a (4 n) | idx_b (4 n) | table (256 x CTAs) | totals (256) | diff (8) | which (1)
+    u32* idx_a = (u32*)scratch;
+    u32* idx_b = idx_a + n;
+    u32* table = idx_b + n;
+    u32* totals = table + 256 * (size_t)sort_ctas;
+    u32* diff = totals + 256;
+    u32* which = diff + 8;
+    H2B_CUDA(cudaMemsetAsync(diff, 0, 9 * 4, ctx->stream));
+    H2B_LAUNCH(ctx, k_key_init, ceil_div(n, 256), 256, 0, d_keys, n, d_init, idx_a, diff);
+    const u32* c_diff = diff;
+    void* args[] = {(void*)&d_keys, (void*)&n, (void*)&idx_a, (void*)&idx_b, (void*)&c_diff, (void*)&table, (void*)&totals, (void*)&which};
+    H2B_CUDA(cudaLaunchCooperativeKernel((const void*)k_radix_sort, dim3((unsigned)sort_ctas), dim3(RS_T), args, 0, ctx->stream));
+    ctx->launches++;
+    H2B_LAUNCH(ctx, k_pick_perm, ceil_div(n, 256), 256, 0, (const u32*)idx_a, (const u32*)idx_b, (const u32*)which, n, d_perm);
+}
+
+size_t exclusive_scan_scratch(u32 n) { return ((size_t)n * 4 + (size_t)ceil_div(n, XS_TILE) * 8 + 255) & ~(size_t)255; }
+
+void exclusive_scan(h2b_ctx* ctx, const u32* d_in, u32 n, u32* d_out, char* scratch) {
+    if (n == 0) return;
+    const u32 ntiles = ceil_div(n, XS_TILE);
+    u32* unused = (u32*)scratch;  // the second scan of the pair runs over the same flags
+    uint2* tile_sums = (uint2*)(scratch + (((size_t)n * 4 + 7) & ~(size_t)7));
+    H2B_LAUNCH(ctx, k_xscan_tiles, ntiles, 256, 0, d_in, d_in, n, d_out, unused, tile_sums);
+    H2B_LAUNCH(ctx, k_xscan_apply, ntiles, 256, 0, n, (const uint2*)tile_sums, d_out, unused);
+}
+
 // Enqueues the whole permutation; the verdict word (bit 0: an input value is missing from the table, bit 1: counts
 // disagree) is left at the returned device address, zero when the argument is satisfiable.
 u32* permute_expression_pair_enqueue(h2b_ctx* ctx, const void* d_input, const void* d_table, uint32_t k, uint32_t blinding_factors,

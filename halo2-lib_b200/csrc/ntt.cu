@@ -330,6 +330,14 @@ void ntt_free_plans(h2b_ctx* ctx) {
     ctx->ntt_plans.clear();
 }
 
+void domain_power_tables(h2b_ctx* ctx, uint32_t k, const void** lo, const void** hi, int* h) {
+    H2B_REQUIRE(k >= 1 && k <= 28, "domain_power_tables: k out of range");
+    const NttPlan* p = get_plan(ctx, k, FR_OMEGA[k], 0);
+    *lo = p->tw_lo;
+    *hi = p->tw_hi;
+    *h = p->h;
+}
+
 void domain_omega(uint32_t k, uint64_t out[4], bool inverse) {
     memcpy(out, inverse ? FR_OMEGA_INV[k] : FR_OMEGA[k], 32);
 }

@@ -19,16 +19,15 @@
 #pragma GCC visibility push(hidden)
 #include "../../include/h2b200_prover.hpp"
 #include "../../include/h2b200_mock.hpp"
+#include "../../include/h2b200_keygen.hpp"
 
 namespace h2bp {
 using namespace h2b;
 
 struct BoundCircuit {
     Context ctx;
-    ProverCircuit cs;
-    BoundCircuit(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, const std::map<std::string, const Fr*>& fixed,
-                 const std::vector<const Fr*>& sigma)
-        : ctx(c), cs(ctx, k, A, L, sel, fixed, sigma) {}
+    std::unique_ptr<ProverCircuit> cs;  // built against ctx (a circuit keeps a reference to its context)
+    explicit BoundCircuit(h2b_ctx* c) : ctx(c) {}
 };
 struct BoundMock {
     Context ctx;
@@ -110,7 +109,9 @@ H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, i
         for (size_t i = 0; i < n_fixed; i++) f[fixed_names[i]] = reinterpret_cast<const Fr*>(fixed[i]);
         std::vector<const Fr*> s;
         for (size_t i = 0; i < n_sigma; i++) s.push_back(reinterpret_cast<const Fr*>(sigma[i]));
-        *out = new BoundCircuit(ctx, k, A, L, selector_lookup != 0, f, s);
+        auto b = std::make_unique<BoundCircuit>(ctx);
+        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s);
+        *out = b.release();
     });
 }
 H2BP_API void h2bp_circuit_free(BoundCircuit* b) { delete b; }
@@ -118,7 +119,7 @@ H2BP_API void h2bp_circuit_free(BoundCircuit* b) { delete b; }
 // shape: degree, chunk, ext_k, bf, u, n_sets, n_lookups, selector_lookup; names: "adv=..\nperm=..\nfixed=..\nsigma=.." (comma-separated)
 H2BP_API int h2bp_circuit_info(BoundCircuit* b, uint64_t* shape, char* names, size_t cap) {
     return run(b ? b->ctx.raw() : nullptr, [&] {
-        const ProverCircuit& cs = b->cs;
+        const ProverCircuit& cs = *b->cs;
         const uint64_t v[8] = {cs.degree, cs.chunk, cs.ext_k, cs.bf, cs.u, cs.n_sets, cs.n_lookups, cs.selector_lookup};
         if (!shape) throw Error(H2B_ERR_ARG, "circuit_info: null shape");
         std::copy(v, v + 8, shape);
@@ -128,14 +129,14 @@ H2BP_API int h2bp_circuit_info(BoundCircuit* b, uint64_t* shape, char* names, si
     });
 }
 H2BP_API int h2bp_circuit_column(BoundCircuit* b, const char* table, const char* name, h2b_poly** poly, size_t* offset, size_t* rows) {
-    return run(b ? b->ctx.raw() : nullptr, [&] { write_column(b->cs.column(table ? table : "", name ? name : ""), poly, offset, rows); });
+    return run(b ? b->ctx.raw() : nullptr, [&] { write_column(b->cs->column(table ? table : "", name ? name : ""), poly, offset, rows); });
 }
 
 // srs: the caller's SRS handle (its shard holds srs_count points); both handles must outlive the session
 H2BP_API int h2bp_session_create(h2b_ctx* ctx, h2b_srs* srs, uint32_t k, size_t srs_count, BoundCircuit* cs, BoundSession** out) {
     return run(ctx, [&] {
         if (!srs || !cs || !out) throw Error(H2B_ERR_ARG, "session_create: null argument");
-        *out = new BoundSession(ctx, srs, k, srs_count, cs->cs);
+        *out = new BoundSession(ctx, srs, k, srs_count, *cs->cs);
     });
 }
 H2BP_API void h2bp_session_free(BoundSession* b) { delete b; }
@@ -256,6 +257,32 @@ H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report
             cells[4 * max_report + 2 * i] = r.constant_cells[i].column;
             cells[4 * max_report + 2 * i + 1] = r.constant_cells[i].row;
         }
+    });
+}
+
+// keygen of a builder (include/h2b200_keygen.hpp).  Out: the circuit (freed with h2bp_circuit_free); break_points (A - 1 words,
+// the count in *n_break_points); vk: 12 limbs per commitment, the fixed columns in the circuit's fixed_names order, then the sigma
+// columns; times: the five phases of KeygenTimes in ms (may be null)
+H2BP_API int h2bp_keygen(h2b_ctx* ctx, h2b_srs* srs, uint32_t k, size_t srs_count, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits,
+                         size_t max_rows, const BuilderView* v, BoundCircuit** out, uint64_t* break_points, uint64_t* n_break_points, uint64_t* vk,
+                         double* times) {
+    return run(ctx, [&] {
+        if (!srs || !v || !out || !n_break_points || !vk || (A > 1 && !break_points)) throw Error(H2B_ERR_ARG, "keygen: null argument");
+        auto b = std::make_unique<BoundCircuit>(ctx);
+        const ParamsKZG params(b->ctx, k, srs, srs_count);
+        KeygenTimes t;
+        KeygenResult r = keygen(b->ctx, params, k, A, L, selector_lookup != 0, lookup_bits, max_rows, *v, &t);
+        b->cs = std::move(r.pk);
+        *n_break_points = r.break_points.size();
+        std::copy(r.break_points.begin(), r.break_points.end(), break_points);
+        size_t i = 0;
+        for (auto& f : r.vk.fixed) std::memcpy(vk + 12 * i++, f.second.x.data(), sizeof(G1));
+        for (auto& p : r.vk.permutation) std::memcpy(vk + 12 * i++, p.x.data(), sizeof(G1));
+        if (times) {
+            const double w[5] = {t.copies, t.forest, t.sigma, t.pk, t.vk};
+            std::copy(w, w + 5, times);
+        }
+        *out = b.release();
     });
 }
 

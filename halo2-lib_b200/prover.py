@@ -143,14 +143,19 @@ class Circuit:
 
     def __init__(self, ctx: Context, k: int, fixed_lagrange: dict, sigma_lagrange: list, A: int = 1, L: int = 0,
                  selector_lookup: bool = True):
-        self.ctx, self.k, self.n, self.A, self.L = ctx, k, 1 << k, A, L
-        fixed = {nm: _rows(a, self.n, nm) for nm, a in fixed_lagrange.items()}
-        sigma = [_rows(a, self.n, "sigma %d" % i) for i, a in enumerate(sigma_lagrange)]
+        n = 1 << k
+        fixed = {nm: _rows(a, n, nm) for nm, a in fixed_lagrange.items()}
+        sigma = [_rows(a, n, "sigma %d" % i) for i, a in enumerate(sigma_lagrange)]
         names = (C.c_char_p * len(fixed))(*[nm.encode() for nm in fixed])
         ptrs = (C.c_void_p * len(fixed))(*[a.ctypes.data for a in fixed.values()])
         sptrs = (C.c_void_p * len(sigma))(*[a.ctypes.data for a in sigma])
         h = C.c_void_p()
         ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h)))
+        self._bind(ctx, k, A, L, h)
+
+    def _bind(self, ctx: Context, k: int, A: int, L: int, h: C.c_void_p):
+        """take ownership of a compiled circuit and read its shape and column names"""
+        self.ctx, self.k, self.n, self.A, self.L = ctx, k, 1 << k, A, L
         self._h = h
         shape, text = (C.c_uint64 * 8)(), C.create_string_buffer(1 << 16)
         ctx.check(lib.h2bp_circuit_info(h, shape, text, len(text)))
@@ -278,6 +283,57 @@ def _geometric(ctx: Context, w: int, n: int) -> np.ndarray:
         out[have:have + m] = ctx.field_op(1, 0, out[:m], np.tile(to_limbs(pow(w, have, R_MOD)), (m, 1)))
         have += m
     return out
+
+
+def _builder_view(who: str, n_cells: int, selectors, advice_equalities, constant_equalities, lookups, cells=None, rational_index=None,
+                  rational_den=None):
+    """(BuilderView, the arrays it points to) of a builder in MockProver's form"""
+    u64 = lambda a: np.ascontiguousarray(a, dtype=np.uint64)
+    V = u64(np.zeros((0, 4)) if cells is None else cells).reshape(-1, 4)
+    S = np.ascontiguousarray(selectors, dtype=np.uint8).reshape(-1)
+    if len(S) != n_cells:
+        raise ValueError(who + ": one selector per cell")
+    E = u64(advice_equalities).reshape(-1, 2)
+    ce, ci = (np.zeros((0, 4)), []) if constant_equalities is None else constant_equalities
+    Kc, Ki = u64(ce).reshape(-1, 4), u64(ci).reshape(-1)
+    if len(Kc) != len(Ki):
+        raise ValueError(who + ": one index per constant")
+    LK = u64(lookups).reshape(-1)
+    RI = u64([] if rational_index is None else rational_index).reshape(-1)
+    RD = u64(np.zeros((0, 4)) if rational_den is None else rational_den).reshape(-1, 4)
+    if len(RI) != len(RD):
+        raise ValueError(who + ": rational_index and rational_den differ in length")
+    p = lambda a: a.ctypes.data if a.size else None
+    view = BuilderView(p(V), n_cells, p(RI), p(RD), len(RI), p(S), p(E), len(E), p(Kc), p(Ki), len(Ki), p(LK), len(LK))
+    return view, (V, S, E, Kc, Ki, LK, RI, RD)
+
+
+def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
+           max_rows: int | None = None, selectors=(), advice_equalities=(), constant_equalities=None, lookups=(), timings: dict | None = None):
+    """keygen_vk + keygen_pk of a halo2-base builder in its keygen form, on the device (h2b::keygen, include/h2b200_keygen.hpp).
+
+    The arguments mean what they mean for MockProver.run (selectors: one per cell of the virtual column, which fixes its length;
+    no witness values are read).  sigma is the one halo2's permutation Assembly builds from halo2-base's copy calls, bit for bit.
+    Returns (circuit, vk, break_points): `circuit` is a Circuit that ProverSession takes; vk = {"fixed": {name: commitment},
+    "permutation": [commitment per permutation column, perm_cols order]}, each commitment affine as 12 Montgomery limbs
+    (x, y, 1; the identity all zero), of the column's Lagrange values.  halo2-base's panics raise H2BError with its message.
+    `timings`, when a dict, receives the milliseconds of the phases copies / forest / sigma / pk / vk."""
+    max_rows = (1 << k) - 9 if max_rows is None else max_rows
+    n_cells = len(np.asarray(selectors).reshape(-1))
+    view, keep = _builder_view("keygen", n_cells, selectors, advice_equalities, constant_equalities, lookups)
+    bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
+    n_fixed = A + (1 if selector_lookup and L == 0 else 0) + (1 if L or selector_lookup else 0) + 1
+    vk = np.zeros((n_fixed + 1 + A + L, 12), dtype=np.uint64)
+    times = np.zeros(5, dtype=np.float64)
+    h = C.c_void_p()
+    ctx.check(lib.h2bp_keygen(ctx.h, params.h, k, params.count, A, L, int(selector_lookup), lookup_bits, max_rows, C.byref(view), C.byref(h),
+                              C.c_void_p(bps.ctypes.data), C.byref(nbp), C.c_void_p(vk.ctypes.data), C.c_void_p(times.ctypes.data)))
+    cs = Circuit.__new__(Circuit)
+    cs._bind(ctx, k, A, L, h)
+    if timings is not None:
+        timings.update(zip(("copies", "forest", "sigma", "pk", "vk"), (float(t) for t in times)))
+    out = {"fixed": {nm: vk[i] for i, nm in enumerate(cs.fixed_names)}, "permutation": list(vk[len(cs.fixed_names):])}
+    return cs, out, [int(b) for b in bps[:nbp.value]]
 
 
 class ProverSession:
@@ -454,23 +510,9 @@ class MockProver:
         every reported equality; break_points; satisfied.  halo2-base's panics raise H2BError with its message."""
         if not 1 <= max_report <= CHECK_MAX_REPORT:
             raise ValueError("MockProver: max_report must be in 1..%d" % CHECK_MAX_REPORT)
-        u64 = lambda a: np.ascontiguousarray(a, dtype=np.uint64)
-        V = u64(cells).reshape(-1, 4)
-        S = np.ascontiguousarray(selectors, dtype=np.uint8).reshape(-1)
-        if len(S) != len(V):
-            raise ValueError("MockProver: one selector per cell")
-        E = u64(advice_equalities).reshape(-1, 2)
-        ce, ci = (np.zeros((0, 4)), []) if constant_equalities is None else constant_equalities
-        Kc, Ki = u64(ce).reshape(-1, 4), u64(ci).reshape(-1)
-        if len(Kc) != len(Ki):
-            raise ValueError("MockProver: one index per constant")
-        LK = u64(lookups).reshape(-1)
-        RI = u64([] if rational_index is None else rational_index).reshape(-1)
-        RD = u64(np.zeros((0, 4)) if rational_den is None else rational_den).reshape(-1, 4)
-        if len(RI) != len(RD):
-            raise ValueError("MockProver: rational_index and rational_den differ in length")
-        p = lambda a: a.ctypes.data if a.size else None
-        view = BuilderView(p(V), len(V), p(RI), p(RD), len(RI), p(S), p(E), len(E), p(Kc), p(Ki), len(Ki), p(LK), len(LK))
+        V = np.ascontiguousarray(cells, dtype=np.uint64).reshape(-1, 4)
+        view, keep = _builder_view("MockProver", len(V), selectors, advice_equalities, constant_equalities, lookups, V, rational_index,
+                                   rational_den)
         A, nl = self.A, self.n_lookups
         bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
         words = np.empty((A + nl + 2, max_report + 1), dtype=np.uint64)

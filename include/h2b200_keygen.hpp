@@ -1,0 +1,148 @@
+// h2b200_keygen.hpp — keygen_vk + keygen_pk for a halo2-base builder in its keygen form, on the device: the break points, the
+// fixed columns (q_j, q_lookup, the table, the constants column c), sigma bit-exact to what halo2's permutation Assembly builds
+// from halo2-base's copy calls, the proving key as a ProverCircuit and the verifying key's commitments.  DESIGN.md §4.8.
+//
+// The builder comes as MockProver takes it (BuilderView, include/h2b200_mock.hpp); keygen reads no witness values: `cells` and
+// the rational pairs are ignored, `n_cells` is used.  The copy calls of BaseCircuitBuilder::synthesize, in order:
+//   1. the break copies of assign_with_constraints: (a{j+1}, 0) ~ (a_j, bp_j), j = 0, 1, ..;
+//   2. L > 0: LookupAnyManager::assign_raw's copies raw(lookup_index[i]) ~ (l{i mod L}, i / L), i = 0, 1, ..;
+//   3. CopyConstraintManager::assign_raw: the advice equalities sorted by (a, b), then the constant equalities sorted by
+//      (constant, cell) as (c, the constant's row) ~ raw(cell), the distinct constants at rows 0, 1, .. of c in that order.
+// So the builder's own order of its equalities does not change the keys.  Errors: halo2-base's panics as MockProver raises them.
+// Instance columns and several constants columns are not covered (the same boundary as MockProver).
+#pragma once
+#include <chrono>
+
+#include "h2b200_mock.hpp"
+
+namespace h2b {
+
+// affine commitments (z = 1; the identity all zero) of the Lagrange columns, as ProverSession commits them
+struct VerifyingKey {
+    std::vector<std::pair<std::string, G1>> fixed;  // the circuit's fixed_names order
+    std::vector<G1> permutation;                    // one per permutation column, perm_cols order
+};
+
+// milliseconds per phase of one keygen call (each phase ends with the stream synchronised)
+struct KeygenTimes {
+    double copies = 0;  // uploads, fixed columns, the copy list and its sorts
+    double forest = 0;  // spanning forest and walk: the sigma map
+    double sigma = 0;   // sigma values
+    double pk = 0;      // the proving key's coefficient and extended-coset forms
+    double vk = 0;      // the commitments
+};
+
+struct KeygenResult {
+    std::vector<uint64_t> break_points;
+    std::unique_ptr<ProverCircuit> pk;
+    VerifyingKey vk;
+};
+
+// params: the SRS of the 2^k domain (its Lagrange bases commit the vk); max_rows as for MockProver (<= 2^k - 7)
+inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits,
+                           size_t max_rows, const BuilderView& b, KeygenTimes* times = nullptr) {
+    using clock = std::chrono::steady_clock;
+    auto t0 = clock::now();
+    auto lap = [&](double KeygenTimes::*field) {
+        const auto t = clock::now();
+        if (times) times->*field = std::chrono::duration<double, std::milli>(t - t0).count();
+        t0 = t;
+    };
+    if (k < 3 || k > 28) throw Error(H2B_ERR_ARG, "keygen: k out of range (3..28)");
+    const size_t n = size_t(1) << k, u = n - (MockProver::BLINDING_FACTORS + 1);
+    const bool sel = selector_lookup && L == 0;
+    if (A < 1) throw Error(H2B_ERR_ARG, "keygen: no gate columns");
+    if (sel && A != 1) throw Error(H2B_ERR_ARG, "keygen: the selector lookup needs exactly one gate column");
+    if (max_rows < 1 || max_rows > u) throw Error(H2B_ERR_ARG, "keygen: max_rows must be in 1..2^k - 7");
+    const size_t n_lookups = L ? L : (sel ? 1 : 0);
+    if (n_lookups && (lookup_bits > 28 || (size_t(1) << lookup_bits) > u)) throw Error(H2B_ERR_ARG, "keygen: the lookup table does not fit the usable rows");
+    const size_t N = b.n_cells, M = b.n_advice_equalities, Mc = b.n_constant_equalities, NL = b.n_lookup;
+    if ((N && !b.selectors) || (M && !b.advice_equalities) || (Mc && !(b.constants && b.constant_index)) || (NL && !b.lookup_index))
+        throw Error(H2B_ERR_ARG, "keygen: a count > 0 needs its array");
+    h2b_ctx* c = ctx.raw();
+    KeygenResult out;
+    out.break_points = MockProver::break_points_of(b.selectors, N, A, max_rows);
+    if (NL) {
+        if (L && (NL + L - 1) / L > max_rows) throw Error(H2B_ERR_ARG, "range lookups would be assigned to unusable rows");
+        if (!L && !sel) throw Error(H2B_ERR_ARG, "range lookups require lookup advice columns");
+    }
+    const size_t nbp = out.break_points.size(), npc = 1 + A + L, E = nbp + (L ? NL : 0) + M + Mc;
+    auto device = [&](const void* host, size_t bytes) {
+        auto p = std::make_unique<Poly>(ctx, bytes / 32 + 1);
+        if (bytes >= 32) p->upload(static_cast<const Fr*>(host), bytes / 32);
+        if (bytes % 32) {
+            Fr last{};
+            std::memcpy(last.data(), static_cast<const char*>(host) + bytes / 32 * 32, bytes % 32);
+            p->upload(&last, 1, bytes / 32);
+        }
+        return p;
+    };
+    const PolyPtr sel_d = device(b.selectors, N), lk_d = device(b.lookup_index, 8 * NL), eq_d = device(b.advice_equalities, 16 * M),
+                  const_d = device(b.constants, 32 * Mc), const_idx_d = device(b.constant_index, 8 * Mc);
+    // the fixed columns in the circuit's order: q0.., [q_lookup], [table], c
+    std::vector<std::string> fixed_names;
+    for (size_t j = 0; j < A; j++) fixed_names.push_back("q" + std::to_string(j));
+    if (sel) fixed_names.push_back("q_lookup");
+    if (n_lookups) fixed_names.push_back("table");
+    fixed_names.push_back("c");
+    const size_t nf = fixed_names.size();
+    Poly fixed(ctx, nf * n), status(ctx, 1);
+    auto col = [&](size_t i) { return static_cast<Fr*>(fixed.at(i * n)); };
+    const uint64_t* bp = nbp ? out.break_points.data() : nullptr;
+    ctx.check(h2b_mock_selectors_dev(c, sel_d->at(), N, bp, nbp, k, A, fixed.at()));
+    uint32_t* st = static_cast<uint32_t*>(status.at());
+    uint32_t v[2] = {0, 0};
+    if (sel) {
+        ctx.check(h2b_mock_lookup_selector_dev(c, lk_d->at(), NL, N, max_rows, k, col(A), st));
+        std::memcpy(v, status.download(0, 1)[0].data(), 8);
+        if (v[0] & 1) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
+        if (v[0] & 2) throw Error(H2B_ERR_ARG, "range lookup assigned to an unusable row");
+    }
+    if (n_lookups) {
+        std::vector<Fr> t(n, Fr{});
+        Fr x{}, one = HostFr::one();
+        for (size_t i = 0; i < (size_t(1) << lookup_bits); i++, x = HostFr::add(x, one)) t[i] = x;
+        ctx.check(h2b_poly_upload(c, fixed.raw(), (nf - 2) * n, t[0].data(), n));
+    }
+    Poly edges(ctx, (8 * E + 31) / 32 + 1);
+    ctx.check(h2b_keygen_copies_dev(c, N, bp, nbp, k, A, L, lk_d->at(), L ? NL : 0, eq_d->at(), M, const_d->at(), const_idx_d->at(), Mc,
+                                    col(nf - 1), edges.at(), st));
+    std::memcpy(v, status.download(0, 1)[0].data(), 8);
+    // in the order of the keygen pass: the lookups, then assign_raw (constants placed first, then the equalities resolved)
+    if (v[0] & 1) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
+    if (v[1] > u)
+        throw Error(H2B_ERR_ARG, "NotEnoughRowsAvailable { current_k: " + std::to_string(k) + " }: " + std::to_string(v[1]) +
+                                     " distinct constants for the " + std::to_string(u) + " usable rows of the constants column");
+    if (v[0] & 2) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
+    lap(&KeygenTimes::copies);
+    Poly map(ctx, (npc * n + 7) / 8), sigma(ctx, npc * n);
+    ctx.check(h2b_keygen_sigma_map_dev(c, edges.at(), E, npc, k, map.at()));
+    lap(&KeygenTimes::forest);
+    ctx.check(h2b_keygen_sigma_values_dev(c, map.at(), npc, k, sigma.at()));
+    lap(&KeygenTimes::sigma);
+    std::map<std::string, const Fr*> fx;
+    for (size_t i = 0; i < nf; i++) fx[fixed_names[i]] = col(i);
+    std::vector<const Fr*> sg;
+    for (size_t i = 0; i < npc; i++) sg.push_back(static_cast<const Fr*>(sigma.at(i * n)));
+    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, sel, fx, sg);
+    lap(&KeygenTimes::pk);
+    // the vk: every fixed column, then every sigma column, committed in Lagrange form, up to 16 MSMs per batch
+    std::vector<const void*> cols;
+    for (size_t i = 0; i < nf; i++) cols.push_back(col(i));
+    for (size_t i = 0; i < npc; i++) cols.push_back(sigma.at(i * n));
+    std::vector<G1> pts(cols.size());
+    Poly d_out(ctx, 48);
+    for (size_t lo = 0; lo < cols.size(); lo += 16) {
+        const size_t m = std::min<size_t>(16, cols.size() - lo);
+        const std::vector<int> basis(m, H2B_BASIS_LAGRANGE);
+        ctx.check(h2b_msm_g1_batch_dev(c, params.raw(), basis.data(), cols.data() + lo, m, n, d_out.at()));
+        ctx.check(h2b_poly_download(c, d_out.raw(), 0, pts[lo].x.data(), m * 3));
+        g1_normalize_host_batch(pts.data() + lo, m);
+    }
+    for (size_t i = 0; i < nf; i++) out.vk.fixed.push_back({fixed_names[i], pts[i]});
+    out.vk.permutation.assign(pts.begin() + nf, pts.end());
+    lap(&KeygenTimes::vk);
+    return out;
+}
+
+}  // namespace h2b

@@ -308,6 +308,17 @@ public:
     // the same with every column as a pointer to its 2^k rows (nothing is copied on the host)
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
                   const std::vector<const Fr*>& sigma)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false) {}
+    // the same with every column as a DEVICE pointer to its 2^k Lagrange values (keygen on the device, h2b200_keygen.hpp): each is
+    // copied on the device, then transformed as above
+    struct OnDevice {};
+    ProverCircuit(OnDevice, const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup,
+                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true) {}
+
+private:
+    ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
+                  const std::vector<const Fr*>& sigma, bool on_device)
         : ctx(ctx), k(k), n(size_t(1) << k), A(A), L(L), selector_lookup(selector_lookup && L == 0) {
         degree = L ? 4 : (this->selector_lookup ? 5 : 3);
         chunk = degree - 2;
@@ -329,11 +340,16 @@ public:
         l0[0] = HostFr::one();
         ll[u] = HostFr::one();
         for (size_t i = 0; i < u; i++) la[i] = HostFr::one();
-        auto add = [&](const std::string& name, const Fr* arr) {
+        auto add = [&](const std::string& name, const Fr* arr, bool device) {
             if (!arr) throw Error(H2B_ERR_ARG, "ProverCircuit: column " + name + " is null");
             auto lg = std::make_unique<Poly>(ctx, n), cf = std::make_unique<Poly>(ctx, n), ex = std::make_unique<Poly>(ctx, size_t(1) << ext_k);
-            lg->upload(arr, n);
-            cf->upload(arr, n);
+            if (device) {
+                ctx.check(h2b_poly_copy_dev(ctx.raw(), lg->at(), arr, n));
+                ctx.check(h2b_poly_copy_dev(ctx.raw(), cf->at(), arr, n));
+            } else {
+                lg->upload(arr, n);
+                cf->upload(arr, n);
+            }
             ctx.check(h2b_lagrange_to_coeff_dev(ctx.raw(), cf->at(), k));
             ctx.check(h2b_coeff_to_extended_dev(ctx.raw(), cf->at(), n, ext_k, ex->at()));
             lagr[name] = std::move(lg);
@@ -343,15 +359,15 @@ public:
         for (auto& nm : fixed_names) {
             auto it = fixed.find(nm);
             if (it == fixed.end()) throw Error(H2B_ERR_ARG, "ProverCircuit: missing fixed column " + nm);
-            add(nm, it->second);
+            add(nm, it->second, on_device);
         }
         for (size_t i = 0; i < perm_cols.size(); i++) {
             sigma_names.push_back("sigma_" + perm_cols[i]);
-            add(sigma_names.back(), sigma[i]);
+            add(sigma_names.back(), sigma[i], on_device);
         }
-        add("l0", l0.data());
-        add("l_last", ll.data());
-        add("l_active", la.data());
+        add("l0", l0.data(), false);
+        add("l_last", ll.data(), false);
+        add("l_active", la.data(), false);
         h2b_ctx_synchronize(ctx.raw());
         // gate programs: GATES_PER_PROGRAM vertical gates each (a program holds at most 64 calculations); every program continues
         // the Horner fold in y from the previous value, so the chain of programs is the one fold evaluate_h does
@@ -391,6 +407,8 @@ public:
             lookup_result = lookup_ev.add_calculation(Calculation::Mul(lb, rg));
         }
     }
+
+public:
 
     // what ProverSession::check needs beyond a proof, built on the first check: the vertical gate as one program on fixed slot 0 /
     // advice slot 0 (bound to q{j}, a{j} per gate column) and the sigma columns decoded into map[c][r] = c' << k | r' (u32);
