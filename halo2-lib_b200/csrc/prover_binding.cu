@@ -82,6 +82,13 @@ void write_text(const std::string& s, char* out, size_t cap) {
     if (!out || s.size() + 1 > cap) throw Error(H2B_ERR_ARG, "name buffer too small");
     std::memcpy(out, s.c_str(), s.size() + 1);
 }
+// one report as max_report + 1 words: the failure count, then the rows, zero-padded
+uint64_t* write_report(uint64_t* p, const ReportItem& e, size_t max_report) {
+    std::fill(p, p + max_report + 1, 0);
+    p[0] = e.first;
+    std::copy(e.second.begin(), e.second.end(), p + 1);
+    return p + max_report + 1;
+}
 void write_column(const NamedColumn& c, h2b_poly** poly, size_t* offset, size_t* rows) {
     if (!poly || !offset || !rows) throw Error(H2B_ERR_ARG, "null output");
     *poly = c.col.poly->raw();
@@ -203,12 +210,7 @@ H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report
         const CheckReport r = b->sess.check(*w, max_report);
         uint64_t* p = report;
         for (auto* part : {&r.gates, &r.lookups, &r.copies})
-            for (auto& [count, rows] : *part) {
-                std::fill(p, p + max_report + 1, 0);
-                p[0] = count;
-                std::copy(rows.begin(), rows.end(), p + 1);
-                p += max_report + 1;
-            }
+            for (auto& e : *part) p = write_report(p, e, max_report);
     });
 }
 
@@ -237,16 +239,9 @@ H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report
         *n_break_points = r.break_points.size();
         std::copy(r.break_points.begin(), r.break_points.end(), break_points);
         uint64_t* p = report;
-        auto put = [&](const std::pair<uint64_t, std::vector<uint64_t>>& e) {
-            std::fill(p, p + max_report + 1, 0);
-            p[0] = e.first;
-            std::copy(e.second.begin(), e.second.end(), p + 1);
-            p += max_report + 1;
-        };
-        for (auto& e : r.gates) put(e);
-        for (auto& e : r.lookups) put(e);
-        put(r.equalities);
-        put(r.constants);
+        for (auto* part : {&r.gates, &r.lookups})
+            for (auto& e : *part) p = write_report(p, e, max_report);
+        write_report(write_report(p, r.equalities, max_report), r.constants, max_report);
         std::fill(cells, cells + 6 * max_report, 0);
         for (size_t i = 0; i < r.equality_cells.size(); i++) {
             const auto& [x, y] = r.equality_cells[i];

@@ -285,6 +285,11 @@ def _geometric(ctx: Context, w: int, n: int) -> np.ndarray:
     return out
 
 
+def _reports(words: np.ndarray, max_report: int) -> list:
+    """report rows of max_report + 1 words (the failure count, then the rows) -> [(count, the first min(count, max_report) rows)]"""
+    return [(int(r[0]), [int(x) for x in r[1:1 + min(int(r[0]), max_report)]]) for r in words]
+
+
 def _builder_view(who: str, n_cells: int, selectors, advice_equalities, constant_equalities, lookups, cells=None, rational_index=None,
                   rational_den=None):
     """(BuilderView, the arrays it points to) of a builder in MockProver's form"""
@@ -438,7 +443,7 @@ class ProverSession:
         A, nl = cs.A, cs.n_lookups
         words = np.empty((A + nl + len(cs.perm_cols), max_report + 1), dtype=np.uint64)
         self._done(lib.h2bp_check(self._h, C.byref(w), max_report, C.c_void_p(words.ctypes.data)))
-        reports = [(int(r[0]), [int(x) for x in r[1:1 + min(int(r[0]), max_report)]]) for r in words]
+        reports = _reports(words, max_report)
         res = {"gates": reports[:A], "lookups": reports[A:A + nl], "copies": reports[A + nl:]}
         res["satisfied"] = not any(c for c, _ in reports)
         return res
@@ -519,7 +524,7 @@ class MockProver:
         cells_out = np.empty(6 * max_report, dtype=np.uint64)
         self.ctx.check(lib.h2bp_mock_run(self._h, C.byref(view), max_report, C.c_void_p(bps.ctypes.data), C.byref(nbp),
                                          C.c_void_p(words.ctypes.data), C.c_void_p(cells_out.ctypes.data)))
-        reports = [(int(r[0]), [int(x) for x in r[1:1 + min(int(r[0]), max_report)]]) for r in words]
+        reports = _reports(words, max_report)
         eq, co = reports[A + nl], reports[A + nl + 1]
         ec = cells_out[:4 * max_report].reshape(-1, 4)
         cc = cells_out[4 * max_report:].reshape(-1, 2)

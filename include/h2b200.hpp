@@ -31,6 +31,7 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "h2b200.h"
@@ -370,53 +371,64 @@ struct Challenges {
     Fr beta{}, gamma{}, theta{}, y{};
     std::vector<Fr> user;  // ValueSource::Challenge(i)
 };
-namespace detail {
-// owns the arrays an h2b_graph points to for the duration of one call (host columns)
-struct GraphHolder {
-    std::vector<uint32_t> prog;
-    std::vector<const void*> fixed, advice, instance;
-    h2b_graph g{};
-    GraphHolder(const GraphEvaluator& ev, ValueSource result, const std::vector<const std::vector<Fr>*>& f,
-                const std::vector<const std::vector<Fr>*>& a, const std::vector<const std::vector<Fr>*>& i, const Challenges& ch)
-        : prog(ev.program()) {
-        for (auto c : f) fixed.push_back(c->data());
-        for (auto c : a) advice.push_back(c->data());
-        for (auto c : i) instance.push_back(c->data());
-        g.program = prog.data();
-        g.program_words = prog.size();
-        g.n_calculations = uint32_t(ev.calculations.size());
-        g.result = result.word();
-        g.constants = reinterpret_cast<const uint64_t*>(ev.constants.data());
-        g.n_constants = ev.constants.size();
-        g.rotations = ev.rotations.data();
-        g.n_rotations = ev.rotations.size();
-        g.fixed = fixed.data();
-        g.n_fixed = fixed.size();
-        g.advice = advice.data();
-        g.n_advice = advice.size();
-        g.instance = instance.data();
-        g.n_instance = instance.size();
-        g.challenges = reinterpret_cast<const uint64_t*>(ch.user.data());
-        g.n_challenges = ch.user.size();
-        std::copy(ch.beta.begin(), ch.beta.end(), g.beta);
-        std::copy(ch.gamma.begin(), ch.gamma.end(), g.gamma);
-        std::copy(ch.theta.begin(), ch.theta.end(), g.theta);
-        std::copy(ch.y.begin(), ch.y.end(), g.y);
+// an h2b_graph together with the arrays it points to (the program words, the column tables, the user challenges): valid while
+// the value lives.  The column tables hold host or device pointers, as the entry point the graph goes to takes them.
+class BoundGraph {
+public:
+    BoundGraph(const GraphEvaluator& ev, ValueSource result, std::vector<const void*> fixed, std::vector<const void*> advice,
+               const Challenges& ch = {}, std::vector<const void*> instance = {})
+        : prog_(ev.program()), fixed_(std::move(fixed)), advice_(std::move(advice)), instance_(std::move(instance)), user_(ch.user) {
+        g_.program = prog_.data();
+        g_.program_words = prog_.size();
+        g_.n_calculations = uint32_t(ev.calculations.size());
+        g_.result = result.word();
+        g_.constants = reinterpret_cast<const uint64_t*>(ev.constants.data());
+        g_.n_constants = ev.constants.size();
+        g_.rotations = ev.rotations.data();
+        g_.n_rotations = ev.rotations.size();
+        g_.fixed = fixed_.data();
+        g_.n_fixed = fixed_.size();
+        g_.advice = advice_.data();
+        g_.n_advice = advice_.size();
+        g_.instance = instance_.data();
+        g_.n_instance = instance_.size();
+        g_.challenges = reinterpret_cast<const uint64_t*>(user_.data());
+        g_.n_challenges = user_.size();
+        std::copy(ch.beta.begin(), ch.beta.end(), g_.beta);
+        std::copy(ch.gamma.begin(), ch.gamma.end(), g_.gamma);
+        std::copy(ch.theta.begin(), ch.theta.end(), g_.theta);
+        std::copy(ch.y.begin(), ch.y.end(), g_.y);
     }
+    BoundGraph(const BoundGraph&) = delete;
+    BoundGraph& operator=(const BoundGraph&) = delete;
+    const h2b_graph* get() const { return &g_; }
+
+private:
+    std::vector<uint32_t> prog_;
+    std::vector<const void*> fixed_, advice_, instance_;
+    std::vector<Fr> user_;
+    h2b_graph g_{};
 };
-inline std::vector<const uint64_t*> ptrs(const std::vector<const std::vector<Fr>*>& cols) {
+
+using Columns = std::vector<const std::vector<Fr>*>;  // extended-domain columns (2^ext_k values each)
+namespace detail {
+inline std::vector<const void*> tables(const Columns& cols) {
+    std::vector<const void*> p;
+    for (auto c : cols) p.push_back(c->data());
+    return p;
+}
+inline std::vector<const uint64_t*> ptrs(const Columns& cols) {
     std::vector<const uint64_t*> p;
     for (auto c : cols) p.push_back(reinterpret_cast<const uint64_t*>(c->data()));
     return p;
 }
 }  // namespace detail
-using Columns = std::vector<const std::vector<Fr>*>;  // extended-domain columns (2^ext_k values each)
 
 // custom gates of evaluate_h: values[i] = graph(previous = values[i]) on every extended-domain row
 inline void quotient_graph(const Context& ctx, const GraphEvaluator& ev, ValueSource result, const Columns& fixed, const Columns& advice,
                            const Columns& instance, const Challenges& ch, uint32_t k, uint32_t ext_k, std::vector<Fr>& values) {
-    detail::GraphHolder h(ev, result, fixed, advice, instance, ch);
-    ctx.check(h2b_quotient_graph(ctx.raw(), &h.g, k, ext_k, reinterpret_cast<uint64_t*>(values.data())));
+    const BoundGraph g(ev, result, detail::tables(fixed), detail::tables(advice), ch, detail::tables(instance));
+    ctx.check(h2b_quotient_graph(ctx.raw(), g.get(), k, ext_k, reinterpret_cast<uint64_t*>(values.data())));
 }
 inline void permutation_fold(const Context& ctx, const Columns& z_sets, const Columns& columns, const Columns& sigma, size_t chunk_len,
                              const std::vector<Fr>& l0, const std::vector<Fr>& l_last, const std::vector<Fr>& l_active,
@@ -431,9 +443,9 @@ inline void lookup_fold(const Context& ctx, const GraphEvaluator& ev, ValueSourc
                         const Columns& instance, const Challenges& ch, const std::vector<Fr>& z, const std::vector<Fr>& permuted_input,
                         const std::vector<Fr>& permuted_table, const std::vector<Fr>& l0, const std::vector<Fr>& l_last,
                         const std::vector<Fr>& l_active, uint32_t k, uint32_t ext_k, std::vector<Fr>& values) {
-    detail::GraphHolder h(ev, result, fixed, advice, instance, ch);
+    const BoundGraph g(ev, result, detail::tables(fixed), detail::tables(advice), ch, detail::tables(instance));
     auto p = [](const std::vector<Fr>& v) { return reinterpret_cast<const uint64_t*>(v.data()); };
-    ctx.check(h2b_lookup_fold(ctx.raw(), &h.g, p(z), p(permuted_input), p(permuted_table), p(l0), p(l_last), p(l_active), k, ext_k,
+    ctx.check(h2b_lookup_fold(ctx.raw(), g.get(), p(z), p(permuted_input), p(permuted_table), p(l0), p(l_last), p(l_active), k, ext_k,
                               reinterpret_cast<uint64_t*>(values.data())));
 }
 inline void divide_by_vanishing_poly(const Context& ctx, std::vector<Fr>& values, uint32_t k, uint32_t ext_k) {

@@ -48,72 +48,37 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         if (times) times->*field = std::chrono::duration<double, std::milli>(t - t0).count();
         t0 = t;
     };
-    if (k < 3 || k > 28) throw Error(H2B_ERR_ARG, "keygen: k out of range (3..28)");
-    const size_t n = size_t(1) << k, u = n - (MockProver::BLINDING_FACTORS + 1);
-    const bool sel = selector_lookup && L == 0;
-    if (A < 1) throw Error(H2B_ERR_ARG, "keygen: no gate columns");
-    if (sel && A != 1) throw Error(H2B_ERR_ARG, "keygen: the selector lookup needs exactly one gate column");
-    if (max_rows < 1 || max_rows > u) throw Error(H2B_ERR_ARG, "keygen: max_rows must be in 1..2^k - 7");
-    const size_t n_lookups = L ? L : (sel ? 1 : 0);
-    if (n_lookups && (lookup_bits > 28 || (size_t(1) << lookup_bits) > u)) throw Error(H2B_ERR_ARG, "keygen: the lookup table does not fit the usable rows");
-    const size_t N = b.n_cells, M = b.n_advice_equalities, Mc = b.n_constant_equalities, NL = b.n_lookup;
-    if ((N && !b.selectors) || (M && !b.advice_equalities) || (Mc && !(b.constants && b.constant_index)) || (NL && !b.lookup_index))
-        throw Error(H2B_ERR_ARG, "keygen: a count > 0 needs its array");
+    const CircuitShape s = builder_shape("keygen", k, A, L, selector_lookup, lookup_bits, max_rows);
+    const size_t n = s.n, N = b.n_cells, M = b.n_advice_equalities, Mc = b.n_constant_equalities, NL = b.n_lookup;
     h2b_ctx* c = ctx.raw();
     KeygenResult out;
-    out.break_points = MockProver::break_points_of(b.selectors, N, A, max_rows);
-    if (NL) {
-        if (L && (NL + L - 1) / L > max_rows) throw Error(H2B_ERR_ARG, "range lookups would be assigned to unusable rows");
-        if (!L && !sel) throw Error(H2B_ERR_ARG, "range lookups require lookup advice columns");
-    }
-    const size_t nbp = out.break_points.size(), npc = 1 + A + L, E = nbp + (L ? NL : 0) + M + Mc;
-    auto device = [&](const void* host, size_t bytes) {
-        auto p = std::make_unique<Poly>(ctx, bytes / 32 + 1);
-        if (bytes >= 32) p->upload(static_cast<const Fr*>(host), bytes / 32);
-        if (bytes % 32) {
-            Fr last{};
-            std::memcpy(last.data(), static_cast<const char*>(host) + bytes / 32 * 32, bytes % 32);
-            p->upload(&last, 1, bytes / 32);
-        }
-        return p;
-    };
-    const PolyPtr sel_d = device(b.selectors, N), lk_d = device(b.lookup_index, 8 * NL), eq_d = device(b.advice_equalities, 16 * M),
-                  const_d = device(b.constants, 32 * Mc), const_idx_d = device(b.constant_index, 8 * Mc);
+    out.break_points = builder_break_points(s, "keygen", max_rows, b, false);
+    const size_t nbp = out.break_points.size(), npc = s.perm_cols.size(), E = nbp + (L ? NL : 0) + M + Mc;
+    PolyPtr sel_d, lk_d, eq_d, const_d, const_idx_d;
+    upload_bytes(ctx, sel_d, b.selectors, N);
+    upload_bytes(ctx, lk_d, b.lookup_index, 8 * NL);
+    upload_bytes(ctx, eq_d, b.advice_equalities, 16 * M);
+    upload_bytes(ctx, const_d, b.constants, 32 * Mc);
+    upload_bytes(ctx, const_idx_d, b.constant_index, 8 * Mc);
     // the fixed columns in the circuit's order: q0.., [q_lookup], [table], c
-    std::vector<std::string> fixed_names;
-    for (size_t j = 0; j < A; j++) fixed_names.push_back("q" + std::to_string(j));
-    if (sel) fixed_names.push_back("q_lookup");
-    if (n_lookups) fixed_names.push_back("table");
-    fixed_names.push_back("c");
-    const size_t nf = fixed_names.size();
+    const size_t nf = s.fixed_names.size();
     Poly fixed(ctx, nf * n), status(ctx, 1);
     auto col = [&](size_t i) { return static_cast<Fr*>(fixed.at(i * n)); };
     const uint64_t* bp = nbp ? out.break_points.data() : nullptr;
     ctx.check(h2b_mock_selectors_dev(c, sel_d->at(), N, bp, nbp, k, A, fixed.at()));
     uint32_t* st = static_cast<uint32_t*>(status.at());
     uint32_t v[2] = {0, 0};
-    if (sel) {
+    if (s.selector_lookup) {
         ctx.check(h2b_mock_lookup_selector_dev(c, lk_d->at(), NL, N, max_rows, k, col(A), st));
         std::memcpy(v, status.download(0, 1)[0].data(), 8);
-        if (v[0] & 1) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
-        if (v[0] & 2) throw Error(H2B_ERR_ARG, "range lookup assigned to an unusable row");
+        builder_panics(s, v[0] & 1, v[0] & 2, 0, false);
     }
-    if (n_lookups) {
-        std::vector<Fr> t(n, Fr{});
-        Fr x{}, one = HostFr::one();
-        for (size_t i = 0; i < (size_t(1) << lookup_bits); i++, x = HostFr::add(x, one)) t[i] = x;
-        ctx.check(h2b_poly_upload(c, fixed.raw(), (nf - 2) * n, t[0].data(), n));
-    }
+    if (s.n_lookups) ctx.check(h2b_poly_upload(c, fixed.raw(), (nf - 2) * n, lookup_table(n, lookup_bits)[0].data(), n));
     Poly edges(ctx, (8 * E + 31) / 32 + 1);
     ctx.check(h2b_keygen_copies_dev(c, N, bp, nbp, k, A, L, lk_d->at(), L ? NL : 0, eq_d->at(), M, const_d->at(), const_idx_d->at(), Mc,
                                     col(nf - 1), edges.at(), st));
     std::memcpy(v, status.download(0, 1)[0].data(), 8);
-    // in the order of the keygen pass: the lookups, then assign_raw (constants placed first, then the equalities resolved)
-    if (v[0] & 1) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
-    if (v[1] > u)
-        throw Error(H2B_ERR_ARG, "NotEnoughRowsAvailable { current_k: " + std::to_string(k) + " }: " + std::to_string(v[1]) +
-                                     " distinct constants for the " + std::to_string(u) + " usable rows of the constants column");
-    if (v[0] & 2) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
+    builder_panics(s, v[0] & 1, false, v[1], v[0] & 2);
     lap(&KeygenTimes::copies);
     Poly map(ctx, (npc * n + 7) / 8), sigma(ctx, npc * n);
     ctx.check(h2b_keygen_sigma_map_dev(c, edges.at(), E, npc, k, map.at()));
@@ -121,10 +86,10 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
     ctx.check(h2b_keygen_sigma_values_dev(c, map.at(), npc, k, sigma.at()));
     lap(&KeygenTimes::sigma);
     std::map<std::string, const Fr*> fx;
-    for (size_t i = 0; i < nf; i++) fx[fixed_names[i]] = col(i);
+    for (size_t i = 0; i < nf; i++) fx[s.fixed_names[i]] = col(i);
     std::vector<const Fr*> sg;
     for (size_t i = 0; i < npc; i++) sg.push_back(static_cast<const Fr*>(sigma.at(i * n)));
-    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, sel, fx, sg);
+    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg);
     lap(&KeygenTimes::pk);
     // the vk: every fixed column, then every sigma column, committed in Lagrange form, up to 16 MSMs per batch
     std::vector<const void*> cols;
@@ -139,7 +104,7 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         ctx.check(h2b_poly_download(c, d_out.raw(), 0, pts[lo].x.data(), m * 3));
         g1_normalize_host_batch(pts.data() + lo, m);
     }
-    for (size_t i = 0; i < nf; i++) out.vk.fixed.push_back({fixed_names[i], pts[i]});
+    for (size_t i = 0; i < nf; i++) out.vk.fixed.push_back({s.fixed_names[i], pts[i]});
     out.vk.permutation.assign(pts.begin() + nf, pts.end());
     lap(&KeygenTimes::vk);
     return out;

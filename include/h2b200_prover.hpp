@@ -297,8 +297,68 @@ struct NamedColumn {
     size_t rows = 0;
 };
 
+// a device buffer of at least m elements, reallocated only when a call needs more than any call before it
+inline Poly* grown(const Context& ctx, PolyPtr& p, size_t m) {
+    if (!p || p->len() < m) p = std::make_unique<Poly>(ctx, std::max<size_t>(m, 1));
+    return p.get();
+}
+// `bytes` host bytes into p (grown): whole 32-byte elements straight from the caller's array, the last 1..31 bytes through a
+// zero-padded element (nothing past the end of the caller's array is read)
+inline Poly* upload_bytes(const Context& ctx, PolyPtr& p, const void* host, size_t bytes) {
+    if (bytes && !host) throw Error(H2B_ERR_ARG, "upload: null pointer");
+    const size_t full = bytes / 32, tail = bytes % 32;
+    Poly* d = grown(ctx, p, full + (tail != 0));
+    if (full) d->upload(static_cast<const Fr*>(host), full);
+    if (tail) {
+        Fr last{};
+        std::memcpy(last.data(), static_cast<const char*>(host) + 32 * full, tail);
+        d->upload(&last, 1, full);
+    }
+    return d;
+}
+
+// ------------------------------------------------------------------------------------------------ the circuit's shape
+// What halo2-base's constraint system is for (k, A, L, selector_lookup): the one place the prover, the check, MockProver and
+// keygen read it from.  The selector lookup needs L = 0; blinding factors max(3, queries of a gate column = 4) + 2 = 6.
+struct CircuitShape {
+    CircuitShape(uint32_t k, size_t A, size_t L, bool selector_lookup)
+        : k(k), n(size_t(1) << k), A(A), L(L), selector_lookup(selector_lookup && L == 0) {
+        degree = L ? 4 : (this->selector_lookup ? 5 : 3);
+        chunk = degree - 2;
+        ext_k = k + (degree == 3 ? 1 : 2);
+        u = n - (bf + 1);
+        for (size_t j = 0; j < A; j++) adv_names.push_back("a" + std::to_string(j));
+        for (size_t t = 0; t < L; t++) adv_names.push_back("l" + std::to_string(t));
+        perm_cols.push_back("c");
+        perm_cols.insert(perm_cols.end(), adv_names.begin(), adv_names.end());
+        n_sets = (perm_cols.size() + chunk - 1) / chunk;
+        n_lookups = L ? L : (this->selector_lookup ? 1 : 0);
+        for (size_t j = 0; j < A; j++) fixed_names.push_back("q" + std::to_string(j));
+        if (this->selector_lookup) fixed_names.push_back("q_lookup");
+        if (n_lookups) fixed_names.push_back("table");
+        fixed_names.push_back("c");
+        for (auto& nm : perm_cols) sigma_names.push_back("sigma_" + nm);
+    }
+    uint32_t k, ext_k = 0;
+    size_t n, A, L;
+    bool selector_lookup;
+    size_t degree = 0, chunk = 0, n_sets = 0, n_lookups = 0, u = 0;
+    uint32_t bf = 6;
+    // adv: a0.., l0..;  perm: c, adv;  fixed: q0.., [q_lookup], [table], c;  sigma: sigma_{perm}
+    std::vector<std::string> adv_names, perm_cols, fixed_names, sigma_names;
+};
+
+// the vertical gate q (a0 + a1 a2 - a3) on fixed and advice slot `slot`, advice rotations 0..3 (flex_gate/mod.rs:80-91)
+inline ValueSource add_vertical_gate(GraphEvaluator& ev, uint32_t slot) {
+    const ValueSource q = ev.add_calculation(Calculation::Store(ValueSource::Fixed(slot, ev.add_rotation(0))));
+    ValueSource a[4];
+    for (int r = 0; r < 4; r++) a[r] = ev.add_calculation(Calculation::Store(ValueSource::Advice(slot, ev.add_rotation(r))));
+    const ValueSource sum = ev.add_calculation(Calculation::Add(a[0], ev.add_calculation(Calculation::Mul(a[1], a[2]))));
+    return ev.add_calculation(Calculation::Mul(q, ev.add_calculation(Calculation::Sub(sum, a[3]))));
+}
+
 // ------------------------------------------------------------------------------------------------ the fixed side of a circuit
-class ProverCircuit {
+class ProverCircuit : public CircuitShape {
 public:
     // fixed: Lagrange values (2^k each) by name — q0..q{A-1}, [q_lookup], [table], c; sigma: one column per permutation column
     // in the order [c, a0.., l0..]
@@ -319,22 +379,7 @@ public:
 private:
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
                   const std::vector<const Fr*>& sigma, bool on_device)
-        : ctx(ctx), k(k), n(size_t(1) << k), A(A), L(L), selector_lookup(selector_lookup && L == 0) {
-        degree = L ? 4 : (this->selector_lookup ? 5 : 3);
-        chunk = degree - 2;
-        ext_k = k + (degree == 3 ? 1 : 2);
-        bf = 6;  // max(3, queries of a gate column = 4) + 2
-        u = n - (bf + 1);
-        for (size_t j = 0; j < A; j++) adv_names.push_back("a" + std::to_string(j));
-        for (size_t t = 0; t < L; t++) adv_names.push_back("l" + std::to_string(t));
-        perm_cols.push_back("c");
-        perm_cols.insert(perm_cols.end(), adv_names.begin(), adv_names.end());
-        n_sets = (perm_cols.size() + chunk - 1) / chunk;
-        n_lookups = L ? L : (this->selector_lookup ? 1 : 0);
-        for (size_t j = 0; j < A; j++) fixed_names.push_back("q" + std::to_string(j));
-        if (this->selector_lookup) fixed_names.push_back("q_lookup");
-        if (n_lookups) fixed_names.push_back("table");
-        fixed_names.push_back("c");
+        : CircuitShape(k, A, L, selector_lookup), ctx(ctx) {
         if (sigma.size() != perm_cols.size()) throw Error(H2B_ERR_ARG, "ProverCircuit: one sigma column per permutation column");
         std::vector<Fr> l0(n, Fr{}), ll(n, Fr{}), la(n, Fr{});
         l0[0] = HostFr::one();
@@ -361,10 +406,7 @@ private:
             if (it == fixed.end()) throw Error(H2B_ERR_ARG, "ProverCircuit: missing fixed column " + nm);
             add(nm, it->second, on_device);
         }
-        for (size_t i = 0; i < perm_cols.size(); i++) {
-            sigma_names.push_back("sigma_" + perm_cols[i]);
-            add(sigma_names.back(), sigma[i], on_device);
-        }
+        for (size_t i = 0; i < perm_cols.size(); i++) add(sigma_names[i], sigma[i], on_device);
         add("l0", l0.data(), false);
         add("l_last", ll.data(), false);
         add("l_active", la.data(), false);
@@ -375,14 +417,7 @@ private:
             GateProgram gp;
             std::vector<ValueSource> parts;
             for (size_t j = j0; j < std::min(A, j0 + GATES_PER_PROGRAM); j++) {
-                const uint32_t i = uint32_t(j - j0);
-                auto adv = [&](int rot) { return gp.ev.add_calculation(Calculation::Store(ValueSource::Advice(i, gp.ev.add_rotation(rot)))); };
-                const ValueSource q = gp.ev.add_calculation(Calculation::Store(ValueSource::Fixed(i, gp.ev.add_rotation(0))));
-                const ValueSource a0 = adv(0), a1 = adv(1), a2 = adv(2), a3 = adv(3);
-                const ValueSource prod = gp.ev.add_calculation(Calculation::Mul(a1, a2));
-                const ValueSource sum = gp.ev.add_calculation(Calculation::Add(a0, prod));
-                const ValueSource diff = gp.ev.add_calculation(Calculation::Sub(sum, a3));
-                parts.push_back(gp.ev.add_calculation(Calculation::Mul(q, diff)));
+                parts.push_back(add_vertical_gate(gp.ev, uint32_t(j - j0)));
                 gp.cols.push_back(j);
             }
             gp.result = gp.ev.add_calculation(Calculation::Horner(ValueSource::PreviousValue(), parts, ValueSource::Y()));
@@ -416,12 +451,7 @@ public:
     void prepare_check() const {
         if (check_map) return;
         GraphEvaluator ev;
-        const uint32_t r0 = ev.add_rotation(0), r1 = ev.add_rotation(1), r2 = ev.add_rotation(2), r3 = ev.add_rotation(3);
-        auto adv = [&](uint32_t rot) { return ev.add_calculation(Calculation::Store(ValueSource::Advice(0, rot))); };
-        const ValueSource q = ev.add_calculation(Calculation::Store(ValueSource::Fixed(0, r0)));
-        const ValueSource a0 = adv(r0), a1 = adv(r1), a2 = adv(r2), a3 = adv(r3);
-        const ValueSource sum = ev.add_calculation(Calculation::Add(a0, ev.add_calculation(Calculation::Mul(a1, a2))));
-        const ValueSource res = ev.add_calculation(Calculation::Mul(q, ev.add_calculation(Calculation::Sub(sum, a3))));
+        const ValueSource res = add_vertical_gate(ev, 0);
         const size_t npc = perm_cols.size();
         auto map = std::make_unique<Poly>(ctx, (npc * n + 7) / 8);
         Poly rep(ctx, (2 * npc + 3) / 4);  // max_report = 1: count and first row per column
@@ -459,12 +489,6 @@ public:
         std::vector<size_t> cols;
     };
     const Context& ctx;
-    uint32_t k, ext_k = 0;
-    size_t n, A, L;
-    bool selector_lookup;
-    size_t degree = 0, chunk = 0, n_sets = 0, n_lookups = 0, u = 0;
-    uint32_t bf = 0;
-    std::vector<std::string> adv_names, perm_cols, fixed_names, sigma_names;
     std::map<std::string, PolyPtr> lagr, coeff, ext;
     std::vector<GateProgram> gate_programs;
     GraphEvaluator lookup_ev;
@@ -520,11 +544,70 @@ struct WitnessView {
     bool assigned_form() const { return n_rational || lookup_index; }
 };
 
-// ProverSession::check: per gate column, lookup and permutation column (perm_cols order) the failure count and the first
-// min(count, max_report) failing rows, ascending
+// the device side of one witness (ProverSession, MockProver): each buffer is reallocated only when a call needs more than any
+// call before it
+struct WitnessBuffers {
+    PolyPtr cells, rational_index, rational_den, lookups;  // lookups: the looked-up values or their indices
+};
+
+// phase 0 up to the advice columns (ProverSession::create_proof and check, MockProver::run): the witness, its Rational pairs and
+// its looked-up cells (values or indices) up; with `rational`, the Rational cells become n * d^-1 before anything reads the
+// witness; then the assignment into `cols` (the A gate columns, then the L lookup columns, 2^k rows each).  d_verdict[0] /
+// d_verdict[1]: the device verdict words of the Rational pairs / of the lookup indices.  random_poly (create_proof): its n
+// pinned coefficients go up into `rnd` on the side queue, beside the assignment.  Returns the bytes uploaded.
+inline size_t assign_witness(const Context& ctx, const CircuitShape& s, const WitnessView& w, bool rational, uint32_t* d_verdict, void* cols,
+                             WitnessBuffers& buf, const Fr* random_poly = nullptr, Poly* rnd = nullptr) {
+    h2b_ctx* c = ctx.raw();
+    const size_t R = w.n_rational;
+    const bool lk_indexed = s.L && w.lookup_index;
+    size_t bytes = 32 * w.n_cells;
+    upload_bytes(ctx, buf.cells, w.cells, 32 * w.n_cells);
+    if (R) {
+        upload_bytes(ctx, buf.rational_den, w.rational_den, 32 * R);
+        upload_bytes(ctx, buf.rational_index, w.rational_index, 8 * R);
+        bytes += 40 * R;
+    }
+    if (s.L) {
+        const size_t each = lk_indexed ? 8 : 32;
+        upload_bytes(ctx, buf.lookups, lk_indexed ? static_cast<const void*>(w.lookup_index) : w.lookup_cells, each * w.n_lookup);
+        bytes += each * w.n_lookup;
+    }
+    if (random_poly) {
+        ctx.check(h2b_ctx_side_begin(c));
+        rnd->upload_async(random_poly, s.n);
+        ctx.check(h2b_ctx_side_end(c));
+        bytes += 32 * s.n;
+    }
+    if (rational)  // before anything reads the witness
+        ctx.check(h2b_apply_rational_dev(c, buf.cells->at(), w.n_cells, R ? buf.rational_index->at() : nullptr, R ? buf.rational_den->at() : nullptr,
+                                         R, d_verdict));
+    ctx.check(h2b_assign_columns_dev(c, buf.cells->at(), w.n_cells, w.n_break_points ? w.break_points : nullptr, w.n_break_points, s.k, s.A, cols));
+    void* lk_cols = static_cast<char*>(cols) + 32 * s.A * s.n;
+    if (lk_indexed)
+        ctx.check(h2b_assign_lookups_indexed_dev(c, buf.cells->at(), w.n_cells, buf.lookups->at(), w.n_lookup, s.k, s.L, lk_cols, d_verdict + 1));
+    else if (s.L)
+        ctx.check(h2b_assign_lookups_dev(c, buf.lookups->at(), w.n_lookup, s.k, s.L, lk_cols));
+    return bytes;
+}
+
+// (failure count, the first min(count, max_report) failing rows or equality indices, ascending)
+using ReportItem = std::pair<uint64_t, std::vector<uint64_t>>;
+// n_items reports as the check kernels write them, max_report + 1 words each (the count, then the rows); a failure clears
+// `satisfied`
+inline std::vector<ReportItem> decode_reports(const uint64_t* w, size_t n_items, size_t max_report, bool& satisfied) {
+    std::vector<ReportItem> out;
+    for (size_t i = 0; i < n_items; i++) {
+        const uint64_t* r = w + (max_report + 1) * i;
+        out.push_back({r[0], std::vector<uint64_t>(r + 1, r + 1 + std::min<uint64_t>(r[0], max_report))});
+        satisfied = satisfied && r[0] == 0;
+    }
+    return out;
+}
+
+// ProverSession::check: per gate column, lookup and permutation column (perm_cols order) a report
 struct CheckReport {
     bool satisfied = true;
-    std::vector<std::pair<uint64_t, std::vector<uint64_t>>> gates, lookups, copies;
+    std::vector<ReportItem> gates, lookups, copies;
 };
 
 struct Proof {
@@ -545,8 +628,8 @@ public:
 
     ProverSession(const Context& ctx, const ParamsKZG& params, const ProverCircuit& cs) : ctx(ctx), params(params), cs(cs), n_loc(cs.n) {
         const size_t n = cs.n, ne = size_t(1) << cs.ext_k;
-        v = std::make_unique<Poly>(ctx, n * cs.A);
-        if (cs.L) lkv = std::make_unique<Poly>(ctx, n * cs.L);
+        witness_bufs.cells = std::make_unique<Poly>(ctx, n * cs.A);  // steady-state proofs allocate nothing
+        if (cs.L) witness_bufs.lookups = std::make_unique<Poly>(ctx, n * cs.L);
         adv_block = std::make_unique<Poly>(ctx, n * (cs.A + cs.L));
         for (size_t j = 0; j < cs.adv_names.size(); j++) lagr[cs.adv_names[j]] = ColRef{adv_block.get(), j * n};
         std::vector<std::string> names = cs.adv_names;
@@ -655,8 +738,8 @@ public:
             }
         };
 
-        // ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside it)
-        assign_witness(wit, random_poly, res.h2d_bytes);
+        // ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside them)
+        res.h2d_bytes += assign_witness(ctx, cs, wit, wit.assigned_form(), verdict_words(), adv_block->at(), witness_bufs, random_poly, rnd);
         std::vector<std::pair<int, ColRef>> items;
         for (auto& nm : cs.adv_names) {
             blind_col(lagr[nm], u);
@@ -743,8 +826,8 @@ public:
                 fx.push_back(cs.ext.at("q" + std::to_string(j))->at());
                 ad.push_back(ext["a" + std::to_string(j)]->at());
             }
-            const h2b_graph g = bind(gp.ev, gp.result, fx, ad, ch);
-            ctx.check(h2b_quotient_graph_dev(c, &g, k, ext_k, h->at()));
+            const BoundGraph g(gp.ev, gp.result, fx, ad, ch);
+            ctx.check(h2b_quotient_graph_dev(c, g.get(), k, ext_k, h->at()));
         }
         {
             std::vector<const void*> tz, tc, ts;
@@ -767,8 +850,8 @@ public:
                 fx = {cs.ext.at("table")->at()};
                 ad = {ext["l" + ts]->at()};
             }
-            const h2b_graph g = bind(cs.lookup_ev, cs.lookup_result, fx, ad, ch);
-            ctx.check(h2b_lookup_fold_dev(c, &g, ext["zl" + ts]->at(), ext["pa" + ts]->at(), ext["ps" + ts]->at(), cs.ext.at("l0")->at(),
+            const BoundGraph g(cs.lookup_ev, cs.lookup_result, fx, ad, ch);
+            ctx.check(h2b_lookup_fold_dev(c, g.get(), ext["zl" + ts]->at(), ext["pa" + ts]->at(), ext["ps" + ts]->at(), cs.ext.at("l0")->at(),
                                           cs.ext.at("l_last")->at(), cs.ext.at("l_active")->at(), k, ext_k, h->at()));
         }
         ctx.check(h2b_divide_by_vanishing_poly_dev(c, h->at(), k, ext_k));
@@ -908,19 +991,17 @@ public:
         check_inputs(wit, "check");
         if (max_report < 1 || max_report > H2B_CHECK_MAX_REPORT) throw Error(H2B_ERR_ARG, "check: max_report out of range");
         cs.prepare_check();
-        size_t h2d = 0;
-        assign_witness(wit, nullptr, h2d);
-        Poly* zero_rows = grown(check_zero, n - u);  // zero-filled, never written
+        assign_witness(ctx, cs, wit, wit.assigned_form(), verdict_words(), adv_block->at(), witness_bufs);
+        Poly* zero_rows = grown(ctx, check_zero, n - u);  // zero-filled, never written
         for (auto& nm : cs.adv_names) ctx.check(h2b_poly_copy_dev(c, lagr[nm].ptr(u), zero_rows->at(), n - u));
         // report block: element 0 = the witness-form verdict words, then max_report + 1 words per gate, lookup, permutation column
         const size_t W = max_report + 1, npc = cs.perm_cols.size(), n_items = A + cs.n_lookups + npc, elems = 1 + (n_items * W + 3) / 4;
-        Poly* rep = grown(check_rep, elems);
+        Poly* rep = grown(ctx, check_rep, elems);
         auto at = [&](size_t i) { return static_cast<char*>(rep->at(1)) + 8 * W * i; };
-        if (wit.assigned_form()) ctx.check(h2b_poly_copy_dev(c, rep->at(), d_out->at(48), 1));
+        if (wit.assigned_form()) ctx.check(h2b_poly_copy_dev(c, rep->at(), verdict_words(), 1));
         for (size_t j = 0; j < A; j++) {
-            const h2b_graph g = bind(cs.check_ev, cs.check_result, {cs.lagr.at("q" + std::to_string(j))->at()}, {lagr["a" + std::to_string(j)].ptr()},
-                                     Challenges{});
-            check_graph_dev(ctx, g, k, u, max_report, at(j));
+            const BoundGraph g(cs.check_ev, cs.check_result, {cs.lagr.at("q" + std::to_string(j))->at()}, {lagr["a" + std::to_string(j)].ptr()});
+            check_graph_dev(ctx, *g.get(), k, u, max_report, at(j));
         }
         for (size_t t = 0; t < cs.n_lookups; t++) {
             const void* in = lagr[L ? "l" + std::to_string(t) : "a0"].ptr();
@@ -940,12 +1021,10 @@ public:
             if (rat_bad || lk_bad) witness_error(rat_bad, lk_bad, "check");
         }
         CheckReport out;
-        for (size_t i = 0; i < n_items; i++) {
-            const uint64_t* r = w + 4 + W * i;
-            std::pair<uint64_t, std::vector<uint64_t>> e{r[0], std::vector<uint64_t>(r + 1, r + 1 + std::min<uint64_t>(r[0], max_report))};
-            out.satisfied = out.satisfied && r[0] == 0;
-            (i < A ? out.gates : i < A + cs.n_lookups ? out.lookups : out.copies).push_back(std::move(e));
-        }
+        const std::vector<ReportItem> items = decode_reports(w + 4, n_items, max_report, out.satisfied);
+        out.gates.assign(items.begin(), items.begin() + A);
+        out.lookups.assign(items.begin() + A, items.begin() + A + cs.n_lookups);
+        out.copies.assign(items.begin() + A + cs.n_lookups, items.end());
         return out;
     }
 
@@ -997,88 +1076,11 @@ private:
         if (lk_bad & 1) why += "; a lookup index is >= the witness length";
         throw Error(H2B_ERR_ARG, who + why);
     }
-    // phase 0 up to the advice columns in adv_block (what create_proof and check share): witness, Rational pairs and lookup
-    // indices or looked-up values up, Rational cells -> n * d^-1, the assignment; with the halo2-base form the verdict words
-    // land in element 48 of d_out.  random_poly != nullptr: it goes up on the side queue, beside the assignment.
-    void assign_witness(const WitnessView& w, const Fr* random_poly, size_t& h2d_bytes) {
-        const uint32_t k = cs.k;
-        const size_t n = cs.n, A = cs.A, L = cs.L, R = w.n_rational;
-        h2b_ctx* c = ctx.raw();
-        const bool lk_indexed = L && w.lookup_index;
-        v->upload(w.cells, w.n_cells);
-        h2d_bytes += w.n_cells * 32;
-        if (R) {
-            grown(rat_den, R)->upload(w.rational_den, R);
-            h2d_bytes += R * 32;
-            upload_u64(rat_idx, w.rational_index, R, h2d_bytes);
-        }
-        if (lk_indexed) {
-            upload_u64(lk_idx, w.lookup_index, w.n_lookup, h2d_bytes);
-        } else if (L) {
-            lkv->upload(w.lookup_cells, w.n_lookup);
-            h2d_bytes += w.n_lookup * 32;
-        }
-        if (random_poly) {
-            ctx.check(h2b_ctx_side_begin(c));
-            rnd->upload_async(random_poly, n);
-            ctx.check(h2b_ctx_side_end(c));
-            h2d_bytes += n * 32;
-        }
-        uint32_t* d_verdict = static_cast<uint32_t*>(d_out->at(48));
-        if (w.assigned_form())  // zeroes both verdict words, then the Rational cells become n * d^-1 before anything reads the witness
-            ctx.check(h2b_apply_rational_dev(c, v->at(), w.n_cells, R ? rat_idx->at() : nullptr, R ? rat_den->at() : nullptr, R, d_verdict));
-        ctx.check(h2b_assign_columns_dev(c, v->at(), w.n_cells, w.n_break_points ? w.break_points : nullptr, w.n_break_points, k, A, adv_block->at()));
-        if (lk_indexed)
-            ctx.check(h2b_assign_lookups_indexed_dev(c, v->at(), w.n_cells, lk_idx->at(), w.n_lookup, k, L, adv_block->at(A * n), d_verdict + 1));
-        else if (L)
-            ctx.check(h2b_assign_lookups_dev(c, lkv->at(), w.n_lookup, k, L, adv_block->at(A * n)));
-    }
+    // phase 0 of the halo2-base witness form: the verdict words, read with the first download of its commitments
+    uint32_t* verdict_words() const { return static_cast<uint32_t*>(d_out->at(48)); }
     Poly* own(size_t m) {
         owned.push_back(std::make_unique<Poly>(ctx, m));
         return owned.back().get();
-    }
-    // a buffer of the halo2-base witness form: reallocated only when a proof needs more than any proof before it
-    Poly* grown(PolyPtr& p, size_t m) {
-        if (!p || p->len() < m) p = std::make_unique<Poly>(ctx, std::max<size_t>(m, 1));
-        return p.get();
-    }
-    // count uint64 words: whole 32-byte elements straight from the caller's array, the last 1..3 words through a zero-padded
-    // element (nothing past the end of the caller's array is read)
-    void upload_u64(PolyPtr& p, const uint64_t* words, size_t count, size_t& h2d_bytes) {
-        Poly* d = grown(p, (count + 3) / 4);
-        const size_t full = count / 4;
-        if (full) d->upload(reinterpret_cast<const Fr*>(words), full);
-        if (count % 4) {
-            Fr tail{};
-            std::memcpy(tail.data(), words + 4 * full, 8 * (count % 4));
-            d->upload(&tail, 1, full);
-        }
-        h2d_bytes += count * 8;
-    }
-    // the arrays an h2b_graph points to live in `hold` until the next bind()
-    h2b_graph bind(const GraphEvaluator& ev, ValueSource result, const std::vector<const void*>& fixed, const std::vector<const void*>& advice,
-                   const Challenges& ch) {
-        hold_prog = ev.program();
-        hold_fixed = fixed;
-        hold_advice = advice;
-        h2b_graph g{};
-        g.program = hold_prog.data();
-        g.program_words = hold_prog.size();
-        g.n_calculations = uint32_t(ev.calculations.size());
-        g.result = result.word();
-        g.constants = reinterpret_cast<const uint64_t*>(ev.constants.data());
-        g.n_constants = ev.constants.size();
-        g.rotations = ev.rotations.data();
-        g.n_rotations = ev.rotations.size();
-        g.fixed = hold_fixed.data();
-        g.n_fixed = hold_fixed.size();
-        g.advice = hold_advice.data();
-        g.n_advice = hold_advice.size();
-        std::copy(ch.beta.begin(), ch.beta.end(), g.beta);
-        std::copy(ch.gamma.begin(), ch.gamma.end(), g.gamma);
-        std::copy(ch.theta.begin(), ch.theta.end(), g.theta);
-        std::copy(ch.y.begin(), ch.y.end(), g.y);
-        return g;
     }
 
     const Context& ctx;
@@ -1087,16 +1089,14 @@ private:
     size_t shard_begin = 0, n_loc;  // shard()
     AllReduce allreduce;
     std::vector<PolyPtr> owned;
-    PolyPtr v, lkv, adv_block;
-    PolyPtr rat_den, rat_idx, lk_idx;  // the halo2-base witness form
+    WitnessBuffers witness_bufs;
+    PolyPtr adv_block;
     PolyPtr check_zero, check_rep;     // check(): zero rows, the report block
     std::map<std::string, ColRef> lagr;
     std::map<std::string, Poly*> coef, ext;
     Poly *inp = nullptr, *rnd = nullptr, *h = nullptr, *d_out = nullptr, *d_status = nullptr, *zero = nullptr;
     std::array<Poly*, 4> tmp{};
     std::array<Poly*, 3> tmp_side{};
-    std::vector<uint32_t> hold_prog;
-    std::vector<const void*> hold_fixed, hold_advice;
 };
 
 }  // namespace h2b
