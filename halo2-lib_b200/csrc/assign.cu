@@ -140,15 +140,6 @@ __global__ void __launch_bounds__(256) k_apply_rational(uint64_t* __restrict__ v
     (Fr::load(values + 4 * idx) * Fr::load_nc(den_inv + 4 * i)).store(values + 4 * idx);
 }
 
-// Assigned::Rational(num, den) -> num * den^-1 (den = 0 -> 0), what batch_invert_assigned produces
-__global__ void __launch_bounds__(128) k_eval_rational(const uint64_t* __restrict__ num, const uint64_t* __restrict__ den,
-                                                       u32 n, uint64_t* __restrict__ out) {
-    u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    Fr d = Fr::load_nc(den + 4 * (size_t)i).inv();
-    (Fr::load_nc(num + 4 * (size_t)i) * d).store(out + 4 * (size_t)i);
-}
-
 // the spans of the ncols columns the walk fills: column c holds V[s_c .. s_c + len_c); columns the walk does not reach are empty
 static std::vector<ColSpan> column_spans(size_t N, const uint64_t* break_points, size_t nbp, size_t rows, size_t ncols) {
     std::vector<ColSpan> spans(ncols, ColSpan{0, 0});
@@ -312,11 +303,6 @@ void apply_rational_run(h2b_ctx* ctx, void* d_values, size_t N, const uint64_t* 
     if (R == 0) return;
     batch_invert_run(ctx, d_den, R);
     H2B_LAUNCH(ctx, k_apply_rational, ceil_div(R, 256), 256, 0, (uint64_t*)d_values, N, d_index, (const uint64_t*)d_den, R, d_status);
-}
-
-void eval_rational_run(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out) {
-    if (n == 0) return;
-    H2B_LAUNCH(ctx, k_eval_rational, ceil_div(n, 128), 128, 0, (const uint64_t*)d_num, (const uint64_t*)d_den, (u32)n, (uint64_t*)d_out);
 }
 
 }  // namespace h2b

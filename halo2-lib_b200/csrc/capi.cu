@@ -54,30 +54,6 @@ cudaEvent_t h2b_ctx::prof_event() {
     return e;
 }
 
-// Runs `body` under the context lock with the context's device current; translates every failure.
-template <class Fn>
-static int guarded(h2b_ctx* ctx, Fn&& body) {
-    if (!ctx) return H2B_ERR_ARG;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    try {
-        H2B_CUDA(cudaSetDevice(ctx->device));
-        body();
-        return H2B_OK;
-    } catch (const StatusError& e) {
-        ctx->err = e.msg;
-        return e.code;
-    } catch (const std::bad_alloc&) {
-        ctx->err = "host allocation failed";
-        return H2B_ERR_OOM;
-    } catch (const std::exception& e) {
-        ctx->err = e.what();
-        return H2B_ERR_CUDA;
-    } catch (...) {
-        ctx->err = "unknown failure";
-        return H2B_ERR_CUDA;
-    }
-}
-
 // ---- device group helpers (h2b_ctx_create_multi): run `fn(member, index)` with the member's device current
 template <class Fn>
 static void group_each(h2b_ctx* ctx, Fn&& fn) {
@@ -94,6 +70,128 @@ static std::vector<T> every_gth(T const* v, size_t m, size_t g, size_t G) {
     return r;
 }
 
+// The staging of a host-pointer entry point, which is its `_dev` form run on copies of the host buffers: one ctx->get of
+// `bytes` in `slot` (the slot keeps the copies apart from the scratch the `*_run` function takes), carved into the
+// inputs, scratch and outputs of the call.  Uploads are enqueued on ctx->stream as the regions are carved; finish()
+// enqueues the downloads of the output regions and synchronises once.
+namespace {
+struct Staging {
+    struct Download {
+        void* host;
+        const void* dev;
+        size_t bytes;
+    };
+    h2b_ctx* ctx;
+    char* base;
+    size_t used = 0, cap;
+    std::vector<Download> downloads;
+    Staging(h2b_ctx* c, int slot, size_t bytes) : ctx(c), cap(bytes) { base = (char*)c->get(slot, bytes); }
+    // the next `bytes` of the slot, 32-byte aligned
+    char* take(size_t bytes) {
+        const size_t at = (used + 31) & ~(size_t)31;
+        H2B_REQUIRE(at + bytes <= cap, "staging overflow");
+        used = at + bytes;
+        return base + at;
+    }
+    // an input: `bytes` from the host, uploaded into the next `room` (at least `bytes`) bytes of the slot
+    char* up(const void* host, size_t bytes, size_t room = 0) {
+        char* d = take(room > bytes ? room : bytes);
+        if (bytes) H2B_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        return d;
+    }
+    // an output: the first `bytes` of the next `room` (at least `bytes`) bytes go to `host` (nowhere when it is null)
+    char* out(void* host, size_t bytes, size_t room = 0) {
+        char* d = take(room > bytes ? room : bytes);
+        if (host && bytes) downloads.push_back({host, d, bytes});
+        return d;
+    }
+    // an input that is also the output
+    char* inout(void* host, size_t bytes) {
+        char* d = up(host, bytes);
+        if (bytes) downloads.push_back({host, d, bytes});
+        return d;
+    }
+    void finish() {
+        for (auto& x : downloads) H2B_CUDA(cudaMemcpyAsync(x.host, x.dev, x.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+};
+}  // namespace
+
+// Every stream and event a context owns, in one list that h2b_ctx_create creates and h2b_ctx_destroy destroys.  Three
+// stream priority levels.  Highest: the bucket reduction of a lane's MSM — its few CTAs take the SM slots that free up
+// first instead of queueing behind the next MSM's accumulation waves (see msm_run_group).  Middle: the lanes and the
+// context's own stream.  Lowest (the default of a plain stream): the copy streams, the side queue and whatever else the
+// caller runs beside the commitments — the polynomial transforms fill the bubbles the MSM pipeline leaves.
+enum StreamPrio { PRIO_DEFAULT, PRIO_LANE, PRIO_TAIL };
+template <class Stream, class Event>
+static void ctx_handles(h2b_ctx* ctx, Stream&& stream, Event&& event) {
+    stream(ctx->own_stream, PRIO_LANE);
+    stream(ctx->copy_stream, PRIO_DEFAULT);
+    stream(ctx->copy_stream2, PRIO_DEFAULT);
+    stream(ctx->side_stream, PRIO_DEFAULT);
+    for (auto& e : ctx->side_ev) event(e);
+    for (auto& row : ctx->pipe_ev)
+        for (auto& e : row) event(e);
+    for (auto& e : ctx->ev) event(e);
+    for (int l = 0; l < h2b_ctx::NLANES; l++) {
+        stream(ctx->lane_stream[l], PRIO_LANE);
+        stream(ctx->lane_tail[l], PRIO_TAIL);
+        event(ctx->lane_acc[l]);
+        event(ctx->lane_tail_done[l]);
+        event(ctx->lane_done[l]);
+        event(ctx->lane_ready[l]);
+        event(ctx->lane_consumed[l]);
+    }
+    event(ctx->fork_ev);
+}
+static void destroy_handles(h2b_ctx* ctx) {
+    ctx_handles(ctx, [](cudaStream_t& s, StreamPrio) { if (s) cudaStreamDestroy(s); }, [](cudaEvent_t& e) { if (e) cudaEventDestroy(e); });
+}
+
+// m columns through three rotating buffer sets: the upload of column i+1 (copy stream) and the downloads of column i-1
+// (second copy stream) overlap the kernels of column i (context stream).  Column i uses set b = i mod 3: it is uploaded
+// from in[i] into up_buf[b], `compute(i, b)` enqueues its kernels, and `download(i, b, down)` waits for pipe_ev[b][1]
+// (or an earlier event of the context stream) before each copy it enqueues.  Enqueue only: see ntt_batch_finish.
+template <class Compute, class Download>
+static void ntt_pipeline(h2b_ctx* ctx, const uint64_t* const* in, size_t m, void* const up_buf[3], size_t up_bytes, Compute&& compute,
+                         Download&& download) {
+    cudaStream_t up = ctx->copy_stream, ks = ctx->stream, down = ctx->copy_stream2;
+    H2B_CUDA(cudaEventRecord(ctx->fork_ev, ks));
+    H2B_CUDA(cudaStreamWaitEvent(up, ctx->fork_ev, 0));
+    for (size_t i = 0; i < m; i++) {
+        const int b = (int)(i % 3);
+        if (i >= 3) H2B_CUDA(cudaStreamWaitEvent(up, ctx->pipe_ev[b][2], 0));  // buffer set b downloaded
+        H2B_CUDA(cudaMemcpyAsync(up_buf[b], in[i], up_bytes, cudaMemcpyHostToDevice, up));
+        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][0], up));
+        H2B_CUDA(cudaStreamWaitEvent(ks, ctx->pipe_ev[b][0], 0));
+        compute(i, b);
+        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][1], ks));
+        download(i, b, down);
+        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][2], down));
+    }
+}
+static void ntt_batch_finish(h2b_ctx* ctx) {
+    H2B_CUDA(cudaStreamSynchronize(ctx->copy_stream2));
+    H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+// One batch per device: on a device group (h2b_ctx_create_multi) polynomial j goes to device j mod G ("one column
+// polynomial per device", SURVEY.md §8e), and every device's pipeline is enqueued before the first wait.
+template <class In, class Out, class Batch>
+static void ntt_deal(h2b_ctx* ctx, In const* in, Out const* out, size_t m, Batch&& batch) {
+    if (ctx->members.size() <= 1) {
+        batch(ctx, in, out, m);
+        return ntt_batch_finish(ctx);
+    }
+    const size_t G = ctx->members.size();
+    group_each(ctx, [&](h2b_ctx* mb, size_t g) {
+        auto vi = every_gth(in, m, g, G);
+        auto vo = every_gth(out, m, g, G);
+        batch(mb, vi.data(), vo.data(), vi.size());
+    });
+    group_each(ctx, [&](h2b_ctx* mb, size_t) { ntt_batch_finish(mb); });
+}
+
 extern "C" {
 
 const char* h2b_version(void) { return "h2b200 0.1.0 (sm_90a)"; }
@@ -103,6 +201,7 @@ int h2b_ctx_create(int device, h2b_ctx** out) {
     *out = nullptr;
     std::lock_guard<std::mutex> lock(g_create_mu);
     h2b_ctx* ctx = nullptr;
+    int rc = H2B_OK;
     try {
         int ndev = 0;
         cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -113,35 +212,12 @@ int h2b_ctx_create(int device, h2b_ctx** out) {
         H2B_CUDA(cudaSetDevice(device));
         ctx = new h2b_ctx();
         ctx->device = device;
-        {   // the context's own stream sits at the lanes' priority: above the side queue (see the lane streams below)
-            int lo_prio = 0, hi_prio = 0;
-            H2B_CUDA(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
-            H2B_CUDA(cudaStreamCreateWithPriority(&ctx->own_stream, cudaStreamNonBlocking, (lo_prio + hi_prio) / 2));
-        }
-        H2B_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-        H2B_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream2, cudaStreamNonBlocking));
-        H2B_CUDA(cudaStreamCreateWithFlags(&ctx->side_stream, cudaStreamNonBlocking));
-        for (auto& e : ctx->side_ev) H2B_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        for (auto& row : ctx->pipe_ev)
-            for (auto& e : row) H2B_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        for (auto& ev : ctx->ev) H2B_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        for (int l = 0; l < h2b_ctx::NLANES; l++) {
-            {   // Three priority levels.  Highest: the bucket reduction of a lane's MSM — its few CTAs take the SM slots that
-                // free up first instead of queueing behind the next MSM's accumulation waves (see msm_run_group).  Middle: the
-                // lanes themselves.  Lowest (the default of a plain stream): the side queue and whatever else the caller runs
-                // beside the commitments — the polynomial transforms fill the bubbles the MSM pipeline leaves.
-                int lo_prio = 0, hi_prio = 0;
-                H2B_CUDA(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
-                H2B_CUDA(cudaStreamCreateWithPriority(&ctx->lane_stream[l], cudaStreamNonBlocking, (lo_prio + hi_prio) / 2));
-                H2B_CUDA(cudaStreamCreateWithPriority(&ctx->lane_tail[l], cudaStreamNonBlocking, hi_prio));
-            }
-            H2B_CUDA(cudaEventCreateWithFlags(&ctx->lane_acc[l], cudaEventDisableTiming));
-            H2B_CUDA(cudaEventCreateWithFlags(&ctx->lane_tail_done[l], cudaEventDisableTiming));
-            H2B_CUDA(cudaEventCreateWithFlags(&ctx->lane_done[l], cudaEventDisableTiming));
-            H2B_CUDA(cudaEventCreateWithFlags(&ctx->lane_ready[l], cudaEventDisableTiming));
-            H2B_CUDA(cudaEventCreateWithFlags(&ctx->lane_consumed[l], cudaEventDisableTiming));
-        }
-        H2B_CUDA(cudaEventCreateWithFlags(&ctx->fork_ev, cudaEventDisableTiming));
+        int lo_prio = 0, hi_prio = 0;
+        H2B_CUDA(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
+        ctx_handles(ctx, [&](cudaStream_t& s, StreamPrio p) {
+            if (p == PRIO_DEFAULT) H2B_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+            else H2B_CUDA(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, p == PRIO_LANE ? (lo_prio + hi_prio) / 2 : hi_prio));
+        }, [](cudaEvent_t& e) { H2B_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); });
         ctx->stream = ctx->own_stream;
         cudaDeviceProp prop;
         H2B_CUDA(cudaGetDeviceProperties(&prop, device));
@@ -150,13 +226,14 @@ int h2b_ctx_create(int device, h2b_ctx** out) {
         return H2B_OK;
     } catch (const StatusError& e) {
         g_create_error = e.msg;
-        delete ctx;
-        return e.code;
+        rc = e.code;
     } catch (...) {
         g_create_error = "unknown failure in h2b_ctx_create";
-        delete ctx;
-        return H2B_ERR_CUDA;
+        rc = H2B_ERR_CUDA;
     }
+    if (ctx) destroy_handles(ctx);  // the streams and events created before the failure
+    delete ctx;
+    return rc;
 }
 
 // One process, several GPUs (SURVEY.md §8(b): h2b_ctx_create(const int* dev_ids, int n_dev, ...)): the returned handle is
@@ -168,35 +245,31 @@ int h2b_ctx_create_multi(const int* dev_ids, int n_dev, h2b_ctx** out) {
     if (!out || !dev_ids || n_dev < 1 || n_dev > 16) return H2B_ERR_ARG;
     *out = nullptr;
     std::vector<h2b_ctx*> made;
-    for (int i = 0; i < n_dev; i++) {
-        for (int j = 0; j < i; j++)
-            if (dev_ids[j] == dev_ids[i]) {
-                std::lock_guard<std::mutex> lock(g_create_mu);
-                g_create_error = "ctx_create_multi: duplicate device id";
-                for (auto* c : made) h2b_ctx_destroy(c);
-                return H2B_ERR_ARG;
-            }
-        h2b_ctx* c = nullptr;
-        int rc = h2b_ctx_create(dev_ids[i], &c);
-        if (rc != H2B_OK) {
-            for (auto* m : made) h2b_ctx_destroy(m);
-            return rc;
-        }
-        made.push_back(c);
-    }
-    h2b_ctx* lead = made[0];
-    lead->members = made;
-    if (n_dev > 1) {
-        int rc = guarded(lead, [&] { peer_connect_local(lead->members); });
-        if (rc != H2B_OK) {
+    int rc = H2B_OK;
+    for (int i = 0; i < n_dev && rc == H2B_OK; i++) {
+        if (std::find(dev_ids, dev_ids + i, dev_ids[i]) != dev_ids + i) {
             std::lock_guard<std::mutex> lock(g_create_mu);
-            g_create_error = lead->err;
-            lead->members.clear();
-            for (auto* m : made) h2b_ctx_destroy(m);
-            return rc;
+            g_create_error = "ctx_create_multi: duplicate device id";
+            rc = H2B_ERR_ARG;
+        } else {
+            h2b_ctx* c = nullptr;
+            rc = h2b_ctx_create(dev_ids[i], &c);  // on failure it has set the message
+            if (rc == H2B_OK) made.push_back(c);
         }
     }
-    *out = lead;
+    if (rc == H2B_OK) {
+        made[0]->members = made;
+        if (n_dev > 1 && (rc = guarded(made[0], [&] { peer_connect_local(made); })) != H2B_OK) {
+            std::lock_guard<std::mutex> lock(g_create_mu);
+            g_create_error = made[0]->err;
+            made[0]->members.clear();  // every context is destroyed on its own below
+        }
+    }
+    if (rc != H2B_OK) {
+        for (auto* m : made) h2b_ctx_destroy(m);
+        return rc;
+    }
+    *out = made[0];
     return H2B_OK;
 }
 int h2b_ctx_device_count(const h2b_ctx* ctx) { return ctx ? (int)(ctx->members.empty() ? 1 : ctx->members.size()) : 0; }
@@ -215,31 +288,11 @@ void h2b_ctx_destroy(h2b_ctx* ctx) {
     for (auto& lane : ctx->ws)
         for (auto& b : lane)
             if (b.p) cudaFree(b.p);
-    for (int l = 0; l < h2b_ctx::NLANES; l++) {
-        if (ctx->lane_stream[l]) cudaStreamDestroy(ctx->lane_stream[l]);
-        if (ctx->lane_tail[l]) cudaStreamDestroy(ctx->lane_tail[l]);
-        if (ctx->lane_acc[l]) cudaEventDestroy(ctx->lane_acc[l]);
-        if (ctx->lane_tail_done[l]) cudaEventDestroy(ctx->lane_tail_done[l]);
-        if (ctx->lane_done[l]) cudaEventDestroy(ctx->lane_done[l]);
-        if (ctx->lane_ready[l]) cudaEventDestroy(ctx->lane_ready[l]);
-        if (ctx->lane_consumed[l]) cudaEventDestroy(ctx->lane_consumed[l]);
-    }
-    if (ctx->fork_ev) cudaEventDestroy(ctx->fork_ev);
     for (auto& b : ctx->pinned)
         if (b.p) cudaFreeHost(b.p);
-    for (auto& ev : ctx->ev)
-        if (ev) cudaEventDestroy(ev);
     for (auto& r : ctx->prof_recs) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
     for (auto& e : ctx->prof_pool) cudaEventDestroy(e);
-    if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
-    if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-    if (ctx->copy_stream2) cudaStreamDestroy(ctx->copy_stream2);
-    if (ctx->side_stream) cudaStreamDestroy(ctx->side_stream);
-    for (auto& e : ctx->side_ev)
-        if (e) cudaEventDestroy(e);
-    for (auto& row : ctx->pipe_ev)
-        for (auto& e : row)
-            if (e) cudaEventDestroy(e);
+    destroy_handles(ctx);
     delete ctx;
 }
 
@@ -358,6 +411,25 @@ int h2b_profile_dump(h2b_ctx* ctx, void* origin_cuda_event, const char* path) {
 }
 
 // ------------------------------------------------------------------------------------------------ SRS
+// Frees a handle and its tables; a device group's parts each on their own device once that device is idle.  The caller
+// holds the context lock.
+static void srs_free(h2b_ctx* ctx, h2b_srs* s) {
+    for (size_t i = 0; i < s->parts.size(); i++) {
+        cudaSetDevice(ctx->members[i]->device);
+        cudaDeviceSynchronize();
+        for (auto& t : s->parts[i]->table)
+            if (t) cudaFree(t);
+        delete s->parts[i];
+    }
+    if (ctx) {
+        cudaSetDevice(ctx->device);
+        cudaDeviceSynchronize();
+    }
+    for (auto& t : s->table)
+        if (t) cudaFree(t);
+    delete s;
+}
+
 static void srs_build(h2b_ctx* ctx, const void* d_g, const void* d_gl, uint32_t k, size_t begin, size_t count, h2b_srs** out) {
     H2B_REQUIRE(out, "srs: null output handle");
     H2B_REQUIRE(k <= 27, "srs: k out of range");
@@ -378,67 +450,49 @@ static void srs_build(h2b_ctx* ctx, const void* d_g, const void* d_gl, uint32_t 
         }
         H2B_CUDA(cudaStreamSynchronize(ctx->stream));
     } catch (...) {
-        for (auto& t : s->table)
-            if (t) cudaFree(t);
-        delete s;
+        srs_free(ctx, s);
         throw;
     }
     *out = s;
+}
+// rows [begin, begin + count) of the host bases g / g_lagrange (either may be null) staged in WS_BASES / WS_MISC2, then built
+static void srs_stage_build(h2b_ctx* ctx, const uint64_t* g, const uint64_t* g_lagrange, uint32_t k, size_t begin, size_t count,
+                            h2b_srs** out) {
+    const uint64_t* host[2] = {g, g_lagrange};
+    const int slot[2] = {WS_BASES, WS_MISC2};
+    const void* dev[2] = {nullptr, nullptr};
+    for (int b = 0; b < 2; b++)
+        if (host[b]) dev[b] = Staging(ctx, slot[b], count * 64).up(host[b] + 8 * begin, count * 64);
+    srs_build(ctx, dev[0], dev[1], k, begin, count, out);
 }
 
 int h2b_srs_upload(h2b_ctx* ctx, const uint64_t* g, const uint64_t* g_lagrange, uint32_t k, size_t begin, size_t count,
                    h2b_srs** out) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(k <= 27 && count >= 1 && begin + count <= ((size_t)1 << k), "srs: bad shard");
-        if (ctx->members.size() > 1) {  // device group: contiguous index ranges, one per device
-            H2B_REQUIRE(out, "srs: null output handle");
-            const size_t G = ctx->members.size();
-            H2B_REQUIRE(count >= G, "srs: fewer bases than devices");
-            h2b_srs* top = new h2b_srs();
-            top->k = k;
-            top->begin = begin;
-            top->count = count;
-            try {
-                group_each(ctx, [&](h2b_ctx* mb, size_t i) {
-                    const size_t lo = begin + count * i / G, hi = begin + count * (i + 1) / G;
-                    const uint64_t* host[2] = {g, g_lagrange};
-                    void* dev[2] = {nullptr, nullptr};
-                    int slot[2] = {WS_BASES, WS_MISC2};
-                    for (int b = 0; b < 2; b++) {
-                        if (!host[b]) continue;
-                        dev[b] = mb->get(slot[b], (hi - lo) * 64);
-                        H2B_CUDA(cudaMemcpyAsync(dev[b], host[b] + 8 * lo, (hi - lo) * 64, cudaMemcpyHostToDevice, mb->stream));
-                    }
-                    h2b_srs* part = nullptr;
-                    srs_build(mb, dev[0], dev[1], k, lo, hi - lo, &part);
-                    top->parts.push_back(part);
-                });
-            } catch (...) {
-                cudaSetDevice(ctx->device);
-                for (size_t i = 0; i < top->parts.size(); i++) {
-                    cudaSetDevice(ctx->members[i]->device);
-                    for (auto& t : top->parts[i]->table)
-                        if (t) cudaFree(t);
-                    delete top->parts[i];
-                }
-                cudaSetDevice(ctx->device);
-                delete top;
-                throw;
-            }
-            top->c = top->parts[0]->c;
-            top->W = top->parts[0]->W;
-            *out = top;
-            return;
+        if (ctx->members.size() <= 1) return srs_stage_build(ctx, g, g_lagrange, k, begin, count, out);
+        // device group: contiguous index ranges, one per device
+        H2B_REQUIRE(out, "srs: null output handle");
+        const size_t G = ctx->members.size();
+        H2B_REQUIRE(count >= G, "srs: fewer bases than devices");
+        h2b_srs* top = new h2b_srs();
+        top->k = k;
+        top->begin = begin;
+        top->count = count;
+        try {
+            group_each(ctx, [&](h2b_ctx* mb, size_t i) {
+                const size_t lo = begin + count * i / G, hi = begin + count * (i + 1) / G;
+                h2b_srs* part = nullptr;
+                srs_stage_build(mb, g, g_lagrange, k, lo, hi - lo, &part);
+                top->parts.push_back(part);
+            });
+        } catch (...) {
+            srs_free(ctx, top);
+            throw;
         }
-        const uint64_t* host[2] = {g, g_lagrange};
-        void* dev[2] = {nullptr, nullptr};
-        int slot[2] = {WS_BASES, WS_MISC2};
-        for (int b = 0; b < 2; b++) {
-            if (!host[b]) continue;
-            dev[b] = ctx->get(slot[b], count * 64);
-            H2B_CUDA(cudaMemcpyAsync(dev[b], host[b] + 8 * begin, count * 64, cudaMemcpyHostToDevice, ctx->stream));
-        }
-        srs_build(ctx, dev[0], dev[1], k, begin, count, out);
+        top->c = top->parts[0]->c;
+        top->W = top->parts[0]->W;
+        *out = top;
     });
 }
 int h2b_srs_upload_dev(h2b_ctx* ctx, const void* d_g, const void* d_g_lagrange, uint32_t k, size_t begin, size_t count,
@@ -453,27 +507,11 @@ int h2b_srs_info(const h2b_srs* srs, int* window_bits, int* windows) {
 }
 void h2b_srs_destroy(h2b_ctx* ctx, h2b_srs* srs) {
     if (!srs) return;
-    if (!srs->parts.empty() && ctx && ctx->members.size() == srs->parts.size()) {
-        std::lock_guard<std::mutex> lock(ctx->mu);
-        for (size_t i = 0; i < srs->parts.size(); i++) {
-            cudaSetDevice(ctx->members[i]->device);
-            cudaDeviceSynchronize();
-            for (auto& t : srs->parts[i]->table)
-                if (t) cudaFree(t);
-            delete srs->parts[i];
-        }
-        cudaSetDevice(ctx->device);
-        delete srs;
-        return;
-    }
-    if (ctx) {
-        std::lock_guard<std::mutex> lock(ctx->mu);
-        cudaSetDevice(ctx->device);
-        cudaDeviceSynchronize();
-    }
-    for (auto& t : srs->table)
-        if (t) cudaFree(t);
-    delete srs;
+    // the parts of a device group's handle are reachable only through that group's context
+    if (!ctx || ctx->members.size() != srs->parts.size()) srs->parts.clear();
+    if (!ctx) return srs_free(nullptr, srs);
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    srs_free(ctx, srs);
 }
 
 // ------------------------------------------------------------------------------------------------ MSM
@@ -510,9 +548,6 @@ int h2b_msm_g1_batch_dev(h2b_ctx* ctx, const h2b_srs* srs, const int* basis, con
         msm_run_batch(ctx, tables.data(), n, srs->c, srs->W, d_scalars, m, d_out);
     });
 }
-// host columns -> m commitments on the host.  Uploads run on the copy stream into per-lane staging buffers; lane l's MSM
-// waits for its upload and releases the buffer as soon as the scatter pass has consumed it.  `reduce`: combine the
-// partial sums of all connected GPUs with the fused NVLink all-reduce kernel before the one device-to-host copy.
 // Enqueue only: the m partial commitments of this context's shard end up in its WS_OUT buffer (returned), lanes joined
 // onto the context's stream.  `row0`: first row of the shard inside the caller's columns.
 static void* msm_batch_enqueue(h2b_ctx* ctx, const h2b_srs* srs, const int* basis, const uint64_t* const* scalars, size_t m, size_t n,
@@ -575,6 +610,10 @@ static void* msm_batch_enqueue(h2b_ctx* ctx, const h2b_srs* srs, const int* basi
     }
     return d_out;
 }
+// the fused all-reduce kernel combines at most 16 points per launch
+static void allreduce_chunked(h2b_ctx* ctx, void* d_points, size_t m) {
+    for (size_t lo = 0; lo < m; lo += 16) peer_allreduce(ctx, (char*)d_points + 96 * lo, m - lo < 16 ? m - lo : 16);
+}
 // host columns -> m commitments on the host.  Uploads run on the copy stream into per-lane staging buffers; lane l's MSM
 // waits for its upload and releases the buffer as soon as the scatter pass has consumed it.  `reduce`: combine the
 // partial sums of all connected GPUs with the fused NVLink all-reduce kernel before the one device-to-host copy.
@@ -594,9 +633,7 @@ static void msm_batch_host(h2b_ctx* ctx, const h2b_srs* srs, const int* basis, c
             const h2b_srs* part = srs->parts[g];
             d_outs[g] = msm_batch_enqueue(mb, part, basis, scalars, m, part->count, part->begin - srs->begin);
         });
-        group_each(ctx, [&](h2b_ctx* mb, size_t g) {
-            for (size_t lo = 0; lo < m; lo += 16) peer_allreduce(mb, (char*)d_outs[g] + 96 * lo, m - lo < 16 ? m - lo : 16);
-        });
+        group_each(ctx, [&](h2b_ctx* mb, size_t g) { allreduce_chunked(mb, d_outs[g], m); });
         H2B_CUDA(cudaMemcpyAsync(h_out, d_outs[0], m * 96, cudaMemcpyDeviceToHost, ctx->stream));
         group_each(ctx, [&](h2b_ctx* mb, size_t) { H2B_CUDA(cudaStreamSynchronize(mb->stream)); });
         memcpy(out_xyz, h_out, m * 96);
@@ -604,8 +641,7 @@ static void msm_batch_host(h2b_ctx* ctx, const h2b_srs* srs, const int* basis, c
     }
     void* d_out = msm_batch_enqueue(ctx, srs, basis, scalars, m, n, 0);
     cudaStream_t ks = ctx->stream;
-    if (reduce && peer_connected(ctx))
-        for (size_t lo = 0; lo < m; lo += 16) peer_allreduce(ctx, (char*)d_out + 96 * lo, m - lo < 16 ? m - lo : 16);
+    if (reduce && peer_connected(ctx)) allreduce_chunked(ctx, d_out, m);
     H2B_CUDA(cudaMemcpyAsync(h_out, d_out, m * 96, cudaMemcpyDeviceToHost, ks));
     H2B_CUDA(cudaStreamSynchronize(ks));
     memcpy(out_xyz, h_out, m * 96);
@@ -627,15 +663,12 @@ int h2b_msm_g1(h2b_ctx* ctx, const h2b_srs* srs, int basis, const uint64_t* scal
 int h2b_msm_g1_bases(h2b_ctx* ctx, const uint64_t* bases, const uint64_t* scalars, size_t n, uint64_t out_xyz[12]) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(bases && scalars && out_xyz && n >= 1, "msm: null pointer or n == 0");
-        void* d_b = ctx->get(WS_BASES, n * 64);
-        void* d_s = ctx->get(WS_SCALARS, n * 32);
-        void* d_o = ctx->get(WS_OUT, 96);
-        H2B_CUDA(cudaMemcpyAsync(d_b, bases, n * 64, cudaMemcpyHostToDevice, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(d_s, scalars, n * 32, cudaMemcpyHostToDevice, ctx->stream));
+        Staging sb(ctx, WS_BASES, n * 64), ss(ctx, WS_SCALARS, n * 32), so(ctx, WS_OUT, 96);
+        void *d_b = sb.up(bases, n * 64), *d_s = ss.up(scalars, n * 32), *d_o = so.take(96);
         msm_run_adhoc(ctx, d_b, n, d_s, d_o);
         uint64_t* h_out = (uint64_t*)ctx->get_pinned(0, 96);
         H2B_CUDA(cudaMemcpyAsync(h_out, d_o, 96, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        so.finish();
         memcpy(out_xyz, h_out, 96);
     });
 }
@@ -648,13 +681,12 @@ int h2b_g1_sum_dev(h2b_ctx* ctx, const void* d_points_xyz, size_t m, void* d_out
 int h2b_g1_sum(h2b_ctx* ctx, const uint64_t* points_xyz, size_t m, uint64_t out_xyz[12]) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(points_xyz && out_xyz, "g1_sum: null pointer");
-        void* d_p = ctx->get(WS_MISC, m * 96 + 96);
-        void* d_o = (char*)d_p + m * 96;
-        H2B_CUDA(cudaMemcpyAsync(d_p, points_xyz, m * 96, cudaMemcpyHostToDevice, ctx->stream));
+        Staging st(ctx, WS_MISC, m * 96 + 96);
+        void *d_p = st.up(points_xyz, m * 96), *d_o = st.take(96);
         g1_sum_run(ctx, d_p, m, d_o);
         uint64_t* h_out = (uint64_t*)ctx->get_pinned(0, 96);
         H2B_CUDA(cudaMemcpyAsync(h_out, d_o, 96, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        st.finish();
         memcpy(out_xyz, h_out, 96);
     });
 }
@@ -662,11 +694,9 @@ int h2b_g1_normalize(h2b_ctx* ctx, uint64_t* points_xyz, size_t m) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(points_xyz, "g1_normalize: null pointer");
         if (m == 0) return;
-        void* d_p = ctx->get(WS_MISC, m * 96);
-        H2B_CUDA(cudaMemcpyAsync(d_p, points_xyz, m * 96, cudaMemcpyHostToDevice, ctx->stream));
-        g1_normalize_run(ctx, d_p, m);
-        H2B_CUDA(cudaMemcpyAsync(points_xyz, d_p, m * 96, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_MISC, m * 96);
+        g1_normalize_run(ctx, st.inout(points_xyz, m * 96), m);
+        st.finish();
     });
 }
 int h2b_g1_fixed_base_mul_dev(h2b_ctx* ctx, const uint64_t base_xy[8], const void* d_scalars, size_t n, void* d_out_xy) {
@@ -679,12 +709,10 @@ int h2b_g1_fixed_base_mul(h2b_ctx* ctx, const uint64_t base_xy[8], const uint64_
     return guarded(ctx, [&] {
         H2B_REQUIRE(base_xy && scalars && out_xy, "fixed_base_mul: null pointer");
         if (n == 0) return;
-        void* d_s = ctx->get(WS_SCALARS, n * 32);
-        void* d_o = ctx->get(WS_BASES, n * 64);
-        H2B_CUDA(cudaMemcpyAsync(d_s, scalars, n * 32, cudaMemcpyHostToDevice, ctx->stream));
+        Staging ss(ctx, WS_SCALARS, n * 32), so(ctx, WS_BASES, n * 64);
+        void *d_s = ss.up(scalars, n * 32), *d_o = so.out(out_xy, n * 64);
         g1_fixed_base_mul_run(ctx, base_xy, d_s, n, d_o);
-        H2B_CUDA(cudaMemcpyAsync(out_xy, d_o, n * 64, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        so.finish();
     });
 }
 
@@ -714,193 +742,147 @@ int h2b_domain_omega(uint32_t k, uint64_t omega_out[4]) {
     domain_omega(k, omega_out, false);
     return H2B_OK;
 }
-// mode: 0 plain (omega given), 1 lagrange_to_coeff, 2 coeff_to_lagrange, 3 extended_to_coeff
-static void ntt_inplace_dev(h2b_ctx* ctx, void* d_a, uint32_t log_n, const uint64_t* omega, int scale, int mode) {
+enum NttKind { NTT_PLAIN, NTT_LAGRANGE_TO_COEFF, NTT_COEFF_TO_LAGRANGE, NTT_EXTENDED_TO_COEFF, NTT_COEFF_TO_EXTENDED };
+// ntt_run's root, scaling and coset mode for each kind; NTT_PLAIN takes the caller's root and scaling
+struct NttArgs {
+    uint64_t w[4];
+    int scale, coset;
+    NttArgs(NttKind kind, uint32_t log_n, const uint64_t* omega = nullptr, int plain_scale = 0) {
+        if (kind == NTT_PLAIN) {
+            memcpy(w, omega, 32);
+            scale = plain_scale;
+            coset = 0;
+            return;
+        }
+        const bool inverse = kind == NTT_LAGRANGE_TO_COEFF || kind == NTT_EXTENDED_TO_COEFF;
+        domain_omega(log_n, w, inverse);
+        scale = inverse;
+        coset = kind == NTT_EXTENDED_TO_COEFF ? 2 : kind == NTT_COEFF_TO_EXTENDED ? 1 : 0;
+    }
+};
+static void ntt_inplace_dev(h2b_ctx* ctx, void* d_a, uint32_t log_n, NttKind kind, const uint64_t* omega = nullptr, int scale = 0) {
     H2B_REQUIRE(d_a, "ntt: null pointer");
     H2B_REQUIRE(log_n <= 28, "ntt: log_n exceeds the two-adicity of Fr (28)");
-    uint64_t w[4];
-    int coset = 0;
-    if (mode == 0) { H2B_REQUIRE(omega, "ntt: null omega"); memcpy(w, omega, 32); }
-    else if (mode == 2) domain_omega(log_n, w, false);
-    else { domain_omega(log_n, w, true); scale = 1; if (mode == 3) coset = 2; }
-    ntt_run(ctx, d_a, (size_t)1 << log_n, d_a, log_n, w, scale, coset);
+    if (kind == NTT_PLAIN) H2B_REQUIRE(omega, "ntt: null omega");
+    const NttArgs t(kind, log_n, omega, scale);
+    ntt_run(ctx, d_a, (size_t)1 << log_n, d_a, log_n, t.w, t.scale, t.coset);
 }
-static void ntt_inplace_host(h2b_ctx* ctx, uint64_t* a, uint32_t log_n, const uint64_t* omega, int scale, int mode) {
+static void ntt_inplace_host(h2b_ctx* ctx, uint64_t* a, uint32_t log_n, NttKind kind, const uint64_t* omega = nullptr, int scale = 0) {
     H2B_REQUIRE(a, "ntt: null pointer");
     H2B_REQUIRE(log_n <= 28, "ntt: log_n exceeds the two-adicity of Fr (28)");
-    size_t bytes = ((size_t)1 << log_n) * 32;
-    void* d = ctx->get(WS_NTT_A, bytes);
-    H2B_CUDA(cudaMemcpyAsync(d, a, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    ntt_inplace_dev(ctx, d, log_n, omega, scale, mode);
-    H2B_CUDA(cudaMemcpyAsync(a, d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+    const size_t bytes = ((size_t)1 << log_n) * 32;
+    Staging st(ctx, WS_NTT_A, bytes);
+    ntt_inplace_dev(ctx, st.inout(a, bytes), log_n, kind, omega, scale);
+    st.finish();
 }
 int h2b_ntt_fr(h2b_ctx* ctx, uint64_t* a, uint32_t log_n, const uint64_t omega[4], int scale_by_n_inv) {
-    return guarded(ctx, [&] { ntt_inplace_host(ctx, a, log_n, omega, scale_by_n_inv, 0); });
+    return guarded(ctx, [&] { ntt_inplace_host(ctx, a, log_n, NTT_PLAIN, omega, scale_by_n_inv); });
 }
 int h2b_ntt_fr_dev(h2b_ctx* ctx, void* d_a, uint32_t log_n, const uint64_t omega[4], int scale_by_n_inv) {
-    return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, log_n, omega, scale_by_n_inv, 0); });
+    return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, log_n, NTT_PLAIN, omega, scale_by_n_inv); });
 }
-int h2b_lagrange_to_coeff(h2b_ctx* ctx, uint64_t* a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_host(ctx, a, k, nullptr, 1, 1); }); }
-int h2b_coeff_to_lagrange(h2b_ctx* ctx, uint64_t* a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_host(ctx, a, k, nullptr, 0, 2); }); }
-int h2b_lagrange_to_coeff_dev(h2b_ctx* ctx, void* d_a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, k, nullptr, 1, 1); }); }
-int h2b_coeff_to_lagrange_dev(h2b_ctx* ctx, void* d_a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, k, nullptr, 0, 2); }); }
-int h2b_extended_to_coeff(h2b_ctx* ctx, uint64_t* a, uint32_t ext_k) { return guarded(ctx, [&] { ntt_inplace_host(ctx, a, ext_k, nullptr, 1, 3); }); }
-int h2b_extended_to_coeff_dev(h2b_ctx* ctx, void* d_a, uint32_t ext_k) { return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, ext_k, nullptr, 1, 3); }); }
+int h2b_lagrange_to_coeff(h2b_ctx* ctx, uint64_t* a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_host(ctx, a, k, NTT_LAGRANGE_TO_COEFF); }); }
+int h2b_coeff_to_lagrange(h2b_ctx* ctx, uint64_t* a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_host(ctx, a, k, NTT_COEFF_TO_LAGRANGE); }); }
+int h2b_lagrange_to_coeff_dev(h2b_ctx* ctx, void* d_a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, k, NTT_LAGRANGE_TO_COEFF); }); }
+int h2b_coeff_to_lagrange_dev(h2b_ctx* ctx, void* d_a, uint32_t k) { return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, k, NTT_COEFF_TO_LAGRANGE); }); }
+int h2b_extended_to_coeff(h2b_ctx* ctx, uint64_t* a, uint32_t ext_k) { return guarded(ctx, [&] { ntt_inplace_host(ctx, a, ext_k, NTT_EXTENDED_TO_COEFF); }); }
+int h2b_extended_to_coeff_dev(h2b_ctx* ctx, void* d_a, uint32_t ext_k) { return guarded(ctx, [&] { ntt_inplace_dev(ctx, d_a, ext_k, NTT_EXTENDED_TO_COEFF); }); }
 
+static void coeff_to_extended_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n_coeffs, uint32_t ext_k, void* d_out) {
+    const NttArgs t(NTT_COEFF_TO_EXTENDED, ext_k);
+    ntt_run(ctx, d_coeffs, n_coeffs, d_out, ext_k, t.w, t.scale, t.coset);
+}
 int h2b_coeff_to_extended_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n_coeffs, uint32_t ext_k, void* d_out) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(d_coeffs && d_out, "coeff_to_extended: null pointer");
         H2B_REQUIRE(ext_k <= 28 && n_coeffs <= ((size_t)1 << ext_k), "coeff_to_extended: sizes out of range");
-        uint64_t w[4];
-        domain_omega(ext_k, w, false);
-        ntt_run(ctx, d_coeffs, n_coeffs, d_out, ext_k, w, 0, 1);
+        coeff_to_extended_dev(ctx, d_coeffs, n_coeffs, ext_k, d_out);
     });
 }
 int h2b_coeff_to_extended(h2b_ctx* ctx, const uint64_t* coeffs, size_t n_coeffs, uint32_t ext_k, uint64_t* out) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(coeffs && out, "coeff_to_extended: null pointer");
         H2B_REQUIRE(ext_k <= 28 && n_coeffs <= ((size_t)1 << ext_k), "coeff_to_extended: sizes out of range");
-        size_t bytes = ((size_t)1 << ext_k) * 32;
-        void* d = ctx->get(WS_NTT_A, bytes);
-        H2B_CUDA(cudaMemcpyAsync(d, coeffs, n_coeffs * 32, cudaMemcpyHostToDevice, ctx->stream));
-        uint64_t w[4];
-        domain_omega(ext_k, w, false);
-        ntt_run(ctx, d, n_coeffs, d, ext_k, w, 0, 1);
+        const size_t bytes = ((size_t)1 << ext_k) * 32;
+        Staging st(ctx, WS_NTT_A, bytes);
+        void* d = st.up(coeffs, n_coeffs * 32, bytes);
+        coeff_to_extended_dev(ctx, d, n_coeffs, ext_k, d);
         H2B_CUDA(cudaMemcpyAsync(out, d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        st.finish();
     });
 }
 
-// m transforms of one kind through three rotating device buffers: the upload of column i+1 (copy stream) and the
-// download of column i-1 (second copy stream) overlap the kernels of column i (context stream).
-// mode: 1 lagrange_to_coeff, 2 coeff_to_lagrange, 3 extended_to_coeff (in place, n_in = 2^log_n), 4 coeff_to_extended.
-static void ntt_batch_finish(h2b_ctx* ctx) {
-    H2B_CUDA(cudaStreamSynchronize(ctx->copy_stream2));
-    H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+static void check_columns(const void* const* a, const void* const* b, size_t m) {
+    for (size_t i = 0; i < m; i++) H2B_REQUIRE(a[i] && b[i], "ntt batch: null column");
 }
-// finish = false: enqueue only (the device group enqueues on every device before it waits for any)
-static void ntt_batch_host(h2b_ctx* ctx, int mode, const uint64_t* const* in, uint64_t* const* out, size_t m, size_t n_in,
-                           uint32_t log_n, bool finish = true) {
+// m transforms of one kind, in[i] -> out[i]; n_coeffs: the input length of NTT_COEFF_TO_EXTENDED (the other kinds transform
+// 2^log_n elements in place)
+static void ntt_batch(h2b_ctx* ctx, NttKind kind, const uint64_t* const* in, uint64_t* const* out, size_t m, uint32_t log_n,
+                      size_t n_coeffs = 0) {
     H2B_REQUIRE(in && out, "ntt batch: null pointer");
-    H2B_REQUIRE(log_n <= 28 && n_in <= ((size_t)1 << log_n), "ntt batch: sizes out of range");
+    H2B_REQUIRE(log_n <= 28 && n_coeffs <= ((size_t)1 << log_n), "ntt batch: sizes out of range");
     if (m == 0) return;
-    const size_t n = (size_t)1 << log_n, bytes = n * 32;
-    const int slots[3] = {WS_NTT_A, WS_NTT_C, WS_NTT_D};
-    void* buf[3];
-    for (int b = 0; b < 3; b++) buf[b] = ctx->get(slots[b], bytes);
-    (void)ctx->get(WS_NTT_B, bytes);  // scratch of ntt_run: allocate before anything is in flight
-    uint64_t w[4];
-    int scale = 0, coset = 0;
-    if (mode == 2 || mode == 4) domain_omega(log_n, w, false);
-    else { domain_omega(log_n, w, true); scale = 1; }
-    if (mode == 3) coset = 2;
-    if (mode == 4) coset = 1;
-    cudaStream_t up = ctx->copy_stream, ks = ctx->stream, down = ctx->copy_stream2;
-    H2B_CUDA(cudaEventRecord(ctx->fork_ev, ks));
-    H2B_CUDA(cudaStreamWaitEvent(up, ctx->fork_ev, 0));
-    for (size_t i = 0; i < m; i++) {
-        const int b = (int)(i % 3);
-        H2B_REQUIRE(in[i] && out[i], "ntt batch: null column");
-        if (i >= 3) H2B_CUDA(cudaStreamWaitEvent(up, ctx->pipe_ev[b][2], 0));  // buffer b downloaded
-        H2B_CUDA(cudaMemcpyAsync(buf[b], in[i], n_in * 32, cudaMemcpyHostToDevice, up));
-        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][0], up));
-        H2B_CUDA(cudaStreamWaitEvent(ks, ctx->pipe_ev[b][0], 0));
-        ntt_run(ctx, buf[b], n_in, buf[b], log_n, w, scale, coset);
-        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][1], ks));
-        H2B_CUDA(cudaStreamWaitEvent(down, ctx->pipe_ev[b][1], 0));
-        H2B_CUDA(cudaMemcpyAsync(out[i], buf[b], bytes, cudaMemcpyDeviceToHost, down));
-        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][2], down));
-    }
-    if (finish) ntt_batch_finish(ctx);
+    check_columns((const void* const*)in, (const void* const*)out, m);
+    const size_t n = (size_t)1 << log_n, bytes = n * 32, n_in = kind == NTT_COEFF_TO_EXTENDED ? n_coeffs : n;
+    const NttArgs t(kind, log_n);
+    ntt_deal(ctx, in, out, m, [&](h2b_ctx* c, const uint64_t* const* vi, uint64_t* const* vo, size_t mc) {
+        if (mc == 0) return;
+        const int slots[3] = {WS_NTT_A, WS_NTT_C, WS_NTT_D};
+        void* buf[3];
+        for (int b = 0; b < 3; b++) buf[b] = c->get(slots[b], bytes);
+        (void)c->get(WS_NTT_B, bytes);  // scratch of ntt_run: allocate before anything is in flight
+        ntt_pipeline(c, vi, mc, buf, n_in * 32, [&](size_t, int b) { ntt_run(c, buf[b], n_in, buf[b], log_n, t.w, t.scale, t.coset); },
+                     [&](size_t i, int b, cudaStream_t down) {
+                         H2B_CUDA(cudaStreamWaitEvent(down, c->pipe_ev[b][1], 0));
+                         H2B_CUDA(cudaMemcpyAsync(vo[i], buf[b], bytes, cudaMemcpyDeviceToHost, down));
+                     });
+    });
 }
 // lagrange_to_coeff followed by coeff_to_extended for m columns, fused: the coefficients go up once, stay on the device
 // for the coset transform, and both results come down on the second copy stream while the next column computes.
-static void ntt_fused_batch_host(h2b_ctx* ctx, uint64_t* const* a, size_t m, uint32_t k, uint32_t ext_k, uint64_t* const* ext_out,
-                                 bool finish = true) {
+static void ntt_fused_batch(h2b_ctx* ctx, uint64_t* const* a, size_t m, uint32_t k, uint32_t ext_k, uint64_t* const* ext_out) {
     H2B_REQUIRE(a && ext_out, "ntt batch: null pointer");
     H2B_REQUIRE(k <= ext_k && ext_k <= 28, "ntt batch: sizes out of range");
     if (m == 0) return;
+    check_columns((const void* const*)a, (const void* const*)ext_out, m);
     const size_t n = (size_t)1 << k, ne = (size_t)1 << ext_k;
-    const int small_slots[3] = {WS_NTT_E, WS_NTT_F, WS_NTT_G}, big_slots[3] = {WS_NTT_A, WS_NTT_C, WS_NTT_D};
-    void *sm[3], *big[3];
-    for (int b = 0; b < 3; b++) {
-        sm[b] = ctx->get(small_slots[b], n * 32);
-        big[b] = ctx->get(big_slots[b], ne * 32);
-    }
-    (void)ctx->get(WS_NTT_B, ne * 32);  // scratch of ntt_run: allocate before anything is in flight
-    uint64_t w_inv[4], w_ext[4];
-    domain_omega(k, w_inv, true);
-    domain_omega(ext_k, w_ext, false);
-    cudaStream_t up = ctx->copy_stream, ks = ctx->stream, down = ctx->copy_stream2;
-    H2B_CUDA(cudaEventRecord(ctx->fork_ev, ks));
-    H2B_CUDA(cudaStreamWaitEvent(up, ctx->fork_ev, 0));
-    for (size_t i = 0; i < m; i++) {
-        const int b = (int)(i % 3);
-        H2B_REQUIRE(a[i] && ext_out[i], "ntt batch: null column");
-        if (i >= 3) H2B_CUDA(cudaStreamWaitEvent(up, ctx->pipe_ev[b][2], 0));  // buffers b downloaded
-        H2B_CUDA(cudaMemcpyAsync(sm[b], a[i], n * 32, cudaMemcpyHostToDevice, up));
-        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][0], up));
-        H2B_CUDA(cudaStreamWaitEvent(ks, ctx->pipe_ev[b][0], 0));
-        ntt_run(ctx, sm[b], n, sm[b], k, w_inv, 1, 0);
-        H2B_CUDA(cudaEventRecord(ctx->ev[b], ks));  // coefficients ready
-        ntt_run(ctx, sm[b], n, big[b], ext_k, w_ext, 0, 1);
-        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][1], ks));
-        H2B_CUDA(cudaStreamWaitEvent(down, ctx->ev[b], 0));
-        H2B_CUDA(cudaMemcpyAsync(a[i], sm[b], n * 32, cudaMemcpyDeviceToHost, down));
-        H2B_CUDA(cudaStreamWaitEvent(down, ctx->pipe_ev[b][1], 0));
-        H2B_CUDA(cudaMemcpyAsync(ext_out[i], big[b], ne * 32, cudaMemcpyDeviceToHost, down));
-        H2B_CUDA(cudaEventRecord(ctx->pipe_ev[b][2], down));
-    }
-    if (finish) ntt_batch_finish(ctx);
-}
-// ---- device group: polynomial j goes to device j mod G ("one column polynomial per device", SURVEY.md §8e); every device
-// runs its own upload / transform / download pipeline, all enqueued before the first wait
-static void group_ntt_batch(h2b_ctx* ctx, int mode, const uint64_t* const* in, uint64_t* const* out, size_t m, size_t n_in, uint32_t log_n) {
-    H2B_REQUIRE(in && out, "ntt batch: null pointer");
-    const size_t G = ctx->members.size();
-    group_each(ctx, [&](h2b_ctx* mb, size_t g) {
-        auto vi = every_gth(in, m, g, G);
-        auto vo = every_gth(out, m, g, G);
-        ntt_batch_host(mb, mode, vi.data(), vo.data(), vi.size(), n_in, log_n, false);
+    const NttArgs inv(NTT_LAGRANGE_TO_COEFF, k), ext(NTT_COEFF_TO_EXTENDED, ext_k);
+    ntt_deal(ctx, a, ext_out, m, [&](h2b_ctx* c, uint64_t* const* va, uint64_t* const* ve, size_t mc) {
+        if (mc == 0) return;
+        const int small_slots[3] = {WS_NTT_E, WS_NTT_F, WS_NTT_G}, big_slots[3] = {WS_NTT_A, WS_NTT_C, WS_NTT_D};
+        void *sm[3], *big[3];
+        for (int b = 0; b < 3; b++) {
+            sm[b] = c->get(small_slots[b], n * 32);
+            big[b] = c->get(big_slots[b], ne * 32);
+        }
+        (void)c->get(WS_NTT_B, ne * 32);  // scratch of ntt_run: allocate before anything is in flight
+        ntt_pipeline(c, va, mc, sm, n * 32,
+                     [&](size_t, int b) {
+                         ntt_run(c, sm[b], n, sm[b], k, inv.w, inv.scale, inv.coset);
+                         H2B_CUDA(cudaEventRecord(c->ev[b], c->stream));  // coefficients ready
+                         ntt_run(c, sm[b], n, big[b], ext_k, ext.w, ext.scale, ext.coset);
+                     },
+                     [&](size_t i, int b, cudaStream_t down) {
+                         H2B_CUDA(cudaStreamWaitEvent(down, c->ev[b], 0));
+                         H2B_CUDA(cudaMemcpyAsync(va[i], sm[b], n * 32, cudaMemcpyDeviceToHost, down));
+                         H2B_CUDA(cudaStreamWaitEvent(down, c->pipe_ev[b][1], 0));
+                         H2B_CUDA(cudaMemcpyAsync(ve[i], big[b], ne * 32, cudaMemcpyDeviceToHost, down));
+                     });
     });
-    group_each(ctx, [&](h2b_ctx* mb, size_t) { ntt_batch_finish(mb); });
-}
-static void group_ntt_fused_batch(h2b_ctx* ctx, uint64_t* const* a, size_t m, uint32_t k, uint32_t ext_k, uint64_t* const* ext_out) {
-    H2B_REQUIRE(a && ext_out, "ntt batch: null pointer");
-    const size_t G = ctx->members.size();
-    group_each(ctx, [&](h2b_ctx* mb, size_t g) {
-        auto va = every_gth(a, m, g, G);
-        auto ve = every_gth(ext_out, m, g, G);
-        ntt_fused_batch_host(mb, va.data(), va.size(), k, ext_k, ve.data(), false);
-    });
-    group_each(ctx, [&](h2b_ctx* mb, size_t) { ntt_batch_finish(mb); });
 }
 int h2b_lagrange_to_coeff_and_extended_batch(h2b_ctx* ctx, uint64_t* const* a, size_t m, uint32_t k, uint32_t ext_k,
                                              uint64_t* const* ext_out) {
-    return guarded(ctx, [&] {
-        if (ctx->members.size() > 1) group_ntt_fused_batch(ctx, a, m, k, ext_k, ext_out);
-        else ntt_fused_batch_host(ctx, a, m, k, ext_k, ext_out);
-    });
+    return guarded(ctx, [&] { ntt_fused_batch(ctx, a, m, k, ext_k, ext_out); });
 }
 int h2b_lagrange_to_coeff_batch(h2b_ctx* ctx, uint64_t* const* a, size_t m, uint32_t k) {
-    return guarded(ctx, [&] {
-        if (ctx->members.size() > 1) group_ntt_batch(ctx, 1, a, a, m, (size_t)1 << (k <= 28 ? k : 0), k);
-        else ntt_batch_host(ctx, 1, a, a, m, (size_t)1 << (k <= 28 ? k : 0), k);
-    });
+    return guarded(ctx, [&] { ntt_batch(ctx, NTT_LAGRANGE_TO_COEFF, a, a, m, k); });
 }
 int h2b_coeff_to_lagrange_batch(h2b_ctx* ctx, uint64_t* const* a, size_t m, uint32_t k) {
-    return guarded(ctx, [&] {
-        if (ctx->members.size() > 1) group_ntt_batch(ctx, 2, a, a, m, (size_t)1 << (k <= 28 ? k : 0), k);
-        else ntt_batch_host(ctx, 2, a, a, m, (size_t)1 << (k <= 28 ? k : 0), k);
-    });
+    return guarded(ctx, [&] { ntt_batch(ctx, NTT_COEFF_TO_LAGRANGE, a, a, m, k); });
 }
 int h2b_coeff_to_extended_batch(h2b_ctx* ctx, const uint64_t* const* coeffs, size_t m, size_t n_coeffs, uint32_t ext_k,
                                 uint64_t* const* out) {
-    return guarded(ctx, [&] {
-        if (ctx->members.size() > 1) group_ntt_batch(ctx, 4, coeffs, out, m, n_coeffs, ext_k);
-        else ntt_batch_host(ctx, 4, coeffs, out, m, n_coeffs, ext_k);
-    });
+    return guarded(ctx, [&] { ntt_batch(ctx, NTT_COEFF_TO_EXTENDED, coeffs, out, m, ext_k, n_coeffs); });
 }
 
 // ------------------------------------------------------------------------------------------------ assignment
@@ -916,13 +898,11 @@ int h2b_assign_columns(h2b_ctx* ctx, const uint64_t* vcol, size_t N, const uint6
     return guarded(ctx, [&] {
         H2B_REQUIRE((vcol || N == 0) && (cols || ncols == 0) && (break_points || nbp == 0), "assign: null pointer");
         H2B_REQUIRE(k <= 28, "assign: k out of range");
-        size_t out_bytes = (ncols << k) * 32;
-        void* d_in = ctx->get(WS_ASSIGN_IN, N * 32);
-        void* d_out = ctx->get(WS_ASSIGN_OUT, out_bytes);
-        if (N) H2B_CUDA(cudaMemcpyAsync(d_in, vcol, N * 32, cudaMemcpyHostToDevice, ctx->stream));
+        const size_t out_bytes = (ncols << k) * 32;
+        Staging si(ctx, WS_ASSIGN_IN, N * 32), so(ctx, WS_ASSIGN_OUT, out_bytes);
+        void *d_in = si.up(vcol, N * 32), *d_out = so.out(cols, out_bytes);
         assign_columns_run(ctx, d_in, N, break_points, nbp, k, ncols, d_out);
-        if (out_bytes) H2B_CUDA(cudaMemcpyAsync(cols, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        so.finish();
     });
 }
 // `Assigned<Fr>` records in, columns out: flatten (Zero / Trivial / Rational with one batched inversion) + the gather
@@ -942,11 +922,11 @@ int h2b_assign_columns_assigned(h2b_ctx* ctx, const uint64_t* cells, size_t N, c
         H2B_REQUIRE((cells || N == 0) && (cols || ncols == 0) && (break_points || nbp == 0), "assign: null pointer");
         H2B_REQUIRE(k <= 28, "assign: k out of range");
         const size_t out_bytes = (ncols << k) * 32;
-        char* d_in = (char*)ctx->get(WS_ASSIGN_IN, N * 72 + N * 32 + 128);
-        void* d_vals = d_in + ((N * 72 + 31) & ~(size_t)31);
-        uint32_t* d_stats = (uint32_t*)((char*)d_vals + N * 32 + 32);
-        void* d_out = ctx->get(WS_ASSIGN_OUT, out_bytes);
-        if (N) H2B_CUDA(cudaMemcpyAsync(d_in, cells, N * 72, cudaMemcpyHostToDevice, ctx->stream));
+        Staging si(ctx, WS_ASSIGN_IN, N * 72 + N * 32 + 128), so(ctx, WS_ASSIGN_OUT, out_bytes);
+        void* d_in = si.up(cells, N * 72);
+        void* d_vals = si.take(N * 32 + 32);
+        uint32_t* d_stats = (uint32_t*)si.take(8);
+        void* d_out = so.out(cols, out_bytes);
         assigned_flatten_run(ctx, d_in, N, d_vals, d_stats, 0);
         uint32_t st[2] = {0, 0};
         if (N) {
@@ -959,8 +939,7 @@ int h2b_assign_columns_assigned(h2b_ctx* ctx, const uint64_t* cells, size_t N, c
         H2B_REQUIRE(st[1] == 0, "assign: a cell record carries a tag other than 0 (Zero), 1 (Trivial), 2 (Rational)");
         if (st[0]) assigned_flatten_run(ctx, d_in, N, d_vals, d_stats, 1);  // Rational cells present: with the batched inversion
         assign_columns_run(ctx, d_vals, N, break_points, nbp, k, ncols, d_out);
-        if (out_bytes) H2B_CUDA(cudaMemcpyAsync(cols, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        so.finish();
     });
 }
 int h2b_assign_lookups_dev(h2b_ctx* ctx, const void* d_vals, size_t N, uint32_t k, size_t L, void* d_cols) {
@@ -973,13 +952,11 @@ int h2b_assign_lookups(h2b_ctx* ctx, const uint64_t* vals, size_t N, uint32_t k,
     return guarded(ctx, [&] {
         H2B_REQUIRE((vals || N == 0) && (cols || L == 0), "assign: null pointer");
         H2B_REQUIRE(k <= 28, "assign: k out of range");
-        size_t out_bytes = (L << k) * 32;
-        void* d_in = ctx->get(WS_ASSIGN_IN, N * 32);
-        void* d_out = ctx->get(WS_ASSIGN_OUT, out_bytes);
-        if (N) H2B_CUDA(cudaMemcpyAsync(d_in, vals, N * 32, cudaMemcpyHostToDevice, ctx->stream));
+        const size_t out_bytes = (L << k) * 32;
+        Staging si(ctx, WS_ASSIGN_IN, N * 32), so(ctx, WS_ASSIGN_OUT, out_bytes);
+        void *d_in = si.up(vals, N * 32), *d_out = so.out(cols, out_bytes);
         assign_lookups_run(ctx, d_in, N, k, L, d_out);
-        if (out_bytes) H2B_CUDA(cudaMemcpyAsync(cols, d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        so.finish();
     });
 }
 int h2b_eval_rational_dev(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out) {
@@ -1005,12 +982,10 @@ int h2b_eval_rational(h2b_ctx* ctx, const uint64_t* num, const uint64_t* den, si
     return guarded(ctx, [&] {
         H2B_REQUIRE((num && den && out) || n == 0, "eval_rational: null pointer");
         if (n == 0) return;
-        char* d = (char*)ctx->get(WS_ASSIGN_IN, 3 * n * 32);
-        H2B_CUDA(cudaMemcpyAsync(d, num, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(d + n * 32, den, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        eval_rational_batched_run(ctx, d, d + n * 32, n, d + 2 * n * 32);
-        H2B_CUDA(cudaMemcpyAsync(out, d + 2 * n * 32, n * 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_ASSIGN_IN, 3 * n * 32);
+        void *d_num = st.up(num, n * 32), *d_den = st.up(den, n * 32), *d_out = st.out(out, n * 32);
+        eval_rational_batched_run(ctx, d_num, d_den, n, d_out);
+        st.finish();
     });
 }
 
@@ -1025,11 +1000,9 @@ int h2b_batch_invert_fr(h2b_ctx* ctx, uint64_t* a, size_t n) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(a || n == 0, "batch_invert: null pointer");
         if (n == 0) return;
-        void* d = ctx->get(WS_ASSIGN_IN, n * 32);
-        H2B_CUDA(cudaMemcpyAsync(d, a, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        batch_invert_run(ctx, d, n);
-        H2B_CUDA(cudaMemcpyAsync(a, d, n * 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_ASSIGN_IN, n * 32);
+        batch_invert_run(ctx, st.inout(a, n * 32), n);
+        st.finish();
     });
 }
 int h2b_grand_product_fr_dev(h2b_ctx* ctx, const void* d_f, const uint64_t start[4], size_t n, void* d_z) {
@@ -1042,11 +1015,10 @@ int h2b_grand_product_fr(h2b_ctx* ctx, const uint64_t* f, const uint64_t start[4
     return guarded(ctx, [&] {
         H2B_REQUIRE(((f && z) || n == 0) && start, "grand_product: null pointer");
         if (n == 0) return;
-        char* d = (char*)ctx->get(WS_ASSIGN_IN, 2 * n * 32);
-        H2B_CUDA(cudaMemcpyAsync(d, f, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        grand_product_run(ctx, d, start, n, d + n * 32);
-        H2B_CUDA(cudaMemcpyAsync(z, d + n * 32, n * 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_ASSIGN_IN, 2 * n * 32);
+        void *d_f = st.up(f, n * 32), *d_z = st.out(z, n * 32);
+        grand_product_run(ctx, d_f, start, n, d_z);
+        st.finish();
     });
 }
 
@@ -1061,15 +1033,12 @@ int h2b_flex_gate_fold(h2b_ctx* ctx, const uint64_t* q_ext, const uint64_t* a_ex
                        uint64_t* acc) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(q_ext && a_ext && y && acc, "flex_gate: null pointer");
-        H2B_REQUIRE(ext_k >= k && ext_k <= 28, "flex_gate: extended_k out of range");
+        H2B_REQUIRE(ext_k <= 28, "flex_gate: extended_k out of range");
         const size_t bytes = ((size_t)1 << ext_k) * 32;
-        char* d = (char*)ctx->get(WS_NTT_A, 3 * bytes);
-        H2B_CUDA(cudaMemcpyAsync(d, q_ext, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(d + bytes, a_ext, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(d + 2 * bytes, acc, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        flex_gate_fold_run(ctx, d, d + bytes, y, k, ext_k, d + 2 * bytes);
-        H2B_CUDA(cudaMemcpyAsync(acc, d + 2 * bytes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_NTT_A, 3 * bytes);
+        void *d_q = st.up(q_ext, bytes), *d_a = st.up(a_ext, bytes), *d_acc = st.inout(acc, bytes);
+        flex_gate_fold_run(ctx, d_q, d_a, y, k, ext_k, d_acc);
+        st.finish();
     });
 }
 
@@ -1085,11 +1054,10 @@ int h2b_g_to_lagrange(h2b_ctx* ctx, const uint64_t* g, uint32_t k, uint64_t* g_l
         H2B_REQUIRE(g && g_lagrange, "g_to_lagrange: null pointer");
         H2B_REQUIRE(k <= 28, "g_to_lagrange: k out of range");
         const size_t bytes = ((size_t)1 << k) * 64;
-        char* d = (char*)ctx->get(WS_BASES, 2 * bytes);
-        H2B_CUDA(cudaMemcpyAsync(d, g, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        g_to_lagrange_run(ctx, d, k, d + bytes);
-        H2B_CUDA(cudaMemcpyAsync(g_lagrange, d + bytes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_BASES, 2 * bytes);
+        void *d_g = st.up(g, bytes), *d_gl = st.out(g_lagrange, bytes);
+        g_to_lagrange_run(ctx, d_g, k, d_gl);
+        st.finish();
     });
 }
 int h2b_srs_setup_dev(h2b_ctx* ctx, const uint64_t tau[4], const uint64_t base_xy[8], uint32_t k, void* d_g, void* d_g_lagrange) {
@@ -1103,11 +1071,10 @@ int h2b_srs_setup(h2b_ctx* ctx, const uint64_t tau[4], const uint64_t base_xy[8]
         H2B_REQUIRE(tau && base_xy, "srs_setup: null pointer");
         H2B_REQUIRE(k <= 28, "srs_setup: k out of range");
         const size_t bytes = ((size_t)1 << k) * 64;
-        char* d = (char*)ctx->get(WS_BASES, 2 * bytes);
-        srs_setup_run(ctx, tau, base_xy, k, g ? d : nullptr, g_lagrange ? d + bytes : nullptr);
-        if (g) H2B_CUDA(cudaMemcpyAsync(g, d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        if (g_lagrange) H2B_CUDA(cudaMemcpyAsync(g_lagrange, d + bytes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_BASES, 2 * bytes);
+        void *d_g = st.out(g, bytes), *d_gl = st.out(g_lagrange, bytes);
+        srs_setup_run(ctx, tau, base_xy, k, g ? d_g : nullptr, g_lagrange ? d_gl : nullptr);
+        st.finish();
     });
 }
 int h2b_g1_check_on_curve_dev(h2b_ctx* ctx, const void* d_points_xy, size_t n, size_t* off_curve) {
@@ -1119,9 +1086,8 @@ int h2b_g1_check_on_curve_dev(h2b_ctx* ctx, const void* d_points_xy, size_t n, s
 int h2b_g1_check_on_curve(h2b_ctx* ctx, const uint64_t* points_xy, size_t n, size_t* off_curve) {
     return guarded(ctx, [&] {
         H2B_REQUIRE((points_xy || n == 0) && off_curve, "check_on_curve: null pointer");
-        void* d = ctx->get(WS_BASES, n * 64);
-        if (n) H2B_CUDA(cudaMemcpyAsync(d, points_xy, n * 64, cudaMemcpyHostToDevice, ctx->stream));
-        *off_curve = g1_count_off_curve_run(ctx, d, n);
+        void* d = Staging(ctx, WS_BASES, n * 64).up(points_xy, n * 64);
+        *off_curve = g1_count_off_curve_run(ctx, d, n);  // returns the count: synchronised
     });
 }
 int h2b_g1_decompress_dev(h2b_ctx* ctx, const void* d_bytes, size_t n, void* d_out_xy, size_t* invalid) {
@@ -1135,26 +1101,30 @@ int h2b_g1_decompress(h2b_ctx* ctx, const uint8_t* bytes, size_t n, uint64_t* ou
         H2B_REQUIRE(((bytes && out_xy) || n == 0) && invalid, "g1_decompress: null pointer");
         *invalid = 0;
         if (n == 0) return;
-        char* d = (char*)ctx->get(WS_BASES, n * 96);
-        H2B_CUDA(cudaMemcpyAsync(d, bytes, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        *invalid = g1_decompress_run(ctx, d, n, d + n * 32);
-        H2B_CUDA(cudaMemcpyAsync(out_xy, d + n * 32, n * 64, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_BASES, n * 96);
+        void *d_in = st.up(bytes, n * 32), *d_out = st.out(out_xy, n * 64);
+        *invalid = g1_decompress_run(ctx, d_in, n, d_out);
+        st.finish();
     });
 }
-int h2b_params_processed_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset,
-                              size_t* g2_offset, size_t* s_g2_offset) {
+// a params image: k (u32 little-endian), g and g_lagrange (2^k G1 points each), g2 and s_g2, with points of `g1` / `g2` bytes
+static int params_view(const uint8_t* bytes, size_t len, size_t g1, size_t g2, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset,
+                       size_t* g2_offset, size_t* s_g2_offset) {
     if (!bytes || !k || len < 4) return H2B_ERR_ARG;
     const uint32_t kk = (uint32_t)bytes[0] | ((uint32_t)bytes[1] << 8) | ((uint32_t)bytes[2] << 16) | ((uint32_t)bytes[3] << 24);
     if (kk > 28) return H2B_ERR_ARG;
     const size_t n = (size_t)1 << kk;
-    if (len < 4 + 2 * n * 32 + 2 * 64) return H2B_ERR_ARG;
+    if (len < 4 + 2 * n * g1 + 2 * g2) return H2B_ERR_ARG;
     *k = kk;
     if (g_offset) *g_offset = 4;
-    if (g_lagrange_offset) *g_lagrange_offset = 4 + n * 32;
-    if (g2_offset) *g2_offset = 4 + 2 * n * 32;
-    if (s_g2_offset) *s_g2_offset = 4 + 2 * n * 32 + 64;
+    if (g_lagrange_offset) *g_lagrange_offset = 4 + n * g1;
+    if (g2_offset) *g2_offset = 4 + 2 * n * g1;
+    if (s_g2_offset) *s_g2_offset = 4 + 2 * n * g1 + g2;
     return H2B_OK;
+}
+int h2b_params_processed_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset,
+                              size_t* g2_offset, size_t* s_g2_offset) {
+    return params_view(bytes, len, 32, 64, k, g_offset, g_lagrange_offset, g2_offset, s_g2_offset);
 }
 // `ParamsKZG::read` of a SerdeFormat::Processed image, device side: decompress g and g_lagrange (every point is thereby
 // on the curve), build the MSM tables.  H2B_ERR_ARG on a malformed image or an invalid point encoding.
@@ -1167,29 +1137,17 @@ int h2b_srs_read_processed(h2b_ctx* ctx, const uint8_t* bytes, size_t len, size_
         const size_t n = (size_t)1 << k;
         if (count == 0 && begin == 0) count = n;
         H2B_REQUIRE(count >= 1 && begin + count <= n, "srs_read: shard outside the 2^k bases");
-        char* d = (char*)ctx->get(WS_BASES, count * (64 + 128));
-        char* d_g = d + count * 64;
-        char* d_gl = d_g + count * 64;
-        H2B_CUDA(cudaMemcpyAsync(d, bytes + og + 32 * begin, count * 32, cudaMemcpyHostToDevice, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(d + count * 32, bytes + ol + 32 * begin, count * 32, cudaMemcpyHostToDevice, ctx->stream));
-        const size_t bad = g1_decompress_run(ctx, d, count, d_g) + g1_decompress_run(ctx, d + count * 32, count, d_gl);
+        Staging st(ctx, WS_BASES, count * (64 + 128));
+        void *c_g = st.up(bytes + og + 32 * begin, count * 32), *c_gl = st.up(bytes + ol + 32 * begin, count * 32);
+        void *d_g = st.take(count * 64), *d_gl = st.take(count * 64);
+        const size_t bad = g1_decompress_run(ctx, c_g, count, d_g) + g1_decompress_run(ctx, c_gl, count, d_gl);
         H2B_REQUIRE(bad == 0, "srs_read: the params image holds an invalid G1 encoding");
         srs_build(ctx, d_g, d_gl, k, begin, count, out);
     });
 }
 int h2b_params_raw_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset, size_t* g2_offset,
                         size_t* s_g2_offset) {
-    if (!bytes || !k || len < 4) return H2B_ERR_ARG;
-    const uint32_t kk = (uint32_t)bytes[0] | ((uint32_t)bytes[1] << 8) | ((uint32_t)bytes[2] << 16) | ((uint32_t)bytes[3] << 24);
-    if (kk > 28) return H2B_ERR_ARG;
-    const size_t n = (size_t)1 << kk;
-    if (len < 4 + 2 * n * 64 + 2 * 128) return H2B_ERR_ARG;
-    *k = kk;
-    if (g_offset) *g_offset = 4;
-    if (g_lagrange_offset) *g_lagrange_offset = 4 + n * 64;
-    if (g2_offset) *g2_offset = 4 + 2 * n * 64;
-    if (s_g2_offset) *s_g2_offset = 4 + 2 * n * 64 + 128;
-    return H2B_OK;
+    return params_view(bytes, len, 64, 128, k, g_offset, g_lagrange_offset, g2_offset, s_g2_offset);
 }
 
 // ------------------------------------------------------------------------------------------------ lookup permutation
@@ -1219,43 +1177,30 @@ int h2b_permute_expression_pair(h2b_ctx* ctx, const uint64_t* input, const uint6
         H2B_REQUIRE(input && table && permuted_input && permuted_table, "permute_expression_pair: null pointer");
         H2B_REQUIRE(k <= 28 && (size_t)blinding_factors + 1 < ((size_t)1 << k), "permute_expression_pair: no usable rows");
         const size_t u = ((size_t)1 << k) - (blinding_factors + 1), bytes = u * 32;
-        char* d = (char*)ctx->get(WS_ASSIGN_IN, 4 * bytes);
-        H2B_CUDA(cudaMemcpyAsync(d, input, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(d + bytes, table, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        const bool missing = permute_expression_pair_run(ctx, d, d + bytes, k, blinding_factors, d + 2 * bytes, d + 3 * bytes);
-        if (missing) throw StatusError{H2B_ERR_UNSATISFIED, "permute_expression_pair: an input value is not in the table (ConstraintSystemFailure)"};
-        H2B_CUDA(cudaMemcpyAsync(permuted_input, d + 2 * bytes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaMemcpyAsync(permuted_table, d + 3 * bytes, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_ASSIGN_IN, 4 * bytes);
+        void *d_in = st.up(input, bytes), *d_tab = st.up(table, bytes), *d_pin = st.out(permuted_input, bytes),
+             *d_ptab = st.out(permuted_table, bytes);
+        if (permute_expression_pair_run(ctx, d_in, d_tab, k, blinding_factors, d_pin, d_ptab))
+            throw StatusError{H2B_ERR_UNSATISFIED, "permute_expression_pair: an input value is not in the table (ConstraintSystemFailure)"};
+        st.finish();
     });
 }
 
 // ------------------------------------------------------------------------------------------------ quotient (general)
 namespace {
-// stages host columns of `bytes` bytes each, back to back, in one workspace slot
-struct ColumnStager {
-    h2b_ctx* ctx;
-    char* base;
-    size_t bytes, used = 0, cap;
-    ColumnStager(h2b_ctx* c, int slot, size_t count, size_t col_bytes) : ctx(c), bytes(col_bytes), cap(count) {
-        base = (char*)c->get(slot, count * col_bytes);
-    }
-    void* put(const void* host) {
-        H2B_REQUIRE(host, "quotient: null column");
-        H2B_REQUIRE(used < cap, "quotient: staging overflow");
-        char* d = base + (used++) * bytes;
-        H2B_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        return d;
-    }
-};
+// a host column of the quotient entry points uploaded into its staging
+void* put_column(Staging& st, const void* host, size_t bytes) {
+    H2B_REQUIRE(host, "quotient: null column");
+    return st.up(host, bytes);
+}
 struct StagedGraph {
     h2b_graph g;
     std::vector<const void*> fixed, advice, instance;
-    StagedGraph(const h2b_graph* src, ColumnStager& st) : g(*src) {
+    StagedGraph(const h2b_graph* src, Staging& st, size_t bytes) : g(*src) {
         H2B_REQUIRE((src->fixed || !src->n_fixed) && (src->advice || !src->n_advice) && (src->instance || !src->n_instance), "graph: null table");
-        for (size_t i = 0; i < src->n_fixed; i++) fixed.push_back(st.put(src->fixed[i]));
-        for (size_t i = 0; i < src->n_advice; i++) advice.push_back(st.put(src->advice[i]));
-        for (size_t i = 0; i < src->n_instance; i++) instance.push_back(st.put(src->instance[i]));
+        for (size_t i = 0; i < src->n_fixed; i++) fixed.push_back(put_column(st, src->fixed[i], bytes));
+        for (size_t i = 0; i < src->n_advice; i++) advice.push_back(put_column(st, src->advice[i], bytes));
+        for (size_t i = 0; i < src->n_instance; i++) instance.push_back(put_column(st, src->instance[i], bytes));
         g.fixed = fixed.data();
         g.advice = advice.data();
         g.instance = instance.data();
@@ -1276,14 +1221,12 @@ int h2b_quotient_graph_dev(h2b_ctx* ctx, const h2b_graph* graph, uint32_t k, uin
 int h2b_quotient_graph(h2b_ctx* ctx, const h2b_graph* graph, uint32_t k, uint32_t ext_k, uint64_t* values) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(graph && values, "quotient_graph: null pointer");
-        H2B_REQUIRE(ext_k >= k && ext_k <= 28, "quotient: extended_k out of range");
+        H2B_REQUIRE(ext_k <= 28, "quotient: extended_k out of range");
         const size_t bytes = ((size_t)1 << ext_k) * 32;
-        ColumnStager st(ctx, WS_NTT_A, graph_columns(graph) + 1, bytes);
-        StagedGraph sg(graph, st);
-        void* d_values = st.put(values);
-        quotient_graph_run(ctx, &sg.g, k, ext_k, d_values);
-        H2B_CUDA(cudaMemcpyAsync(values, d_values, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_NTT_A, (graph_columns(graph) + 1) * bytes);
+        StagedGraph sg(graph, st, bytes);
+        quotient_graph_run(ctx, &sg.g, k, ext_k, st.inout(values, bytes));
+        st.finish();
     });
 }
 int h2b_lookup_fold_dev(h2b_ctx* ctx, const h2b_graph* graph, const void* d_z, const void* d_permuted_input,
@@ -1299,15 +1242,15 @@ int h2b_lookup_fold(h2b_ctx* ctx, const h2b_graph* graph, const uint64_t* z, con
                     uint32_t ext_k, uint64_t* values) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(graph && values, "lookup_fold: null pointer");
-        H2B_REQUIRE(ext_k >= k && ext_k <= 28, "quotient: extended_k out of range");
+        H2B_REQUIRE(ext_k <= 28, "quotient: extended_k out of range");
         const size_t bytes = ((size_t)1 << ext_k) * 32;
-        ColumnStager st(ctx, WS_NTT_A, graph_columns(graph) + 7, bytes);
-        StagedGraph sg(graph, st);
-        void *dz = st.put(z), *dpi = st.put(permuted_input), *dpt = st.put(permuted_table), *d0 = st.put(l0), *dl = st.put(l_last),
-             *da = st.put(l_active), *dv = st.put(values);
-        lookup_fold_run(ctx, &sg.g, dz, dpi, dpt, d0, dl, da, k, ext_k, dv);
-        H2B_CUDA(cudaMemcpyAsync(values, dv, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_NTT_A, (graph_columns(graph) + 7) * bytes);
+        StagedGraph sg(graph, st, bytes);
+        void* d[6];
+        const void* host[6] = {z, permuted_input, permuted_table, l0, l_last, l_active};
+        for (int i = 0; i < 6; i++) d[i] = put_column(st, host[i], bytes);
+        lookup_fold_run(ctx, &sg.g, d[0], d[1], d[2], d[3], d[4], d[5], k, ext_k, st.inout(values, bytes));
+        st.finish();
     });
 }
 int h2b_permutation_fold_dev(h2b_ctx* ctx, const void* const* d_z, size_t n_sets, const void* const* d_columns, const void* const* d_sigma,
@@ -1328,18 +1271,18 @@ int h2b_permutation_fold(h2b_ctx* ctx, const uint64_t* const* z, size_t n_sets, 
     return guarded(ctx, [&] {
         if (n_sets == 0) return;
         H2B_REQUIRE(z && columns && sigma && values && beta && gamma && y, "permutation_fold: null pointer");
-        H2B_REQUIRE(ext_k >= k && ext_k <= 28, "quotient: extended_k out of range");
+        H2B_REQUIRE(ext_k <= 28, "quotient: extended_k out of range");
         const size_t bytes = ((size_t)1 << ext_k) * 32;
-        ColumnStager st(ctx, WS_NTT_A, n_sets + 2 * n_cols + 4, bytes);
+        Staging st(ctx, WS_NTT_A, (n_sets + 2 * n_cols + 4) * bytes);
         std::vector<const void*> dz, dc, ds;
-        for (size_t i = 0; i < n_sets; i++) dz.push_back(st.put(z[i]));
-        for (size_t i = 0; i < n_cols; i++) dc.push_back(st.put(columns[i]));
-        for (size_t i = 0; i < n_cols; i++) ds.push_back(st.put(sigma[i]));
-        void *d0 = st.put(l0), *dl = st.put(l_last), *da = st.put(l_active), *dv = st.put(values);
+        for (size_t i = 0; i < n_sets; i++) dz.push_back(put_column(st, z[i], bytes));
+        for (size_t i = 0; i < n_cols; i++) dc.push_back(put_column(st, columns[i], bytes));
+        for (size_t i = 0; i < n_cols; i++) ds.push_back(put_column(st, sigma[i], bytes));
+        void *d0 = put_column(st, l0, bytes), *dl = put_column(st, l_last, bytes), *da = put_column(st, l_active, bytes),
+             *dv = st.inout(values, bytes);
         permutation_fold_run(ctx, dz.data(), n_sets, dc.data(), ds.data(), n_cols, chunk_len, d0, dl, da, beta, gamma, y, blinding_factors,
                              k, ext_k, dv);
-        H2B_CUDA(cudaMemcpyAsync(values, dv, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        st.finish();
     });
 }
 
@@ -1352,13 +1295,11 @@ int h2b_divide_by_vanishing_poly_dev(h2b_ctx* ctx, void* d_values, uint32_t k, u
 int h2b_divide_by_vanishing_poly(h2b_ctx* ctx, uint64_t* values, uint32_t k, uint32_t ext_k) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(values, "divide_by_vanishing_poly: null pointer");
-        H2B_REQUIRE(ext_k > k && ext_k <= 28, "quotient: extended_k out of range");
+        H2B_REQUIRE(ext_k <= 28, "quotient: extended_k out of range");
         const size_t bytes = ((size_t)1 << ext_k) * 32;
-        void* d = ctx->get(WS_NTT_A, bytes);
-        H2B_CUDA(cudaMemcpyAsync(d, values, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        divide_by_vanishing_run(ctx, d, k, ext_k);
-        H2B_CUDA(cudaMemcpyAsync(values, d, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_NTT_A, bytes);
+        divide_by_vanishing_run(ctx, st.inout(values, bytes), k, ext_k);
+        st.finish();
     });
 }
 
@@ -1453,28 +1394,25 @@ int h2b_keygen_sigma_values_dev(h2b_ctx* ctx, const void* d_map, size_t n_cols, 
 }
 
 // ------------------------------------------------------------------------------------------------ opening arithmetic
+// the value lands in WS_OUT and comes back to the host through pinned memory in both forms
+static void eval_polynomial_to_host(h2b_ctx* ctx, const void* d_coeffs, size_t n, const uint64_t x[4], uint64_t out[4]) {
+    void* d_out = ctx->get(WS_OUT, 32);
+    eval_polynomial_run(ctx, d_coeffs, n, x, d_out);
+    uint64_t* bounce = (uint64_t*)ctx->get_pinned(0, 4096);
+    H2B_CUDA(cudaMemcpyAsync(bounce, d_out, 32, cudaMemcpyDeviceToHost, ctx->stream));
+    H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+    memcpy(out, bounce, 32);
+}
 int h2b_eval_polynomial_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n, const uint64_t x[4], uint64_t out[4]) {
     return guarded(ctx, [&] {
         H2B_REQUIRE((d_coeffs || n == 0) && x && out, "eval_polynomial: null pointer");
-        void* d_out = ctx->get(WS_OUT, 32);
-        eval_polynomial_run(ctx, d_coeffs, n, x, d_out);
-        uint64_t* bounce = (uint64_t*)ctx->get_pinned(0, 4096);
-        H2B_CUDA(cudaMemcpyAsync(bounce, d_out, 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
-        memcpy(out, bounce, 32);
+        eval_polynomial_to_host(ctx, d_coeffs, n, x, out);
     });
 }
 int h2b_eval_polynomial(h2b_ctx* ctx, const uint64_t* coeffs, size_t n, const uint64_t x[4], uint64_t out[4]) {
     return guarded(ctx, [&] {
         H2B_REQUIRE((coeffs || n == 0) && x && out, "eval_polynomial: null pointer");
-        void* d = ctx->get(WS_ASSIGN_IN, n * 32);
-        if (n) H2B_CUDA(cudaMemcpyAsync(d, coeffs, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        void* d_out = ctx->get(WS_OUT, 32);
-        eval_polynomial_run(ctx, d, n, x, d_out);
-        uint64_t* bounce = (uint64_t*)ctx->get_pinned(0, 4096);
-        H2B_CUDA(cudaMemcpyAsync(bounce, d_out, 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
-        memcpy(out, bounce, 32);
+        eval_polynomial_to_host(ctx, Staging(ctx, WS_ASSIGN_IN, n * 32).up(coeffs, n * 32), n, x, out);
     });
 }
 int h2b_kate_division_dev(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t z[4], void* d_q) {
@@ -1487,13 +1425,12 @@ int h2b_kate_division_dev(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_
 int h2b_kate_division(h2b_ctx* ctx, const uint64_t* a, size_t n, const uint64_t z[4], uint64_t* q) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(a && z && (q || n <= 1), "kate_division: null pointer");
-        H2B_REQUIRE(n >= 1, "kate_division: empty polynomial");
+        H2B_REQUIRE(n >= 1, "kate_division: empty polynomial");  // before (n - 1) sizes the output
         if (n == 1) return;
-        char* d = (char*)ctx->get(WS_ASSIGN_IN, 2 * n * 32);
-        H2B_CUDA(cudaMemcpyAsync(d, a, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        kate_division_run(ctx, d, n, z, d + n * 32);
-        H2B_CUDA(cudaMemcpyAsync(q, d + n * 32, (n - 1) * 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_ASSIGN_IN, 2 * n * 32);
+        void *d_a = st.up(a, n * 32), *d_q = st.out(q, (n - 1) * 32, n * 32);
+        kate_division_run(ctx, d_a, n, z, d_q);
+        st.finish();
     });
 }
 int h2b_poly_lincomb_dev(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* scalars, size_t m, size_t n, void* d_out) {
@@ -1507,13 +1444,11 @@ int h2b_poly_lincomb(h2b_ctx* ctx, const uint64_t* const* polys, const uint64_t*
         H2B_REQUIRE(polys && scalars && (out || n == 0), "poly_lincomb: null pointer");
         H2B_REQUIRE(m >= 1 && m <= 32, "poly_lincomb: 1..32 polynomials per call");
         if (n == 0) return;
-        ColumnStager st(ctx, WS_NTT_A, m + 1, n * 32);
+        Staging st(ctx, WS_NTT_A, (m + 1) * n * 32);
         std::vector<const void*> dp;
-        for (size_t j = 0; j < m; j++) dp.push_back(st.put(polys[j]));
-        char* d_out = st.base + m * st.bytes;
-        poly_lincomb_run(ctx, dp.data(), scalars, m, n, d_out);
-        H2B_CUDA(cudaMemcpyAsync(out, d_out, n * 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        for (size_t j = 0; j < m; j++) dp.push_back(put_column(st, polys[j], n * 32));
+        poly_lincomb_run(ctx, dp.data(), scalars, m, n, st.out(out, n * 32));
+        st.finish();
     });
 }
 
@@ -1522,12 +1457,10 @@ int h2b_test_field_op(h2b_ctx* ctx, int field, int op, const uint64_t* a, const 
     return guarded(ctx, [&] {
         H2B_REQUIRE(a && out && (b || (op > 2 && op < 7) || op == 9) && (field == 0 || field == 1) && op >= 0 && op <= 9, "field_op: bad argument");
         if (n == 0) return;
-        char* d = (char*)ctx->get(WS_ASSIGN_IN, 3 * n * 32);
-        H2B_CUDA(cudaMemcpyAsync(d, a, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        if (b) H2B_CUDA(cudaMemcpyAsync(d + n * 32, b, n * 32, cudaMemcpyHostToDevice, ctx->stream));
-        field_op_run(ctx, field, op, d, d + n * 32, n, d + 2 * n * 32);
-        H2B_CUDA(cudaMemcpyAsync(out, d + 2 * n * 32, n * 32, cudaMemcpyDeviceToHost, ctx->stream));
-        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+        Staging st(ctx, WS_ASSIGN_IN, 3 * n * 32);
+        void *d_a = st.up(a, n * 32), *d_b = st.up(b, b ? n * 32 : 0, n * 32), *d_out = st.out(out, n * 32);
+        field_op_run(ctx, field, op, d_a, d_b, n, d_out);
+        st.finish();
     });
 }
 

@@ -9,6 +9,8 @@
 #include <vector>
 #include <array>
 #include <algorithm>
+#include <new>
+#include <stdexcept>
 
 #include "../../include/h2b200.h"
 
@@ -164,6 +166,31 @@ namespace h2b {
         }                                                                        \
     } while (0)
 
+// Runs the body of a C entry point under the context lock with the context's device current; maps every failure to a
+// status code and h2b_last_error()'s message.  No exception leaves an entry point.
+template <class Fn>
+static int guarded(h2b_ctx* ctx, Fn&& body) {
+    if (!ctx) return H2B_ERR_ARG;
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    try {
+        H2B_CUDA(cudaSetDevice(ctx->device));
+        body();
+        return H2B_OK;
+    } catch (const StatusError& e) {
+        ctx->err = e.msg;
+        return e.code;
+    } catch (const std::bad_alloc&) {
+        ctx->err = "host allocation failed";
+        return H2B_ERR_OOM;
+    } catch (const std::exception& e) {
+        ctx->err = e.what();
+        return H2B_ERR_CUDA;
+    } catch (...) {
+        ctx->err = "unknown failure";
+        return H2B_ERR_CUDA;
+    }
+}
+
 static inline unsigned ceil_div(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 static inline int ceil_log2(size_t n) {
     int l = 0;
@@ -198,7 +225,6 @@ void assign_columns_run(h2b_ctx* ctx, const void* d_vcol, size_t N, const uint64
                         uint32_t k, size_t ncols, void* d_cols);
 void assigned_flatten_run(h2b_ctx* ctx, const void* d_recs, size_t N, void* d_values, uint32_t* d_stats, int invert);
 void assign_lookups_run(h2b_ctx* ctx, const void* d_vals, size_t N, uint32_t k, size_t L, void* d_cols);
-void eval_rational_run(h2b_ctx* ctx, const void* d_num, const void* d_den, size_t n, void* d_out);
 // halo2-base form of the witness (asynchronous; violations land in *d_status, which both zero first)
 void apply_rational_run(h2b_ctx* ctx, void* d_values, size_t N, const uint64_t* d_index, void* d_den, size_t R, uint32_t* d_status);
 // MockProver on halo2-base's keygen data (include/h2b200.h, "MockProver for a halo2-base builder")

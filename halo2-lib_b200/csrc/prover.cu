@@ -180,34 +180,10 @@ void fr_mul_elementwise_run(h2b_ctx* ctx, const void* d_a, const void* d_b, size
 
 using namespace h2b;
 
-// the guarded() wrapper of capi.cu is file-local there; the same mapping, restated for this translation unit
-template <class Fn>
-static int guarded_p(h2b_ctx* ctx, Fn&& body) {
-    if (!ctx) return H2B_ERR_ARG;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    try {
-        H2B_CUDA(cudaSetDevice(ctx->device));
-        body();
-        return H2B_OK;
-    } catch (const StatusError& e) {
-        ctx->err = e.msg;
-        return e.code;
-    } catch (const std::bad_alloc&) {
-        ctx->err = "host allocation failed";
-        return H2B_ERR_OOM;
-    } catch (const std::exception& e) {
-        ctx->err = e.what();
-        return H2B_ERR_CUDA;
-    } catch (...) {
-        ctx->err = "unknown failure";
-        return H2B_ERR_CUDA;
-    }
-}
-
 extern "C" {
 
 int h2b_poly_alloc(h2b_ctx* ctx, size_t n_elems, h2b_poly** out) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(out, "poly_alloc: null output handle");
         *out = nullptr;
         H2B_REQUIRE(n_elems >= 1 && n_elems <= ((size_t)1 << 30), "poly_alloc: size out of range");
@@ -238,7 +214,7 @@ void h2b_poly_free(h2b_ctx* ctx, h2b_poly* poly) {
 void* h2b_poly_device_ptr(const h2b_poly* poly) { return poly ? poly->p : nullptr; }
 size_t h2b_poly_len(const h2b_poly* poly) { return poly ? poly->n : 0; }
 int h2b_poly_upload(h2b_ctx* ctx, h2b_poly* poly, size_t offset, const uint64_t* host, size_t n) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(poly && (host || n == 0), "poly_upload: null pointer");
         H2B_REQUIRE(offset <= poly->n && n <= poly->n - offset, "poly_upload: range outside the polynomial");
         if (n == 0) return;
@@ -247,26 +223,26 @@ int h2b_poly_upload(h2b_ctx* ctx, h2b_poly* poly, size_t offset, const uint64_t*
     });
 }
 int h2b_poly_upload_async(h2b_ctx* ctx, h2b_poly* poly, size_t offset, const uint64_t* pinned_host, size_t n) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(poly && (pinned_host || n == 0), "poly_upload_async: null pointer");
         H2B_REQUIRE(offset <= poly->n && n <= poly->n - offset, "poly_upload_async: range outside the polynomial");
         if (n) H2B_CUDA(cudaMemcpyAsync((char*)poly->p + offset * 32, pinned_host, n * 32, cudaMemcpyHostToDevice, ctx->stream));
     });
 }
 int h2b_poly_copy_dev(h2b_ctx* ctx, void* d_dst, const void* d_src, size_t n) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE((d_dst && d_src) || n == 0, "poly_copy: null pointer");
         if (n) H2B_CUDA(cudaMemcpyAsync(d_dst, d_src, n * 32, cudaMemcpyDeviceToDevice, ctx->stream));
     });
 }
 int h2b_poly_zero(h2b_ctx* ctx, h2b_poly* poly) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(poly, "poly_zero: null pointer");
         H2B_CUDA(cudaMemsetAsync(poly->p, 0, poly->n * 32, ctx->stream));
     });
 }
 int h2b_poly_download(h2b_ctx* ctx, const h2b_poly* poly, size_t offset, uint64_t* host, size_t n) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(poly && (host || n == 0), "poly_download: null pointer");
         H2B_REQUIRE(offset <= poly->n && n <= poly->n - offset, "poly_download: range outside the polynomial");
         if (n == 0) return;
@@ -278,7 +254,7 @@ int h2b_poly_download(h2b_ctx* ctx, const h2b_poly* poly, size_t offset, uint64_
 int h2b_permutation_product_dev(h2b_ctx* ctx, const void* const* d_columns, const void* const* d_sigma, size_t n_cols, size_t first_col,
                                 const uint64_t beta[4], const uint64_t gamma[4], uint32_t k, uint32_t blinding_factors,
                                 const void* d_start, void* d_z) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(d_columns && d_sigma && beta && gamma && d_z, "permutation_product: null pointer");
         permutation_product_run(ctx, d_columns, d_sigma, n_cols, first_col, beta, gamma, k, blinding_factors, d_start, d_z);
     });
@@ -286,19 +262,19 @@ int h2b_permutation_product_dev(h2b_ctx* ctx, const void* const* d_columns, cons
 int h2b_lookup_product_dev(h2b_ctx* ctx, const void* d_input, const void* d_table, const void* d_permuted_input,
                            const void* d_permuted_table, const uint64_t beta[4], const uint64_t gamma[4], uint32_t k,
                            uint32_t blinding_factors, void* d_z) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE(d_input && d_table && d_permuted_input && d_permuted_table && beta && gamma && d_z, "lookup_product: null pointer");
         lookup_product_run(ctx, d_input, d_table, d_permuted_input, d_permuted_table, beta, gamma, k, blinding_factors, d_z);
     });
 }
 int h2b_fr_mul_elementwise_dev(h2b_ctx* ctx, const void* d_a, const void* d_b, size_t n, void* d_out) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE((d_a && d_b && d_out) || n == 0, "fr_mul_elementwise: null pointer");
         fr_mul_elementwise_run(ctx, d_a, d_b, n, d_out);
     });
 }
 int h2b_eval_polynomial_batch_dev(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* xs, size_t m, size_t n, uint64_t* out) {
-    return guarded_p(ctx, [&] {
+    return guarded(ctx, [&] {
         H2B_REQUIRE((d_polys && xs && out) || m == 0, "eval_polynomial_batch: null pointer");
         if (m == 0) return;
         H2B_REQUIRE(m <= 4096, "eval_polynomial_batch: at most 4096 evaluations per call");
