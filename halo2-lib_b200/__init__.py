@@ -9,6 +9,10 @@ from .host import (  # noqa: F401
     ConstraintSystemFailure,
     Context,
     ParamsKZG,
+    gen_srs,
+    srs_path,
+    seeded_tau,
+    g2_generator_mul,
     EvaluationDomain,
     best_multiexp,
     best_fft,

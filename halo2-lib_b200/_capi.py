@@ -119,6 +119,12 @@ SIGNATURES = {
     "h2b_params_processed_view": (_int, [_vp, _sz, C.POINTER(_u32), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
     "h2b_srs_read_processed": (_int, [_vp, _vp, _sz, _sz, _sz, C.POINTER(_vp)]),
     "h2b_params_raw_view": (_int, [_vp, _sz, C.POINTER(_u32), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz), C.POINTER(_sz)]),
+    "h2b_g1_compress": (_int, [_vp, _vp, _sz, _vp]),
+    "h2b_g1_compress_dev": (_int, [_vp, _vp, _sz, _vp]),
+    "h2b_srs_seeded_tau": (_int, [_vp, _vp]),
+    "h2b_g2_generator_mul": (_int, [_vp, _vp, _vp]),
+    "h2b_params_write_processed": (_int, [_vp, _vp, _vp, _u32, _vp, _vp, C.POINTER(_sz)]),
+    "h2b_params_write_raw": (_int, [_vp, _vp, _vp, _u32, _vp, _vp, C.POINTER(_sz)]),
     "h2b_permute_expression_pair": (_int, [_vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "h2b_permute_expression_pair_dev": (_int, [_vp, _vp, _vp, _u32, _u32, _vp, _vp]),
     "h2b_permute_expression_pair_async_dev": (_int, [_vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp]),

@@ -1,6 +1,7 @@
 // capi.cu — the extern "C" surface declared in include/h2b200.h: context, SRS handles, staging of host buffers.
 // No exception leaves this file: every entry point maps failures to a status code + h2b_last_error().
 #include <cstring>
+#include <functional>
 
 #include "h2b_internal.cuh"
 
@@ -1148,6 +1149,60 @@ int h2b_srs_read_processed(h2b_ctx* ctx, const uint8_t* bytes, size_t len, size_
 int h2b_params_raw_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset, size_t* g2_offset,
                         size_t* s_g2_offset) {
     return params_view(bytes, len, 64, 128, k, g_offset, g_lagrange_offset, g2_offset, s_g2_offset);
+}
+int h2b_g1_compress_dev(h2b_ctx* ctx, const void* d_xy, size_t n, void* d_bytes) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((d_xy && d_bytes) || n == 0, "g1_compress: null pointer");
+        g1_compress_run(ctx, d_xy, n, d_bytes);
+    });
+}
+int h2b_g1_compress(h2b_ctx* ctx, const uint64_t* xy, size_t n, uint8_t* bytes) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE((xy && bytes) || n == 0, "g1_compress: null pointer");
+        if (n == 0) return;
+        Staging st(ctx, WS_BASES, n * 96);
+        void *d_in = st.up(xy, n * 64), *d_out = st.out(bytes, n * 32);
+        g1_compress_run(ctx, d_in, n, d_out);
+        st.finish();
+    });
+}
+// `ParamsKZG::write`: u32 LE k | g | g_lagrange | g2 | s_g2 with G1 points of `g1` bytes and the caller's `g2_bytes` bytes of
+// G2 encodings.  A null `out` asks for the size (no device work); otherwise *len is the capacity on entry, the size on return.
+static int params_write(h2b_ctx* ctx, uint32_t k, size_t g1, size_t g2_bytes, const void* d_g, const void* d_gl, const uint8_t* g2,
+                        uint8_t* out, size_t* len, const std::function<void(size_t, uint8_t*)>& bases) {
+    if (!len || k > 28) return H2B_ERR_ARG;
+    const size_t n = (size_t)1 << k, need = 4 + 2 * n * g1 + g2_bytes;
+    if (!out) {
+        *len = need;
+        return H2B_OK;
+    }
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_g && d_gl && g2, "params_write: null pointer");
+        H2B_REQUIRE(*len >= need, "params_write: the buffer is shorter than the image");
+        for (int i = 0; i < 4; i++) out[i] = (uint8_t)(k >> (8 * i));
+        bases(n, out + 4);
+        std::memcpy(out + 4 + 2 * n * g1, g2, g2_bytes);
+        *len = need;
+    });
+}
+int h2b_params_write_processed(h2b_ctx* ctx, const void* d_g, const void* d_g_lagrange, uint32_t k, const uint8_t g2[128], uint8_t* out,
+                               size_t* len) {
+    return params_write(ctx, k, 32, 128, d_g, d_g_lagrange, g2, out, len, [&](size_t n, uint8_t* dst) {
+        // both bases compressed into one staging buffer, one download
+        Staging st(ctx, WS_BASES, 2 * n * 32);
+        char* d = st.out(dst, 2 * n * 32);
+        g1_compress_run(ctx, d_g, n, d);
+        g1_compress_run(ctx, d_g_lagrange, n, d + n * 32);
+        st.finish();
+    });
+}
+int h2b_params_write_raw(h2b_ctx* ctx, const void* d_g, const void* d_g_lagrange, uint32_t k, const uint8_t g2[256], uint8_t* out, size_t* len) {
+    return params_write(ctx, k, 64, 256, d_g, d_g_lagrange, g2, out, len, [&](size_t n, uint8_t* dst) {
+        // the bases already are the RawBytes layout (Montgomery limbs)
+        H2B_CUDA(cudaMemcpyAsync(dst, d_g, n * 64, cudaMemcpyDeviceToHost, ctx->stream));
+        H2B_CUDA(cudaMemcpyAsync(dst + n * 64, d_g_lagrange, n * 64, cudaMemcpyDeviceToHost, ctx->stream));
+        H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+    });
 }
 
 // ------------------------------------------------------------------------------------------------ lookup permutation

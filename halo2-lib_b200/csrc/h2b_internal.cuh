@@ -294,6 +294,7 @@ void g_to_lagrange_run(h2b_ctx* ctx, const void* d_g, uint32_t k, void* d_g_lagr
 void srs_setup_run(h2b_ctx* ctx, const uint64_t tau[4], const uint64_t base_xy[8], uint32_t k, void* d_g, void* d_g_lagrange);
 size_t g1_count_off_curve_run(h2b_ctx* ctx, const void* d_points, size_t n);
 size_t g1_decompress_run(h2b_ctx* ctx, const void* d_bytes, size_t n, void* d_out_xy);
+void g1_compress_run(h2b_ctx* ctx, const void* d_xy, size_t n, void* d_bytes);
 // ---- poly.cu
 void eval_polynomial_run(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t x[4], void* d_out);
 void eval_polynomial_batch_run(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* xs, size_t m, size_t n, void* d_out);

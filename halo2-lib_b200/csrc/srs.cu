@@ -85,6 +85,23 @@ __global__ void __launch_bounds__(128) k_g1_decompress(const uint8_t* __restrict
     if (bad) atomicAdd(invalid, 1ull);
     r.store(out + i);
 }
+// the inverse of k_g1_decompress (`G1Affine::to_bytes`, what `ParamsKZG::write` emits in SerdeFormat::Processed): canonical x
+// little-endian, bit 6 of byte 31 = parity of the canonical y; the identity (0, 0) -> all zero but bit 7 of byte 31.  Two
+// from_mont per point and nothing else: 64 bytes read, 32 written, bound by HBM.
+__global__ void __launch_bounds__(256) k_g1_compress(const Affine* __restrict__ pts, size_t n, uint8_t* __restrict__ bytes) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Affine p = Affine::load(pts + i);
+    uint4 lo = make_uint4(0, 0, 0, 0), hi = make_uint4(0, 0, 0, 0x80000000u);
+    if (!p.is_identity()) {
+        const Fq x = p.x.from_mont(), y = p.y.from_mont();
+        lo = make_uint4(x.l[0], x.l[1], x.l[2], x.l[3]);
+        hi = make_uint4(x.l[4], x.l[5], x.l[6], x.l[7] | ((y.l[0] & 1u) << 30));
+    }
+    uint4* q = reinterpret_cast<uint4*>(bytes + 32 * i);
+    q[0] = lo;
+    q[1] = hi;
+}
 
 // ---------------------------------------------------------------- GLV scalar multiplication
 // lambda = 0xb3c4d79d41a917585bfc41088d8daaa78b17ea66b99c90dd (lambda^2 + lambda + 1 = 0 mod r) acts on G1 as
@@ -373,6 +390,12 @@ size_t g1_decompress_run(h2b_ctx* ctx, const void* d_bytes, size_t n, void* d_ou
     H2B_CUDA(cudaMemcpyAsync(bounce, d_cnt, 8, cudaMemcpyDeviceToHost, ctx->stream));
     H2B_CUDA(cudaStreamSynchronize(ctx->stream));
     return (size_t)bounce[0];
+}
+
+// points: n affine Montgomery points on the device -> n x 32 bytes on the device (asynchronous)
+void g1_compress_run(h2b_ctx* ctx, const void* d_xy, size_t n, void* d_bytes) {
+    if (n == 0) return;
+    H2B_LAUNCH(ctx, k_g1_compress, ceil_div(n, 256), 256, 0, (const Affine*)d_xy, n, (uint8_t*)d_bytes);
 }
 
 }  // namespace h2b

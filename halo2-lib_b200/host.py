@@ -12,8 +12,9 @@ Arrays are numpy uint64 in the `[u64;4]` little-endian Montgomery layout.  Every
 through libh2b200.so; nothing here does field arithmetic on the CPU."""
 from __future__ import annotations
 import ctypes as C
+import os
 import numpy as np
-from ._capi import lib, H2B_OK, H2B_ERR_LAYOUT, H2B_ERR_UNSATISFIED, BASIS_MONOMIAL, BASIS_LAGRANGE
+from ._capi import lib, H2B_OK, H2B_ERR_ARG, H2B_ERR_LAYOUT, H2B_ERR_UNSATISFIED, BASIS_MONOMIAL, BASIS_LAGRANGE
 
 
 class H2BError(RuntimeError):
@@ -185,14 +186,70 @@ def best_fft(ctx: Context, a, omega_m, log_n: int) -> np.ndarray:
     return a
 
 
+_P_MOD = 0x30644E72E131A029B85045B68181585D97816A916871CA8D3C208C16D87CFD47
+# the G1 generator (1, 2), Montgomery limbs: the base of ParamsKZG::setup
+G1_GENERATOR = np.array([(v << 256) % _P_MOD >> (64 * i) & 0xFFFFFFFFFFFFFFFF for v in (1, 2) for i in range(4)], dtype=np.uint64)
+
+
+class _DeviceBuffer:
+    """`elems` x 32 bytes of device memory (one h2b_poly); an affine G1 point takes two elements"""
+
+    def __init__(self, ctx: Context, elems: int):
+        self.ctx, h = ctx, C.c_void_p()
+        ctx.check(lib.h2b_poly_alloc(ctx.h, elems, C.byref(h)))
+        self.h, self.ptr = h, int(lib.h2b_poly_device_ptr(h))
+
+    def free(self):
+        if self.h:
+            lib.h2b_poly_free(self.ctx.h, self.h)
+            self.h = None
+
+
+def seeded_tau(seed: bytes = bytes(32)) -> np.ndarray:
+    """tau of `ParamsKZG::setup(k, ChaCha20Rng::from_seed(seed))` (gen_srs: 32 zero bytes), Montgomery limbs"""
+    s = np.frombuffer(bytes(seed), dtype=np.uint8).copy()
+    assert len(s) == 32, "the seed is 32 bytes"
+    t = np.zeros(4, dtype=np.uint64)
+    rc = lib.h2b_srs_seeded_tau(_ptr8(s), _ptr(t))
+    if rc != H2B_OK:
+        raise H2BError(rc, "h2b_srs_seeded_tau")
+    return t
+
+
+def g2_generator_mul(tau) -> tuple[bytes, bytes]:
+    """(g2 | s_g2 compressed, g2 | s_g2 raw) with s_g2 = tau * g2: the G2 pair of a params image in both formats"""
+    t = _u64(tau, 4).reshape(4)
+    proc, raw = np.zeros(128, dtype=np.uint8), np.zeros(256, dtype=np.uint8)
+    rc = lib.h2b_g2_generator_mul(_ptr(t), _ptr8(proc), _ptr8(raw))
+    if rc != H2B_OK:
+        raise H2BError(rc, "h2b_g2_generator_mul: tau must be below r")
+    return proc.tobytes(), raw.tobytes()
+
+
+def _ptr8(a: np.ndarray):
+    return C.c_void_p(a.ctypes.data)
+
+
+def _image_view(view, image: np.ndarray) -> tuple:
+    k, off = C.c_uint32(), [C.c_size_t() for _ in range(4)]
+    if view(_ptr8(image), len(image), C.byref(k), *[C.byref(o) for o in off]) != H2B_OK:
+        raise H2BError(H2B_ERR_ARG, "not a params image")
+    return k.value, [o.value for o in off]
+
+
 class ParamsKZG:
-    """The base arrays of `ParamsKZG<Bn256>` (g, g_lagrange) resident on the GPU, sharded [begin, begin+count)."""
+    """The base arrays of `ParamsKZG<Bn256>` (g, g_lagrange) resident on the GPU, sharded [begin, begin+count).
+
+    Params made by setup_seeded / gen_srs / read_downsized also keep g and g_lagrange themselves on the device (whole, not
+    sharded) and the G2 pair (g2, s_g2), so that they can be written (`ParamsKZG::write`) and downsized."""
 
     def __init__(self, ctx: Context, k: int, g=None, g_lagrange=None, begin: int = 0, count: int | None = None,
                  device_ptrs: bool = False):
         self.ctx, self.k, self.n = ctx, k, 1 << k
         self.begin = begin
         self.count = (self.n - begin) if count is None else count
+        self._g = self._gl = None  # _DeviceBuffer of setup_seeded / read_downsized
+        self.g2_processed = self.g2_raw = None  # g2 | s_g2 in the Processed (128 bytes) and RawBytes (256 bytes) encodings
         h = C.c_void_p()
         if device_ptrs:
             rc = lib.h2b_srs_upload_dev(ctx.h, C.c_void_p(g or 0), C.c_void_p(g_lagrange or 0), k, begin, self.count, C.byref(h))
@@ -241,16 +298,150 @@ class ParamsKZG:
     def commit_dev(self, basis: int, d_scalars: int, n: int, d_out: int):
         self.ctx.check(lib.h2b_msm_g1_dev(self.ctx.h, self.h, basis, C.c_void_p(d_scalars), n, C.c_void_p(d_out)))
 
+    # ---- creating, writing and downsizing halo2-lib's params (gen_srs, ParamsKZG::write, Params::downsize)
+    @classmethod
+    def _resident(cls, ctx: Context, k: int, g: _DeviceBuffer, gl: _DeviceBuffer, g2_processed, g2_raw):
+        try:
+            params = cls(ctx, k, g.ptr, gl.ptr, device_ptrs=True)
+        except Exception:
+            g.free(); gl.free()
+            raise
+        params._g, params._gl, params.g2_processed, params.g2_raw = g, gl, g2_processed, g2_raw
+        return params
+
+    @classmethod
+    def setup_seeded(cls, ctx: Context, k: int, seed: bytes = bytes(32)) -> "ParamsKZG":
+        """`ParamsKZG::setup(k, ChaCha20Rng::from_seed(seed))`, what gen_srs creates: g, g_lagrange at halo2-lib's tau on the
+        device, the G2 pair on the host"""
+        tau = seeded_tau(seed)
+        g, gl = _DeviceBuffer(ctx, 2 << k), _DeviceBuffer(ctx, 2 << k)
+        try:
+            ctx.check(lib.h2b_srs_setup_dev(ctx.h, _ptr(tau), _ptr(G1_GENERATOR), k, C.c_void_p(g.ptr), C.c_void_p(gl.ptr)))
+        except Exception:
+            g.free(); gl.free()
+            raise
+        return cls._resident(ctx, k, g, gl, *g2_generator_mul(tau))
+
+    @classmethod
+    def read_downsized(cls, ctx: Context, image, k: int | None = None) -> "ParamsKZG":
+        """`read_params(K).downsize(k)` from a SerdeFormat::Processed image: only the first 2^k encodings of g are decompressed,
+        g_lagrange is rebuilt from them (g_to_lagrange) and G2 is kept; the 2^K bases never reach the device.  H2BError
+        (H2B_ERR_ARG) for a malformed image or an invalid encoding."""
+        img = np.frombuffer(bytes(image), dtype=np.uint8) if not isinstance(image, np.ndarray) else np.ascontiguousarray(image, dtype=np.uint8)
+        big_k, (og, _, og2, _) = _image_view(lib.h2b_params_processed_view, img)
+        k = big_k if k is None else k
+        if k > big_k:
+            raise H2BError(H2B_ERR_ARG, f"downsize: k = {k} above the image's k = {big_k}")
+        n = 1 << k
+        enc, g, gl = _DeviceBuffer(ctx, n), _DeviceBuffer(ctx, 2 * n), _DeviceBuffer(ctx, 2 * n)
+        try:
+            ctx.check(lib.h2b_poly_upload(ctx.h, enc.h, 0, _ptr8(img[og:og + 32 * n]), n))
+            bad = C.c_size_t()
+            ctx.check(lib.h2b_g1_decompress_dev(ctx.h, C.c_void_p(enc.ptr), n, C.c_void_p(g.ptr), C.byref(bad)))
+            if bad.value:
+                raise H2BError(H2B_ERR_ARG, "read_params: the params image holds an invalid G1 encoding")
+            ctx.check(lib.h2b_g_to_lagrange_dev(ctx.h, C.c_void_p(g.ptr), k, C.c_void_p(gl.ptr)))
+        except Exception:
+            g.free(); gl.free()
+            raise
+        finally:
+            enc.free()
+        return cls._resident(ctx, k, g, gl, img[og2:og2 + 128].tobytes(), None)
+
+    @classmethod
+    def read(cls, ctx: Context, image) -> "ParamsKZG":
+        """`ParamsKZG::read` of a SerdeFormat::Processed image: the SRS handle through h2b_srs_read_processed (the bases are
+        not kept, so these params cannot be written or downsized); H2BError (H2B_ERR_ARG) for a malformed image or an invalid
+        encoding"""
+        img = np.frombuffer(bytes(image), dtype=np.uint8) if not isinstance(image, np.ndarray) else np.ascontiguousarray(image, dtype=np.uint8)
+        h = C.c_void_p()
+        ctx.check(lib.h2b_srs_read_processed(ctx.h, _ptr8(img), len(img), 0, 0, C.byref(h)))
+        params = cls.__new__(cls)
+        k, (_, _, og2, _) = _image_view(lib.h2b_params_processed_view, img)
+        params.ctx, params.k, params.n, params.begin, params.count, params.h = ctx, k, 1 << k, 0, 1 << k, h
+        params._g = params._gl = params.g2_raw = None
+        params.g2_processed = img[og2:og2 + 128].tobytes()
+        cb, w = C.c_int(), C.c_int()
+        lib.h2b_srs_info(h, C.byref(cb), C.byref(w))
+        params.window_bits, params.windows = cb.value, w.value
+        return params
+
+    def _need_bases(self, what: str):
+        if self._g is None:
+            raise H2BError(H2B_ERR_ARG, f"{what}: these params do not keep their bases on the device (use setup_seeded / read_downsized)")
+
+    def write(self, format: str = "processed") -> bytes:
+        """`ParamsKZG::write` in SerdeFormat::Processed ("processed") or RawBytes ("raw"): u32 LE k | g | g_lagrange | g2 | s_g2"""
+        self._need_bases("write")
+        fn, g2 = {"processed": (lib.h2b_params_write_processed, self.g2_processed), "raw": (lib.h2b_params_write_raw, self.g2_raw)}[format]
+        if g2 is None:
+            raise H2BError(H2B_ERR_ARG, f"write: the {format} encoding of G2 is not known for params read from an image")
+        ln = C.c_size_t()
+        self.ctx.check(fn(self.ctx.h, None, None, self.k, None, None, C.byref(ln)))
+        out = np.empty(ln.value, dtype=np.uint8)
+        g2a = np.frombuffer(g2, dtype=np.uint8).copy()
+        self.ctx.check(fn(self.ctx.h, C.c_void_p(self._g.ptr), C.c_void_p(self._gl.ptr), self.k, _ptr8(g2a), _ptr8(out), C.byref(ln)))
+        return out.tobytes()
+
+    def downsize(self, k: int):
+        """`Params::downsize(k)` in place: g keeps its first 2^k points, g_lagrange is rebuilt from them, G2 stays"""
+        self._need_bases("downsize")
+        if k > self.k:
+            raise H2BError(H2B_ERR_ARG, f"downsize: k = {k} above the params' k = {self.k}")
+        n = 1 << k
+        g, gl = _DeviceBuffer(self.ctx, 2 * n), _DeviceBuffer(self.ctx, 2 * n)
+        try:
+            self.ctx.check(lib.h2b_poly_copy_dev(self.ctx.h, C.c_void_p(g.ptr), C.c_void_p(self._g.ptr), 2 * n))
+            self.ctx.check(lib.h2b_g_to_lagrange_dev(self.ctx.h, C.c_void_p(g.ptr), k, C.c_void_p(gl.ptr)))
+            h = C.c_void_p()
+            self.ctx.check(lib.h2b_srs_upload_dev(self.ctx.h, C.c_void_p(g.ptr), C.c_void_p(gl.ptr), k, 0, n, C.byref(h)))
+        except Exception:
+            g.free(); gl.free()
+            raise
+        lib.h2b_srs_destroy(self.ctx.h, self.h)
+        self._g.free(); self._gl.free()
+        self.h, self._g, self._gl, self.k, self.n, self.count = h, g, gl, k, n, n
+        cb, w = C.c_int(), C.c_int()
+        lib.h2b_srs_info(self.h, C.byref(cb), C.byref(w))
+        self.window_bits, self.windows = cb.value, w.value
+
     def close(self):
         if getattr(self, "h", None):
             lib.h2b_srs_destroy(self.ctx.h, self.h)
             self.h = None
+        for b in (getattr(self, "_g", None), getattr(self, "_gl", None)):
+            if b is not None:
+                b.free()
 
     def __del__(self):
         try:
             self.close()
         except Exception:
             pass
+
+
+def srs_path(k: int, dir: str | None = None) -> str:
+    """where gen_srs caches the params of 2^k rows: $PARAMS_DIR (or ./params) / kzg_bn254_{k}.srs"""
+    return os.path.join(dir if dir is not None else os.environ.get("PARAMS_DIR", "./params"), f"kzg_bn254_{k}.srs")
+
+
+def gen_srs(ctx: Context, k: int, dir: str | None = None) -> ParamsKZG:
+    """halo2-base `gen_srs(k)` = read_or_create_srs: read the cached SerdeFormat::Processed params when the file exists
+    (ParamsKZG.read), else create them with setup_seeded (zero seed), create the directory and write the file"""
+    path = srs_path(k, dir)
+    if os.path.exists(path):
+        with open(path, "rb") as f:
+            return ParamsKZG.read(ctx, f.read())
+    params = ParamsKZG.setup_seeded(ctx, k)
+    try:
+        image = params.write("processed")
+        os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
+        with open(path, "wb") as f:
+            f.write(image)
+    except Exception:
+        params.close()
+        raise
+    return params
 
 
 class EvaluationDomain:

@@ -147,6 +147,30 @@ int h2b_g1_decompress_dev(h2b_ctx* ctx, const void* d_bytes, size_t n, void* d_o
 int h2b_params_processed_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset,
                               size_t* g2_offset, size_t* s_g2_offset);
 int h2b_srs_read_processed(h2b_ctx* ctx, const uint8_t* bytes, size_t len, size_t begin, size_t count, h2b_srs** out);
+/* The write side (`gen_srs` = read_or_create_srs, halo2-base/src/utils/mod.rs:413-443, and `ParamsKZG::write`).
+ * h2b_g1_compress: n affine points (Montgomery, identity (0,0)) -> n x 32-byte encodings, the exact inverse of
+ * h2b_g1_decompress (canonical x little-endian, bit 6 of byte 31 = parity of the canonical y, identity = all zero but bit 7
+ * of byte 31); one thread per point.
+ * h2b_srs_seeded_tau: the tau of `ParamsKZG::setup(k, ChaCha20Rng::from_seed(seed))` (gen_srs: seed = 32 zero bytes):
+ * rand_chacha's ChaCha20 stream (64-bit block counter from 0, stream 0), 64 bytes through `Fr::random` =
+ * from_uniform_bytes, (lo + hi 2^256) mod r; tau in Montgomery form.  Host-only.
+ * h2b_g2_generator_mul: g2 = the EIP-197 generator of the BN254 twist and s_g2 = tau * g2 in both encodings of a params
+ * image: processed = g2 | s_g2 compressed (64 bytes each: x.c0 | x.c1 canonical little-endian, bit 7 of byte 63 =
+ * identity, bit 6 = sgn0(y)), raw = g2 | s_g2 as x.c0 | x.c1 | y.c0 | y.c1 Montgomery limbs (128 bytes each); either output may
+ * be NULL.  tau must be below r.  Host-only.
+ * h2b_params_write_processed / h2b_params_write_raw: the image u32 LE k | g | g_lagrange | g2 | s_g2 from the device bases
+ * d_g, d_g_lagrange (2^k x 8 limbs each) and the G2 pair of h2b_g2_generator_mul, into the caller's buffer `out`: *len is
+ * its capacity on entry and the image size on return; out = NULL only asks for the size.  Processed compresses both bases on
+ * the device into one staging buffer and downloads it with one copy.  h2b_params_processed_view / h2b_srs_read_processed /
+ * h2b_params_raw_view read the images back. */
+int h2b_g1_compress(h2b_ctx* ctx, const uint64_t* xy, size_t n, uint8_t* bytes);
+int h2b_g1_compress_dev(h2b_ctx* ctx, const void* d_xy, size_t n, void* d_bytes);
+int h2b_srs_seeded_tau(const uint8_t seed[32], uint64_t tau[4]);
+int h2b_g2_generator_mul(const uint64_t tau[4], uint8_t processed[128], uint8_t raw[256]);
+int h2b_params_write_processed(h2b_ctx* ctx, const void* d_g, const void* d_g_lagrange, uint32_t k, const uint8_t g2[128], uint8_t* out,
+                               size_t* len);
+int h2b_params_write_raw(h2b_ctx* ctx, const void* d_g, const void* d_g_lagrange, uint32_t k, const uint8_t g2[256], uint8_t* out,
+                         size_t* len);
 
 /* ---- MSM: replaces halo2curves-axiom 0.7.3 msm::best_multiexp(coeffs, bases) -> G1, as reached from
  *      ParamsKZG::commit / commit_lagrange inside create_proof (SURVEY.md §3.3, §8 a2/a4) ------------- */

@@ -22,6 +22,9 @@
 //   halo2_proofs::poly::EvaluationDomain::divide_by_vanishing_poly                    h2b::divide_by_vanishing_poly
 //   halo2_proofs::arithmetic::{eval_polynomial, kate_division}                        h2b::eval_polynomial, kate_division
 //   halo2_proofs::poly::kzg::commitment::g_to_lagrange                                h2b::g_to_lagrange
+//   ParamsKZG::{setup (ChaCha20Rng seeded), write, read}, Params::downsize              h2b::ParamsKZG::{setup_seeded, write,
+//                                                                                     read, read_downsized, downsize}
+//   halo2_base::utils::fs::gen_srs (read_or_create_srs, utils/mod.rs:413-443)         h2b::gen_srs
 //
 // Where the Rust code panics (`expect("prover should not fail")`, halo2-base/src/utils/testing.rs:48; index out of
 // bounds in assign_witnesses) these wrappers throw h2b::Error; nothing is computed on the CPU.
@@ -29,6 +32,9 @@
 #include <algorithm>
 #include <array>
 #include <cstdint>
+#include <cstdlib>
+#include <filesystem>
+#include <fstream>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -105,7 +111,51 @@ inline void best_fft(const Context& ctx, std::vector<Fr>& a, const Fr& omega, ui
     ctx.check(h2b_ntt_fr(ctx.raw(), reinterpret_cast<uint64_t*>(a.data()), log_n, omega.data(), 0));
 }
 
+enum class SerdeFormat { Processed, RawBytes };
+
+namespace detail {
+// elems x 32 bytes of device memory (one h2b_poly); an affine G1 point takes two elements
+class DeviceBuffer {
+public:
+    DeviceBuffer() = default;
+    DeviceBuffer(const Context& ctx, size_t elems) : ctx_(&ctx) { ctx.check(h2b_poly_alloc(ctx.raw(), elems, &h_)); }
+    DeviceBuffer(DeviceBuffer&& o) noexcept : ctx_(o.ctx_), h_(o.h_) { o.h_ = nullptr; }
+    DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+        std::swap(ctx_, o.ctx_);
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    ~DeviceBuffer() {
+        if (h_) h2b_poly_free(ctx_->raw(), h_);
+    }
+    void* ptr() const { return h_ ? h2b_poly_device_ptr(h_) : nullptr; }
+    h2b_poly* raw() const { return h_; }
+
+private:
+    const Context* ctx_ = nullptr;
+    h2b_poly* h_ = nullptr;
+};
+// the G1 generator (1, 2), Montgomery limbs: the base of ParamsKZG::setup
+inline const uint64_t* g1_generator() {
+    static const uint64_t g[8] = {0xd35d438dc58f0d9dULL, 0x0a78eb28f5c70b3dULL, 0x666ea36f7879462cULL, 0x0e0a77c19a07df2fULL,
+                                  0xa6ba871b8b1e1b3aULL, 0x14f1d651eb8e167bULL, 0xccdd46def0f28c58ULL, 0x1c14ef83340fbe5eULL};
+    return g;
+}
+struct ImageView {
+    uint32_t k;
+    size_t off[4];  // g, g_lagrange, g2, s_g2
+};
+inline ImageView processed_view(const std::vector<uint8_t>& image) {
+    ImageView v{};
+    const int rc = h2b_params_processed_view(image.data(), image.size(), &v.k, &v.off[0], &v.off[1], &v.off[2], &v.off[3]);
+    if (rc != H2B_OK) throw Error(H2B_ERR_ARG, "read_params: not a SerdeFormat::Processed params image");
+    return v;
+}
+}  // namespace detail
+
 // The base arrays of ParamsKZG<Bn256> resident on one GPU (this rank's shard [begin, begin + count)).
+// Params made by setup_seeded / read_downsized (and gen_srs when it creates the file) also keep g and g_lagrange themselves on
+// the device, whole, and the G2 pair (g2, s_g2): they can be written (ParamsKZG::write) and downsized (Params::downsize).
 class ParamsKZG {
 public:
     ParamsKZG(const Context& ctx, uint32_t k, const std::vector<G1Affine>& g, const std::vector<G1Affine>& g_lagrange,
@@ -126,6 +176,82 @@ public:
     }
     ParamsKZG(const ParamsKZG&) = delete;
     ParamsKZG& operator=(const ParamsKZG&) = delete;
+    ParamsKZG(ParamsKZG&& o) noexcept
+        : ctx_(o.ctx_), k_(o.k_), count_(o.count_), srs_(o.srs_), owned_(o.owned_), g_(std::move(o.g_)), gl_(std::move(o.gl_)),
+          g2_processed_(std::move(o.g2_processed_)), g2_raw_(std::move(o.g2_raw_)) {
+        o.srs_ = nullptr;
+    }
+
+    // `ParamsKZG::setup(k, ChaCha20Rng::from_seed(seed))`, what gen_srs creates (seed = 32 zero bytes): g and g_lagrange at
+    // halo2-lib's tau on the device, the G2 pair on the host
+    static ParamsKZG setup_seeded(const Context& ctx, uint32_t k, const std::array<uint8_t, 32>& seed = {}) {
+        Fr tau{};
+        if (h2b_srs_seeded_tau(seed.data(), tau.data()) != H2B_OK) throw Error(H2B_ERR_ARG, "setup_seeded: null seed");
+        detail::DeviceBuffer g(ctx, size_t(2) << k), gl(ctx, size_t(2) << k);
+        ctx.check(h2b_srs_setup_dev(ctx.raw(), tau.data(), detail::g1_generator(), k, g.ptr(), gl.ptr()));
+        std::vector<uint8_t> proc(128), raw(256);
+        if (h2b_g2_generator_mul(tau.data(), proc.data(), raw.data()) != H2B_OK) throw Error(H2B_ERR_ARG, "setup_seeded: tau");
+        return ParamsKZG(ctx, k, std::move(g), std::move(gl), std::move(proc), std::move(raw));
+    }
+    // `ParamsKZG::read` of a SerdeFormat::Processed image (h2b_srs_read_processed): the SRS handle only, so these params cannot
+    // be written or downsized.  Error(H2B_ERR_ARG) for a malformed image or an invalid point encoding.
+    static ParamsKZG read(const Context& ctx, const std::vector<uint8_t>& image) {
+        const detail::ImageView v = detail::processed_view(image);
+        ParamsKZG p(ctx, v.k, nullptr, size_t(1) << v.k);
+        p.owned_ = true;
+        ctx.check(h2b_srs_read_processed(ctx.raw(), image.data(), image.size(), 0, 0, &p.srs_));
+        p.g2_processed_.assign(image.begin() + v.off[2], image.begin() + v.off[2] + 128);
+        return p;
+    }
+    // `read_params(K).downsize(k)` from a SerdeFormat::Processed image: only the first 2^k encodings of g are decompressed on the
+    // device, g_lagrange is rebuilt from them and G2 is kept; the 2^K bases never reach the device
+    static ParamsKZG read_downsized(const Context& ctx, const std::vector<uint8_t>& image, uint32_t k) {
+        const detail::ImageView v = detail::processed_view(image);
+        if (k > v.k) throw Error(H2B_ERR_ARG, "downsize: k above the image's k");
+        const size_t n = size_t(1) << k;
+        detail::DeviceBuffer enc(ctx, n), g(ctx, 2 * n), gl(ctx, 2 * n);
+        ctx.check(h2b_poly_upload(ctx.raw(), enc.raw(), 0, reinterpret_cast<const uint64_t*>(image.data() + v.off[0]), n));
+        size_t bad = 0;
+        ctx.check(h2b_g1_decompress_dev(ctx.raw(), enc.ptr(), n, g.ptr(), &bad));
+        if (bad) throw Error(H2B_ERR_ARG, "read_params: the params image holds an invalid G1 encoding");
+        ctx.check(h2b_g_to_lagrange_dev(ctx.raw(), g.ptr(), k, gl.ptr()));
+        return ParamsKZG(ctx, k, std::move(g), std::move(gl), std::vector<uint8_t>(image.begin() + v.off[2], image.begin() + v.off[2] + 128), {});
+    }
+    // `ParamsKZG::write`: u32 LE k | g | g_lagrange | g2 | s_g2
+    std::vector<uint8_t> write(SerdeFormat format = SerdeFormat::Processed) const {
+        need_bases("write");
+        const bool proc = format == SerdeFormat::Processed;
+        const std::vector<uint8_t>& g2 = proc ? g2_processed_ : g2_raw_;
+        if (g2.empty()) throw Error(H2B_ERR_ARG, "write: the G2 encoding of this format is not known for params read from an image");
+        auto fn = proc ? h2b_params_write_processed : h2b_params_write_raw;
+        size_t len = 0;
+        ctx_.check(fn(ctx_.raw(), nullptr, nullptr, k_, nullptr, nullptr, &len));
+        std::vector<uint8_t> out(len);
+        ctx_.check(fn(ctx_.raw(), g_.ptr(), gl_.ptr(), k_, g2.data(), out.data(), &len));
+        return out;
+    }
+    // `Params::downsize(k)` in place: g keeps its first 2^k points, g_lagrange is rebuilt from them (g_to_lagrange), G2 stays
+    void downsize(uint32_t k) {
+        need_bases("downsize");
+        if (k > k_) throw Error(H2B_ERR_ARG, "downsize: k above the params' k");
+        const size_t n = size_t(1) << k;
+        detail::DeviceBuffer g(ctx_, 2 * n), gl(ctx_, 2 * n);
+        ctx_.check(h2b_poly_copy_dev(ctx_.raw(), g.ptr(), g_.ptr(), 2 * n));
+        ctx_.check(h2b_g_to_lagrange_dev(ctx_.raw(), g.ptr(), k, gl.ptr()));
+        h2b_srs* srs = nullptr;
+        ctx_.check(h2b_srs_upload_dev(ctx_.raw(), g.ptr(), gl.ptr(), k, 0, n, &srs));
+        if (owned_) h2b_srs_destroy(ctx_.raw(), srs_);
+        srs_ = srs;
+        owned_ = true;
+        g_ = std::move(g);
+        gl_ = std::move(gl);
+        k_ = k;
+        count_ = n;
+    }
+    // the whole bases on the device (2^k x 8 limbs each), null for params that do not keep them
+    const void* g_dev() const { return g_.ptr(); }
+    const void* g_lagrange_dev() const { return gl_.ptr(); }
+    const std::vector<uint8_t>& g2_processed() const { return g2_processed_; }  // g2 | s_g2, 64 bytes each
     uint32_t k() const { return k_; }
     const h2b_srs* raw() const { return srs_; }  // for the `_dev` entry points (the resident prover, h2b200_prover.hpp)
     // ParamsKZG::commit(poly in coefficient form) / commit_lagrange(poly in Lagrange form)
@@ -146,6 +272,15 @@ public:
     }
 
 private:
+    ParamsKZG(const Context& ctx, uint32_t k, detail::DeviceBuffer g, detail::DeviceBuffer gl, std::vector<uint8_t> g2_processed,
+              std::vector<uint8_t> g2_raw)
+        : ctx_(ctx), k_(k), count_(size_t(1) << k), g_(std::move(g)), gl_(std::move(gl)), g2_processed_(std::move(g2_processed)),
+          g2_raw_(std::move(g2_raw)) {
+        ctx.check(h2b_srs_upload_dev(ctx.raw(), g_.ptr(), gl_.ptr(), k, 0, count_, &srs_));
+    }
+    void need_bases(const char* what) const {
+        if (!g_.ptr()) throw Error(H2B_ERR_ARG, std::string(what) + ": these params do not keep their bases on the device");
+    }
     G1 commit_(int basis, const std::vector<Fr>& poly) const {
         G1 out;
         ctx_.check(h2b_msm_g1(ctx_.raw(), srs_, basis, reinterpret_cast<const uint64_t*>(poly.data()), poly.size(), out.x.data()));
@@ -156,7 +291,35 @@ private:
     size_t count_;
     h2b_srs* srs_ = nullptr;
     bool owned_ = true;
+    detail::DeviceBuffer g_, gl_;
+    std::vector<uint8_t> g2_processed_, g2_raw_;
 };
+
+// where gen_srs caches the params of 2^k rows: dir (default $PARAMS_DIR, else ./params) / kzg_bn254_{k}.srs
+inline std::string srs_path(uint32_t k, std::string dir = "") {
+    if (dir.empty()) {
+        const char* env = std::getenv("PARAMS_DIR");
+        dir = env ? env : "./params";
+    }
+    return dir + "/kzg_bn254_" + std::to_string(k) + ".srs";
+}
+// halo2-base `gen_srs(k)` = read_or_create_srs: read the cached SerdeFormat::Processed params when the file exists
+// (ParamsKZG::read), else create them (setup_seeded, zero seed), create the directory and write the file
+inline ParamsKZG gen_srs(const Context& ctx, uint32_t k, const std::string& dir = "") {
+    const std::string path = srs_path(k, dir);
+    std::ifstream in(path, std::ios::binary);
+    if (in) {
+        std::vector<uint8_t> image((std::istreambuf_iterator<char>(in)), std::istreambuf_iterator<char>());
+        return ParamsKZG::read(ctx, image);
+    }
+    ParamsKZG params = ParamsKZG::setup_seeded(ctx, k);
+    const std::vector<uint8_t> image = params.write(SerdeFormat::Processed);
+    std::filesystem::create_directories(std::filesystem::path(path).parent_path());
+    std::ofstream out(path, std::ios::binary);
+    out.write(reinterpret_cast<const char*>(image.data()), std::streamsize(image.size()));
+    if (!out) throw Error(H2B_ERR_ARG, "gen_srs: cannot write " + path);
+    return params;
+}
 
 // EvaluationDomain::new(j, k): j = cs.degree(); quotient_poly_degree = j - 1; extended_k = least e >= k with
 // 2^e >= n * (j - 1) (SURVEY.md Appendix B).
