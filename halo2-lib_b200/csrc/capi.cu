@@ -1510,10 +1510,11 @@ int h2b_poly_lincomb(h2b_ctx* ctx, const uint64_t* const* polys, const uint64_t*
 // ------------------------------------------------------------------------------------------------ test hook
 int h2b_test_field_op(h2b_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out) {
     return guarded(ctx, [&] {
-        H2B_REQUIRE(a && out && (b || (op > 2 && op < 7) || op == 9) && (field == 0 || field == 1) && op >= 0 && op <= 9, "field_op: bad argument");
+        H2B_REQUIRE(a && out && (b || (op > 2 && op < 7) || op == 9) && (field == 0 || field == 1) && op >= 0 && op <= 10, "field_op: bad argument");
         if (n == 0) return;
-        Staging st(ctx, WS_ASSIGN_IN, 3 * n * 32);
-        void *d_a = st.up(a, n * 32), *d_b = st.up(b, b ? n * 32 : 0, n * 32), *d_out = st.out(out, n * 32);
+        const size_t in = (op == 10 ? 2 : 1) * n * 32;  // op 10 reads two operand pairs per output
+        Staging st(ctx, WS_ASSIGN_IN, 2 * in + n * 32);
+        void *d_a = st.up(a, in), *d_b = st.up(b, b ? in : 0, in), *d_out = st.out(out, n * 32);
         field_op_run(ctx, field, op, d_a, d_b, n, d_out);
         st.finish();
     });

@@ -748,7 +748,7 @@ __global__ void __launch_bounds__(128) k_field_op(int op, const uint64_t* __rest
     u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     F x = F::load(a + 4 * (size_t)i), y = F::zero(), r;
-    if (op <= 2 || op == 7 || op == 8) y = F::load(b + 4 * (size_t)i);
+    if (op <= 2 || op == 7 || op == 8 || op == 10) y = F::load(b + 4 * (size_t)i);
     switch (op) {
         case 0: r = x * y; break;
         case 1: r = x + y; break;
@@ -759,6 +759,9 @@ __global__ void __launch_bounds__(128) k_field_op(int op, const uint64_t* __rest
         case 7: r = F::mul_add_mul(x, y, x + y, x - y); break;  // a*b + (a+b)(a-b)
         case 8: r = F::mul_sub_mul(x, y, y, y); break;          // a*b - b*b
         case 9: r = x.inv_bgcd(); break;
+        case 10:  // a*b + c*d on four independent operands: the second pair sits n elements further on
+            r = F::mul_add_mul(x, y, F::load(a + 4 * ((size_t)n + i)), F::load(b + 4 * ((size_t)n + i)));
+            break;
         default: r = x.to_mont(); break;
     }
     r.store(out + 4 * (size_t)i);

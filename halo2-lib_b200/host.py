@@ -127,10 +127,16 @@ class Context:
         return out
 
     def field_op(self, field: int, op: int, a, b=None) -> np.ndarray:
+        """element-wise test hook h2b_test_field_op; op 10 takes 2n rows in `a` and `b` ((a_i, b_i) then (a_{n+i}, b_{n+i}))
+        and returns n rows"""
         a = _u64(a, 4)
         bb = _u64(b, 4) if b is not None else None
-        out = np.empty_like(a)
-        self.check(lib.h2b_test_field_op(self.h, field, op, _ptr(a), _ptr(bb), len(a), _ptr(out)))
+        n = len(a)
+        if op == 10:
+            assert n % 2 == 0 and (bb is None or len(bb) == n), "field_op 10: a and b hold 2n rows each"
+            n //= 2
+        out = np.empty((n, 4), dtype=np.uint64)
+        self.check(lib.h2b_test_field_op(self.h, field, op, _ptr(a), _ptr(bb), n, _ptr(out)))
         return out
 
     def batch_invert(self, a) -> np.ndarray:

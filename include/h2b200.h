@@ -541,7 +541,9 @@ int h2b_eval_polynomial_batch_dev(h2b_ctx* ctx, const void* const* d_polys, cons
 /* ---- test hooks (field arithmetic of the kernels, element-wise on the device) --------------------- */
 /* field: 0 = Fq, 1 = Fr; op: 0 mul, 1 add, 2 sub, 3 inv(a), 4 from_mont(a), 5 to_mont(a), 6 sqr(a),
  * 7 a*b + (a+b)(a-b) and 8 a*b - b*b through the fused two-product Montgomery routine of the group law,
- * 9 inv(a) by the binary extended Euclidean routine the single-lane inversions use */
+ * 9 inv(a) by the binary extended Euclidean routine the single-lane inversions use,
+ * 10 a[i]*b[i] + a[n+i]*b[n+i] through the fused two-product routine with four independent operands (a and b then hold
+ * 2n elements each, out n) */
 int h2b_test_field_op(h2b_ctx* ctx, int field, int op, const uint64_t* a, const uint64_t* b, size_t n, uint64_t* out);
 
 #ifdef __cplusplus

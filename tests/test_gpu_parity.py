@@ -50,8 +50,8 @@ def test_field_ops(ctx, h2b, which, m):
     assert np.array_equal(ctx.field_op(which, 5, ints_to_limbs(a)), A)
     assert np.array_equal(ctx.field_op(which, 3, A[:300]), orc.f_inv(which, A[:300]))
     assert np.array_equal(ctx.field_op(which, 9, A[:600]), orc.f_inv(which, A[:600]))  # binary-Euclid inversion (single-lane paths)
-    with pytest.raises(h2b.H2BError):  # the ops end at 9
-        ctx.field_op(which, 10, A[:3000])
+    with pytest.raises(h2b.H2BError):  # the ops end at 10
+        ctx.field_op(which, 11, A[:3000])
     # products of edge x edge (carry patterns)
     ea = [x for x in edge for _ in edge]
     eb = [y for _ in edge for y in edge]
