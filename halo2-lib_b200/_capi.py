@@ -144,6 +144,7 @@ SIGNATURES = {
     "h2b_check_constants_dev": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp, _vp]),
     "h2b_count_distinct_dev": (_int, [_vp, _vp, _sz, _vp]),
     "h2b_keygen_copies_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "h2b_keygen_instance_edges_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _sz, _sz, _vp, _vp, _vp, _vp]),
     "h2b_keygen_sigma_map_dev": (_int, [_vp, _vp, _sz, _sz, _u32, _vp]),
     "h2b_keygen_sigma_values_dev": (_int, [_vp, _vp, _sz, _u32, _vp]),
     "h2b_divide_by_vanishing_poly": (_int, [_vp, _vp, _u32, _u32]),
@@ -177,6 +178,7 @@ class Witness(C.Structure):
         ("cells", _vp), ("n_cells", _sz), ("break_points", _vp), ("n_break_points", _sz),
         ("lookup_cells", _vp), ("lookup_index", _vp), ("n_lookup", _sz),
         ("rational_index", _vp), ("rational_den", _vp), ("n_rational", _sz),
+        ("instance", _vp), ("n_instance", _vp), ("n_instance_columns", _sz),
     ]
 
 
@@ -186,6 +188,7 @@ class BuilderView(C.Structure):
         ("cells", _vp), ("n_cells", _sz), ("rational_index", _vp), ("rational_den", _vp), ("n_rational", _sz),
         ("selectors", _vp), ("advice_equalities", _vp), ("n_advice_equalities", _sz),
         ("constants", _vp), ("constant_index", _vp), ("n_constant_equalities", _sz), ("lookup_index", _vp), ("n_lookup", _sz),
+        ("instance_index", _vp), ("instance_values", _vp), ("n_instance", _vp), ("n_instance_columns", _sz),
     ]
 
 
@@ -197,7 +200,7 @@ _witp = C.POINTER(Witness)
 _u64s = C.POINTER(C.c_uint64)
 
 PROVER_SIGNATURES = {
-    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp)]),
+    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, _sz, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp)]),
     "h2bp_circuit_free": (None, [_vp]),
     "h2bp_circuit_info": (_int, [_vp, _u64s, C.c_char_p, _sz]),
     "h2bp_circuit_column": (_int, [_vp, C.c_char_p, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
@@ -208,7 +211,7 @@ PROVER_SIGNATURES = {
     "h2bp_session_shard": (_int, [_vp, _sz, _sz, ALLREDUCE_FN, _vp]),
     "h2bp_prove": (_int, [_vp, _witp, _vp, BLIND_FN, _vp, COMMIT_FN, _vp, _vp, _vp, _vp, _vp]),
     "h2bp_check": (_int, [_vp, _witp, _sz, _vp]),
-    "h2bp_mock_create": (_int, [_vp, _u32, _sz, _sz, _int, _u32, _sz, C.POINTER(_vp), _u64s]),
+    "h2bp_mock_create": (_int, [_vp, _u32, _sz, _sz, _int, _u32, _sz, _sz, C.POINTER(_vp), _u64s]),
     "h2bp_mock_free": (None, [_vp]),
     "h2bp_mock_column": (_int, [_vp, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
     "h2bp_mock_run": (_int, [_vp, C.POINTER(BuilderView), _sz, _vp, _u64s, _vp, _vp]),

@@ -1435,6 +1435,17 @@ int h2b_keygen_copies_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, 
                           (const uint64_t*)d_const_index, Mc, d_c, d_edges, d_status);
     });
 }
+int h2b_keygen_instance_edges_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
+                                  size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges, uint32_t* d_status) {
+    return guarded(ctx, [&] {
+        size_t total = 0;
+        for (size_t m = 0; m < I && n_index; m++) total += n_index[m];
+        H2B_REQUIRE((break_points || nbp == 0) && (n_index || I == 0) && (d_index || total == 0) && (d_edges || total == 0) &&
+                        (d_status || I == 0),
+                    "keygen_instance_edges: null pointer");
+        keygen_instance_edges_run(ctx, N, break_points, nbp, k, A, L, usable, I, n_index, (const uint64_t*)d_index, d_edges, d_status);
+    });
+}
 int h2b_keygen_sigma_map_dev(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map) {
     return guarded(ctx, [&] {
         H2B_REQUIRE((d_edges || E == 0) && d_map, "keygen_sigma_map: null pointer");

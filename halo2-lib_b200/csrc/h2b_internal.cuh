@@ -275,6 +275,8 @@ void domain_power_tables(h2b_ctx* ctx, uint32_t k, const void** lo, const void**
 void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, const uint64_t* d_lookup_index,
                        size_t n_lookup, const uint64_t* d_pairs, size_t M, const void* d_consts, const uint64_t* d_const_index, size_t Mc,
                        void* d_c, void* d_edges, uint32_t* status);
+void keygen_instance_edges_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, size_t usable,
+                               size_t I, const size_t* n_index, const uint64_t* d_index, void* d_edges, uint32_t* status);
 void keygen_sigma_map_run(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map);
 void keygen_sigma_values_run(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma);
 // ---- check.cu (MockProver::verify's checks; reports of max_report + 1 words per item, see include/h2b200.h)

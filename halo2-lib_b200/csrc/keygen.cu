@@ -6,8 +6,9 @@
 // two classes when they were made, in call order:  sigma = t_1 o t_2 o .. o t_F.  Those copies are the spanning forest
 // Kruskal builds with weight = call index (unique: the weights are distinct), found here by Borůvka; sigma(x) is the walk
 // from x that keeps crossing the largest forest edge below the last one crossed (t_F is applied first).
-//   copies:  u32 cell-id pairs (c n + r, permutation column c in [c, a0.., l0..] order) in call order: break copies, lookup
-//            copies, advice equalities sorted by (a, b), constant equalities sorted by (constant, cell);
+//   copies:  u32 cell-id pairs (c n + r, permutation column c in [c, a0.., l0.., i0..] order) in call order: break copies,
+//            lookup copies, advice equalities sorted by (a, b), constant equalities sorted by (constant, cell), and then
+//            (assign_instances, after the region) the instance copies column by column;
 //   forest:  hook-and-compress rounds: atomicMin of the incident edge index per component root; a root hooks onto the root
 //            across its edge (of two roots that chose the same edge the lower stays a root); pointer jumping until flat;
 //   walk:    2E darts (vertex, edge) sorted by lookup.cu's radix sort; a dart's successor is the dart before its twin at the
@@ -55,6 +56,26 @@ __device__ __forceinline__ u32 raw_cell(const Layout& y, uint64_t p) {
     }
     const uint64_t s = lo ? __ldg(y.ends + lo - 1) : 0;
     return (1 + lo) * y.n + (u32)(p - s);
+}
+
+// the gate walk's layout: ends[j] = bp_0 + .. + bp_j uploaded to d_ends (nbp + 1 words, stream-ordered)
+static Layout upload_layout(h2b_ctx* ctx, const char* who, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
+                            uint64_t* d_ends) {
+    Layout y;
+    y.nbp = (u32)nbp;
+    y.n = (u32)1 << k;
+    y.A = (u32)A;
+    y.L = (u32)L;
+    y.N = N;
+    y.ends = d_ends;
+    std::vector<uint64_t> ends(nbp + 1, 0);
+    for (size_t j = 0, acc = 0; j < nbp; j++) {
+        H2B_REQUIRE(break_points[j] < y.n, std::string(who) + ": a break point is >= 2^k");
+        acc += break_points[j];
+        ends[j] = acc;
+    }
+    H2B_CUDA(cudaMemcpyAsync(d_ends, ends.data(), 8 * (nbp + 1), cudaMemcpyHostToDevice, ctx->stream));
+    return y;
 }
 
 // lookup copy i: raw(index[i]) ~ (l_{i mod L}, i / L); an index >= N sets bit 0 of *status
@@ -141,12 +162,6 @@ void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, siz
     H2B_REQUIRE(N < ((size_t)1 << 32) && n_lookup < ((size_t)1 << 31) && M < ((size_t)1 << 31) && Mc < ((size_t)1 << 31),
                 "keygen_copies: at most 2^32 - 1 cells and 2^31 - 1 copies of each kind");
     H2B_REQUIRE(L || n_lookup == 0, "keygen_copies: lookup copies need lookup-advice columns");
-    Layout y;
-    y.nbp = (u32)nbp;
-    y.n = (u32)n;
-    y.A = (u32)A;
-    y.L = (u32)L;
-    y.N = N;
     const u32 m = (u32)std::max(M, Mc);
     const int ctas = sort_column_ctas(ctx, std::max<u32>(m, 1));
     // scratch: ends | keys (32 m) | second keys (32 m) | order (4 m) | order2 (4 m) | heads (4 m) | rows (4 m) | sort | scan
@@ -154,20 +169,15 @@ void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, siz
                  o_ord2 = o_ord + al(4 * (size_t)m), o_heads = o_ord2 + al(4 * (size_t)m), o_rows = o_heads + al(4 * (size_t)m),
                  o_sort = o_rows + al(4 * (size_t)m), o_scan = o_sort + al(sort_keys_scratch(m, ctas));
     Scratch s(o_scan + al(exclusive_scan_scratch(m)));
-    std::vector<uint64_t> ends(nbp + 1, 0);
+    const Layout y = upload_layout(ctx, "keygen_copies", N, break_points, nbp, k, A, L, s.at<uint64_t>(0));
     std::vector<uint32_t> brk(2 * nbp);
-    for (size_t j = 0, acc = 0; j < nbp; j++) {
-        acc += break_points[j];
-        ends[j] = acc;
+    for (size_t j = 0; j < nbp; j++) {
         brk[2 * j] = (u32)((2 + j) * n);                      // (a_{j+1}, 0)
         brk[2 * j + 1] = (u32)((1 + j) * n + break_points[j]);  // (a_j, bp_j)
-        H2B_REQUIRE(break_points[j] < n, "keygen_copies: a break point is >= 2^k");
     }
-    y.ends = s.at<uint64_t>(0);
     uint2* edges = (uint2*)d_edges;
     H2B_CUDA(cudaMemsetAsync(status, 0, 8, ctx->stream));
     H2B_CUDA(cudaMemsetAsync(d_c, 0, 32 * n, ctx->stream));
-    H2B_CUDA(cudaMemcpyAsync(s.p, ends.data(), 8 * (nbp + 1), cudaMemcpyHostToDevice, ctx->stream));
     if (nbp) H2B_CUDA(cudaMemcpyAsync(edges, brk.data(), 8 * nbp, cudaMemcpyHostToDevice, ctx->stream));
     edges += nbp;
     if (n_lookup) H2B_LAUNCH(ctx, k_kg_lookup_edges, ceil_div(n_lookup, 256), 256, 0, y, d_lookup_index, (u32)n_lookup, edges, status);
@@ -196,6 +206,42 @@ void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, siz
         u32* last = status + 1;
         H2B_CUDA(cudaMemcpyAsync(last, rows + Mc - 1, 4, cudaMemcpyDeviceToDevice, ctx->stream));
         H2B_LAUNCH(ctx, k_kg_add_word, 1, 1, 0, (const u32*)(heads + Mc - 1), last);
+    }
+    H2B_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+// instance copy r of column `col` (assign_instances): raw(index[r]) ~ (i_col, r).  *status (this column's word): bit 0 an index
+// >= N at a row <= usable (halo2-base's expect runs before the copy of the same row), bit 1 a row >= usable (Assembly::copy
+// fails there); such copies are written as the no-op (0, 0)
+__global__ void __launch_bounds__(256) k_kg_instance_edges(Layout y, const uint64_t* __restrict__ index, u32 m, u32 col, u32 usable,
+                                                           uint2* __restrict__ edges, u32* __restrict__ status) {
+    const u32 r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= m) return;
+    const uint64_t p = __ldg(index + r);
+    if (p >= y.N && r <= usable) atomicOr(status, 1u);
+    if (r >= usable) atomicOr(status, 2u);
+    const bool ok = p < y.N && r < usable;
+    edges[r] = ok ? make_uint2(raw_cell(y, p), (1 + y.A + y.L + col) * y.n + r) : make_uint2(0, 0);
+}
+
+void keygen_instance_edges_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, size_t usable,
+                               size_t I, const size_t* n_index, const uint64_t* d_index, void* d_edges, uint32_t* status) {
+    H2B_REQUIRE(k >= 3 && k <= 28, "keygen_instance_edges: k out of range (3..28)");
+    const size_t n = (size_t)1 << k;
+    H2B_REQUIRE(A >= 1 && nbp < A && usable <= n, "keygen_instance_edges: need A >= 1 gate columns, fewer break points and usable <= 2^k");
+    H2B_REQUIRE((1 + A + L + I) * n < NONE, "keygen_instance_edges: the permutation columns hold more than 2^32 - 1 cells");
+    H2B_REQUIRE(N < ((size_t)1 << 32), "keygen_instance_edges: at most 2^32 - 1 cells");
+    Scratch s(8 * (nbp + 1));
+    const Layout y = upload_layout(ctx, "keygen_instance_edges", N, break_points, nbp, k, A, L, s.at<uint64_t>(0));
+    if (I) H2B_CUDA(cudaMemsetAsync(status, 0, 4 * I, ctx->stream));
+    uint2* edges = (uint2*)d_edges;
+    for (size_t col = 0; col < I; col++) {
+        H2B_REQUIRE(n_index[col] < ((size_t)1 << 31), "keygen_instance_edges: at most 2^31 - 1 cells per instance column");
+        if (n_index[col])
+            H2B_LAUNCH(ctx, k_kg_instance_edges, ceil_div(n_index[col], 256), 256, 0, y, d_index, (u32)n_index[col], (u32)col, (u32)usable, edges,
+                       status + col);
+        d_index += n_index[col];
+        edges += n_index[col];
     }
     H2B_CUDA(cudaStreamSynchronize(ctx->stream));
 }

@@ -32,8 +32,8 @@ struct BoundCircuit {
 struct BoundMock {
     Context ctx;
     MockProver mock;
-    BoundMock(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, uint32_t lookup_bits, size_t max_rows)
-        : ctx(c), mock(ctx, k, A, L, sel, lookup_bits, max_rows) {}
+    BoundMock(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, uint32_t lookup_bits, size_t max_rows, size_t I)
+        : ctx(c), mock(ctx, k, A, L, sel, lookup_bits, max_rows, I) {}
 };
 struct BoundSession {
     Context ctx;
@@ -106,8 +106,8 @@ typedef int (*h2bp_commit_fn)(void* user, int basis, const uint64_t* rows, size_
 
 #define H2BP_API extern "C" __attribute__((visibility("default")))
 
-// fixed: n_fixed named columns (at least the circuit's fixed_names), sigma: one per permutation column; 2^k rows each
-H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, const char* const* fixed_names,
+// fixed: n_fixed named columns (at least the circuit's fixed_names), sigma: one per permutation column; 2^k rows each; I instance columns
+H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, size_t I, const char* const* fixed_names,
                                  const uint64_t* const* fixed, size_t n_fixed, const uint64_t* const* sigma, size_t n_sigma,
                                  BoundCircuit** out) {
     return run(ctx, [&] {
@@ -117,7 +117,7 @@ H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, i
         std::vector<const Fr*> s;
         for (size_t i = 0; i < n_sigma; i++) s.push_back(reinterpret_cast<const Fr*>(sigma[i]));
         auto b = std::make_unique<BoundCircuit>(ctx);
-        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s);
+        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s, I);
         *out = b.release();
     });
 }
@@ -202,8 +202,8 @@ H2BP_API int h2bp_prove(BoundSession* b, const WitnessView* w, const uint64_t* r
     });
 }
 
-// the constraint check.  report: max_report + 1 words per gate column, lookup and permutation column (in that order): the
-// failure count, then the first min(count, max_report) failing rows ascending
+// the constraint check.  report: max_report + 1 words per gate column, lookup and permutation column (in that order, instance
+// columns last): the failure count, then the first min(count, max_report) failing rows ascending
 H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report, uint64_t* report) {
     return run(b ? b->ctx.raw() : nullptr, [&] {
         if (!w || !report) throw Error(H2B_ERR_ARG, "check: null argument");
@@ -214,12 +214,13 @@ H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report
     });
 }
 
-// MockProver of a builder (include/h2b200_mock.hpp).  n_lookups: the number of lookup reports (L, 1 for the selector lookup, or 0)
-H2BP_API int h2bp_mock_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits, size_t max_rows,
+// MockProver of a builder (include/h2b200_mock.hpp), I instance columns.  n_lookups: the number of lookup reports (L, 1 for the
+// selector lookup, or 0)
+H2BP_API int h2bp_mock_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits, size_t max_rows, size_t I,
                               BoundMock** out, uint64_t* n_lookups) {
     return run(ctx, [&] {
         if (!out || !n_lookups) throw Error(H2B_ERR_ARG, "mock_create: null argument");
-        *out = new BoundMock(ctx, k, A, L, selector_lookup != 0, lookup_bits, max_rows);
+        *out = new BoundMock(ctx, k, A, L, selector_lookup != 0, lookup_bits, max_rows, I);
         *n_lookups = (*out)->mock.n_lookups;
     });
 }
@@ -229,8 +230,9 @@ H2BP_API int h2bp_mock_column(BoundMock* b, const char* name, h2b_poly** poly, s
 }
 
 // one run.  break_points: A - 1 words (the count in *n_break_points); report: max_report + 1 words per gate column, lookup, then
-// the advice equalities and the constant equalities (as h2bp_check); cells: max_report x (column, row, column, row) of the
-// reported advice equalities, then max_report x (column, row) of the reported constant equalities
+// the advice equalities, the constant equalities and each instance column (as h2bp_check); cells: max_report x (column, row,
+// column, row) of the reported advice equalities, then max_report x (column, row) of the reported constant equalities, then
+// the same for the reported rows of each instance column
 H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report, uint64_t* break_points, uint64_t* n_break_points,
                            uint64_t* report, uint64_t* cells) {
     return run(b ? b->ctx.raw() : nullptr, [&] {
@@ -241,8 +243,9 @@ H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report
         uint64_t* p = report;
         for (auto* part : {&r.gates, &r.lookups})
             for (auto& e : *part) p = write_report(p, e, max_report);
-        write_report(write_report(p, r.equalities, max_report), r.constants, max_report);
-        std::fill(cells, cells + 6 * max_report, 0);
+        p = write_report(write_report(p, r.equalities, max_report), r.constants, max_report);
+        for (auto& e : r.instances) p = write_report(p, e, max_report);
+        std::fill(cells, cells + (6 + 2 * r.instances.size()) * max_report, 0);
         for (size_t i = 0; i < r.equality_cells.size(); i++) {
             const auto& [x, y] = r.equality_cells[i];
             const uint64_t w[4] = {x.column, x.row, y.column, y.row};
@@ -252,12 +255,17 @@ H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report
             cells[4 * max_report + 2 * i] = r.constant_cells[i].column;
             cells[4 * max_report + 2 * i + 1] = r.constant_cells[i].row;
         }
+        for (size_t m = 0; m < r.instance_cells.size(); m++)
+            for (size_t i = 0; i < r.instance_cells[m].size(); i++) {
+                cells[(6 + 2 * m) * max_report + 2 * i] = r.instance_cells[m][i].column;
+                cells[(6 + 2 * m) * max_report + 2 * i + 1] = r.instance_cells[m][i].row;
+            }
     });
 }
 
 // keygen of a builder (include/h2b200_keygen.hpp).  Out: the circuit (freed with h2bp_circuit_free); break_points (A - 1 words,
 // the count in *n_break_points); vk: 12 limbs per commitment, the fixed columns in the circuit's fixed_names order, then the sigma
-// columns; times: the five phases of KeygenTimes in ms (may be null)
+// columns (1 + A + L + v->n_instance_columns); times: the five phases of KeygenTimes in ms (may be null)
 H2BP_API int h2bp_keygen(h2b_ctx* ctx, h2b_srs* srs, uint32_t k, size_t srs_count, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits,
                          size_t max_rows, const BuilderView* v, BoundCircuit** out, uint64_t* break_points, uint64_t* n_break_points, uint64_t* vk,
                          double* times) {

@@ -137,12 +137,13 @@ class Circuit:
       A gate-advice columns a0..a{A-1}, each with its selector q{j} and the vertical gate (flex_gate/mod.rs:80-91);
       L lookup-advice columns l0..l{L-1}, each looked up in `table` as it is (range/mod.rs:131-150); with L = 0 the one
       lookup is `q_lookup * a0 in table` (range/mod.rs:92-94), or none at all with selector_lookup = False;
-      one constants column c; equality on [c, a0.., l0..] in that order (the permutation's column order).
+      one constants column c; I instance columns i0..i{I-1} (BaseConfig::configure, gates/circuit/mod.rs:87-93);
+      equality on [c, a0.., l0.., i0..] in that order (the permutation's column order).
     The shape numbers and column names are read from the compiled circuit.  `lagr`, `coeff`, `ext` (by column name) and
     `sigma_map` (the decoded sigma of the check) look up its device columns."""
 
     def __init__(self, ctx: Context, k: int, fixed_lagrange: dict, sigma_lagrange: list, A: int = 1, L: int = 0,
-                 selector_lookup: bool = True):
+                 selector_lookup: bool = True, I: int = 0):
         n = 1 << k
         fixed = {nm: _rows(a, n, nm) for nm, a in fixed_lagrange.items()}
         sigma = [_rows(a, n, "sigma %d" % i) for i, a in enumerate(sigma_lagrange)]
@@ -150,7 +151,7 @@ class Circuit:
         ptrs = (C.c_void_p * len(fixed))(*[a.ctypes.data for a in fixed.values()])
         sptrs = (C.c_void_p * len(sigma))(*[a.ctypes.data for a in sigma])
         h = C.c_void_p()
-        ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h)))
+        ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), I, names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h)))
         self._bind(ctx, k, A, L, h)
 
     def _bind(self, ctx: Context, k: int, A: int, L: int, h: C.c_void_p):
@@ -163,6 +164,7 @@ class Circuit:
         self.selector_lookup = bool(sel)
         lists = {key: v.split(",") for key, v in (line.split("=", 1) for line in text.value.decode().split("\n"))}
         self.adv_names, self.perm_cols, self.fixed_names, self.sigma_names = (lists[key] for key in ("adv", "perm", "fixed", "sigma"))
+        self.I = len(self.perm_cols) - 1 - A - L
         self.lagr, self.coeff, self.ext = _Columns(self, "lagr"), _Columns(self, "coeff"), _Columns(self, "ext")
 
     def column(self, table: str, name: str = "") -> Column:
@@ -290,9 +292,22 @@ def _reports(words: np.ndarray, max_report: int) -> list:
     return [(int(r[0]), [int(x) for x in r[1:1 + min(int(r[0]), max_report)]]) for r in words]
 
 
+def _instance_columns(who: str, I: int, columns, width: int):
+    """(pointer array, length array, the arrays) of I instance columns: `columns` a list of I arrays (uint64 indices, width 1, or
+    Montgomery values, width 4); None: every column empty"""
+    cols = [()] * I if columns is None else list(columns)
+    if len(cols) != I:
+        raise ValueError("%s: %d instance columns for a circuit with %d" % (who, len(cols), I))
+    arrs = [np.ascontiguousarray(c, dtype=np.uint64).reshape(-1, width) for c in cols]
+    ptrs = (C.c_void_p * max(I, 1))(*[a.ctypes.data if a.size else None for a in arrs])
+    lens = (C.c_size_t * max(I, 1))(*[len(a) for a in arrs])
+    return ptrs, lens, arrs
+
+
 def _builder_view(who: str, n_cells: int, selectors, advice_equalities, constant_equalities, lookups, cells=None, rational_index=None,
-                  rational_den=None):
-    """(BuilderView, the arrays it points to) of a builder in MockProver's form"""
+                  rational_den=None, I: int = 0, instances=None, public=None):
+    """(BuilderView, the arrays it points to) of a builder in MockProver's form; instances: per instance column the indices of
+    its cells, public: per instance column its values (MockProver)"""
     u64 = lambda a: np.ascontiguousarray(a, dtype=np.uint64)
     V = u64(np.zeros((0, 4)) if cells is None else cells).reshape(-1, 4)
     S = np.ascontiguousarray(selectors, dtype=np.uint8).reshape(-1)
@@ -310,25 +325,38 @@ def _builder_view(who: str, n_cells: int, selectors, advice_equalities, constant
         raise ValueError(who + ": rational_index and rational_den differ in length")
     p = lambda a: a.ctypes.data if a.size else None
     view = BuilderView(p(V), n_cells, p(RI), p(RD), len(RI), p(S), p(E), len(E), p(Kc), p(Ki), len(Ki), p(LK), len(LK))
-    return view, (V, S, E, Kc, Ki, LK, RI, RD)
+    ip, il, ia = _instance_columns(who, I, instances, 1)
+    keep = (V, S, E, Kc, Ki, LK, RI, RD, ip, il, ia)
+    if I:
+        view.instance_index, view.n_instance, view.n_instance_columns = C.cast(ip, C.c_void_p), C.cast(il, C.c_void_p), I
+        if public is not None:
+            vp, vl, va = _instance_columns(who, I, public, 4)
+            if list(vl)[:I] != list(il)[:I]:
+                raise ValueError(who + ": one public value per instance cell")
+            view.instance_values = C.cast(vp, C.c_void_p)
+            keep += (vp, vl, va)
+    return view, keep
 
 
 def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
-           max_rows: int | None = None, selectors=(), advice_equalities=(), constant_equalities=None, lookups=(), timings: dict | None = None):
+           max_rows: int | None = None, selectors=(), advice_equalities=(), constant_equalities=None, lookups=(), timings: dict | None = None,
+           I: int = 0, instances=None):
     """keygen_vk + keygen_pk of a halo2-base builder in its keygen form, on the device (h2b::keygen, include/h2b200_keygen.hpp).
 
     The arguments mean what they mean for MockProver.run (selectors: one per cell of the virtual column, which fixes its length;
     no witness values are read).  sigma is the one halo2's permutation Assembly builds from halo2-base's copy calls, bit for bit.
+    I instance columns, `instances` the indices of each one's cells (BaseCircuitBuilder::assigned_instances; None: all empty):
+    their copies follow the region's.
     Returns (circuit, vk, break_points): `circuit` is a Circuit that ProverSession takes; vk = {"fixed": {name: commitment},
     "permutation": [commitment per permutation column, perm_cols order]}, each commitment affine as 12 Montgomery limbs
     (x, y, 1; the identity all zero), of the column's Lagrange values.  halo2-base's panics raise H2BError with its message.
     `timings`, when a dict, receives the milliseconds of the phases copies / forest / sigma / pk / vk."""
     max_rows = (1 << k) - 9 if max_rows is None else max_rows
     n_cells = len(np.asarray(selectors).reshape(-1))
-    view, keep = _builder_view("keygen", n_cells, selectors, advice_equalities, constant_equalities, lookups)
+    view, keep = _builder_view("keygen", n_cells, selectors, advice_equalities, constant_equalities, lookups, I=I, instances=instances)
     bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
     n_fixed = A + (1 if selector_lookup and L == 0 else 0) + (1 if L or selector_lookup else 0) + 1
-    vk = np.zeros((n_fixed + 1 + A + L, 12), dtype=np.uint64)
+    vk = np.zeros((n_fixed + 1 + A + L + I, 12), dtype=np.uint64)
     times = np.zeros(5, dtype=np.float64)
     h = C.c_void_p()
     ctx.check(lib.h2bp_keygen(ctx.h, params.h, k, params.count, A, L, int(selector_lookup), lookup_bits, max_rows, C.byref(view), C.byref(h),
@@ -412,10 +440,9 @@ class ProverSession:
             raise err
         self.ctx.check(rc)
 
-    @staticmethod
-    def _witness(who, witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr, n_rational,
-                 lookup_index_ptr):
-        """(Witness, the break points array it points to)"""
+    def _witness(self, who, witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr, n_rational,
+                 lookup_index_ptr, instances=None):
+        """(Witness, the arrays it points to)"""
         if lookup_ptr and lookup_index_ptr:
             raise ValueError(who + ": pass the looked-up cells either as values (lookup_ptr) or as indices (lookup_index_ptr)")
         if n_rational and not (rational_index_ptr and rational_den_ptr):
@@ -423,20 +450,25 @@ class ProverSession:
         bp = np.ascontiguousarray([] if break_points is None else break_points, dtype=np.uint64).reshape(-1)
         w = Witness(witness_ptr or None, n_cells, bp.ctypes.data if len(bp) else None, len(bp), lookup_ptr or None,
                     lookup_index_ptr or None, n_lookup, rational_index_ptr or None, rational_den_ptr or None, n_rational)
-        return w, bp
+        I = self.cs.I
+        inst = _instance_columns(who, I, instances, 4)
+        if I:
+            w.instance, w.n_instance, w.n_instance_columns = C.cast(inst[0], C.c_void_p), C.cast(inst[1], C.c_void_p), I
+        return w, (bp, inst)
 
     def check(self, witness_ptr: int, n_cells: int, break_points=None, lookup_ptr: int = 0, n_lookup: int = 0, rational_index_ptr: int = 0,
-              rational_den_ptr: int = 0, n_rational: int = 0, lookup_index_ptr: int = 0, max_report: int = 16) -> dict:
+              rational_den_ptr: int = 0, n_rational: int = 0, lookup_index_ptr: int = 0, max_report: int = 16, instances=None) -> dict:
         """MockProver::verify for this circuit: which gates, lookups and copy constraints the witness breaks, and where.
         Takes the witness exactly as `prove` does and runs the same assignment; no blinding, no random polynomial, no transcript.
         The values checked are the ones a proof would commit before blinding, with rows >= u read as 0:
           gates[j]    rows r < u with q{j}(r) (a{j}(r) + a{j}(r+1) a{j}(r+2) - a{j}(r+3)) != 0 (rotations mod n);
           lookups[t]  rows r < u whose input (q_lookup * a0, or l{t}) is not among the table's rows [0, u);
-          copies[c]   rows r < n of permutation column c (perm_cols order) whose value differs from the cell sigma_c(r) names.
+          copies[c]   rows r < n of permutation column c (perm_cols order) whose value differs from the cell sigma_c(r) names;
+                      an instance column holds the public values `instances` (as for `prove`) at rows [0, len), zero after.
         Each entry is (failure count, the first min(count, max_report) failing rows ascending).  Every report comes down in one
         copy.  A bad halo2-base index raises H2BError; so does a sigma entry that names no cell (on the circuit's first check)."""
-        w, bp = self._witness("check", witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr,
-                              n_rational, lookup_index_ptr)
+        w, keep = self._witness("check", witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr,
+                                n_rational, lookup_index_ptr, instances)
         if not 1 <= max_report <= CHECK_MAX_REPORT:
             raise ValueError("check: max_report must be in 1..%d" % CHECK_MAX_REPORT)
         cs = self.cs
@@ -450,7 +482,7 @@ class ProverSession:
 
     def prove(self, witness_ptr: int, n_cells: int, random_poly_ptr: int, seed: int = 0, break_points=None,
               lookup_ptr: int = 0, n_lookup: int = 0, rational_index_ptr: int = 0, rational_den_ptr: int = 0, n_rational: int = 0,
-              lookup_index_ptr: int = 0) -> dict:
+              lookup_index_ptr: int = 0, instances=None) -> dict:
         """witness_ptr: host pointer (pinned) to the n_cells Montgomery Fr cells of the virtual column, `break_points` as
         keygen pinned them; lookup_ptr / n_lookup: the cells to look up (L > 0); random_poly_ptr: n elements.
 
@@ -458,9 +490,13 @@ class ProverSession:
         Rational(n, d) cell, rational_index_ptr / rational_den_ptr the n_rational (uint64 virtual-column index, Montgomery d)
         pairs, indices strictly increasing; lookup_index_ptr (instead of lookup_ptr) the n_lookup uint64 virtual-column
         indices of the looked-up cells in `assign_raw` order.  The device makes of them what batch_invert_assigned and
-        assign_raw make (d = 0 -> 0).  A bad index raises H2BError once phase 0's commitments are down; no proof is returned."""
-        w, bp = self._witness("prove", witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr,
-                              n_rational, lookup_index_ptr)
+        assign_raw make (d = 0 -> 0).  A bad index raises H2BError once phase 0's commitments are down; no proof is returned.
+
+        instances: the public values, one (len_m x 4) Montgomery array per instance column of the circuit (None: all empty); they
+        enter the transcript before the advice commitments, column by column, and fill rows [0, len_m) of the column.  More than
+        u values in a column raise H2BError (InstanceTooLarge)."""
+        w, keep = self._witness("prove", witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr,
+                                n_rational, lookup_index_ptr, instances)
         self._rng = np.random.default_rng(seed)
         cm = np.empty((self.n_commitments, 12), dtype=np.uint64)
         ev = np.empty((len(self.queries), 4), dtype=np.uint64)
@@ -485,14 +521,15 @@ class MockProver:
 
     Shape as `Circuit`: A gate-advice columns, L lookup-advice columns (or the selector lookup when L = 0, or no lookup), one
     constants column, the table 0 .. 2^lookup_bits - 1, and max_rows = 2^k - unusable_rows as calculate_params gets it
-    (at most 2^k - 7; default 2^k - 9, BaseTester's unusable_rows).  `lagr[name]` (a{j}, l{t}, q{j}, q_lookup, table) views the columns of the last run."""
+    (at most 2^k - 7; default 2^k - 9, BaseTester's unusable_rows), and I instance columns.  `lagr[name]` (a{j}, l{t}, q{j},
+    q_lookup, table) views the columns of the last run."""
 
     def __init__(self, ctx: Context, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
-                 max_rows: int | None = None):
-        self.ctx, self.k, self.A, self.L = ctx, k, A, L
+                 max_rows: int | None = None, I: int = 0):
+        self.ctx, self.k, self.A, self.L, self.I = ctx, k, A, L, I
         self.max_rows = (1 << k) - 9 if max_rows is None else max_rows
         h, nl = C.c_void_p(), C.c_uint64()
-        ctx.check(lib.h2bp_mock_create(ctx.h, k, A, L, int(selector_lookup), lookup_bits, self.max_rows, C.byref(h), C.byref(nl)))
+        ctx.check(lib.h2bp_mock_create(ctx.h, k, A, L, int(selector_lookup), lookup_bits, self.max_rows, I, C.byref(h), C.byref(nl)))
         self._h, self.n_lookups = h, int(nl.value)
         self.lagr = _Columns(self, "lagr")
 
@@ -504,7 +541,7 @@ class MockProver:
         return Column(self.ctx, poly, off.value, rows.value)
 
     def run(self, cells, selectors, advice_equalities=(), constant_equalities=None, lookups=(), rational_index=None, rational_den=None,
-            max_report: int = 16) -> dict:
+            max_report: int = 16, instances=None, public=None) -> dict:
         """cells: the virtual column (n x 4 Montgomery limbs), in either witness form (rational_index / rational_den: the
         (uint64 index, Montgomery d) pairs of the Rational cells, indices strictly increasing); selectors: one bool per cell;
         advice_equalities: (a, b) index pairs; constant_equalities: (constants (m x 4 Montgomery limbs), indices); lookups:
@@ -512,26 +549,34 @@ class MockProver:
 
         Returns gates[j], lookups[t] (failing rows < u), equalities and constants (failing equality indices), each as
         (count, the first min(count, max_report) ascending); equality_cells / constant_cells: the raw cells ((column, row)) of
-        every reported equality; break_points; satisfied.  halo2-base's panics raise H2BError with its message."""
+        every reported equality; break_points; satisfied.  halo2-base's panics raise H2BError with its message.
+
+        instances / public: per instance column, the indices of its cells and its public values (Montgomery), one value per cell
+        (None: all empty).  instances[m] reports the rows r whose cell differs from public[m][r], instance_cells[m] their raw
+        cells; more than u values raise H2BError (InstanceTooLarge)."""
         if not 1 <= max_report <= CHECK_MAX_REPORT:
             raise ValueError("MockProver: max_report must be in 1..%d" % CHECK_MAX_REPORT)
         V = np.ascontiguousarray(cells, dtype=np.uint64).reshape(-1, 4)
+        I = self.I
         view, keep = _builder_view("MockProver", len(V), selectors, advice_equalities, constant_equalities, lookups, V, rational_index,
-                                   rational_den)
+                                   rational_den, I, instances, [()] * I if public is None else public)
         A, nl = self.A, self.n_lookups
         bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
-        words = np.empty((A + nl + 2, max_report + 1), dtype=np.uint64)
-        cells_out = np.empty(6 * max_report, dtype=np.uint64)
+        words = np.empty((A + nl + 2 + I, max_report + 1), dtype=np.uint64)
+        cells_out = np.empty((6 + 2 * I) * max_report, dtype=np.uint64)
         self.ctx.check(lib.h2bp_mock_run(self._h, C.byref(view), max_report, C.c_void_p(bps.ctypes.data), C.byref(nbp),
                                          C.c_void_p(words.ctypes.data), C.c_void_p(cells_out.ctypes.data)))
         reports = _reports(words, max_report)
         eq, co = reports[A + nl], reports[A + nl + 1]
         ec = cells_out[:4 * max_report].reshape(-1, 4)
-        cc = cells_out[4 * max_report:].reshape(-1, 2)
+        cc = cells_out[4 * max_report:6 * max_report].reshape(-1, 2)
+        inst = reports[A + nl + 2:]
+        ic = [cells_out[(6 + 2 * m) * max_report:(8 + 2 * m) * max_report].reshape(-1, 2)[:len(inst[m][1])] for m in range(I)]
         return {"gates": reports[:A], "lookups": reports[A:A + nl], "equalities": eq, "constants": co,
                 "equality_cells": [((int(c[0]), int(c[1])), (int(c[2]), int(c[3]))) for c in ec[:len(eq[1])]],
                 "constant_cells": [(int(c[0]), int(c[1])) for c in cc[:len(co[1])]],
-                "break_points": [int(b) for b in bps[:nbp.value]], "satisfied": not any(c for c, _ in reports)}
+                "break_points": [int(b) for b in bps[:nbp.value]], "satisfied": not any(c for c, _ in reports),
+                "instances": inst, "instance_cells": [[(int(c[0]), int(c[1])) for c in x] for x in ic]}
 
     def free(self):
         if self._h:

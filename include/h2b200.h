@@ -467,8 +467,8 @@ int h2b_check_constants_dev(h2b_ctx* ctx, const void* d_cells, size_t N, const v
 int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count);
 
 /* ---- keygen of a halo2-base builder: the permutation side of keygen_vk / keygen_pk (see h2b200_keygen.hpp, DESIGN.md §4.8).
- * Cells are u32 ids c 2^k + r, c the permutation column in [c, a0.., a{A-1}, l0.., l{L-1}] order.  Synchronous; scratch is
- * allocated and freed per call.
+ * Cells are u32 ids c 2^k + r, c the permutation column in [c, a0.., a{A-1}, l0.., l{L-1}, i0.., i{I-1}] order.  Synchronous;
+ * scratch is allocated and freed per call.
  *   h2b_keygen_copies_dev        the constants column and the copy calls of BaseCircuitBuilder::synthesize in halo2-base's order,
  *                                into d_edges (E = nbp + n_lookup + M + Mc u32 pairs): the break copies (a{j+1}, 0) ~ (a_j,
  *                                bp_j) (break_points: host); the lookup copies raw(index[i]) ~ (l{i mod L}, i / L); the M advice
@@ -479,6 +479,13 @@ int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_
  *                                cell belongs to the column it ends).  d_status (2 words): [0] bit 0 a looked-up index >= N, bit 1
  *                                an equality index >= N (nothing read through it); [1] the number of distinct constants (rows of
  *                                d_c >= 2^k are not written).
+ *   h2b_keygen_instance_edges_dev  the copies of BaseCircuitBuilder::assign_instances, which follow the ones above: for each
+ *                                instance column m < I in order and each row r < n_index[m] (host array), raw(index_m[r]) ~
+ *                                (i_m, r), index_m the next n_index[m] uint64 of d_index (the columns back to back), into d_edges
+ *                                (n_index[0] + .. + n_index[I-1] u32 pairs; pass the edges after those of h2b_keygen_copies_dev).
+ *                                d_status (I words, zeroed first): word m bit 0 an index >= N at a row r <= usable (halo2-base's
+ *                                "instance not assigned" comes before that row's copy), bit 1 a row r >= usable (halo2's copy
+ *                                fails with NotEnoughRowsAvailable there); such copies are written as (0, 0), which joins nothing.
  *   h2b_keygen_sigma_map_dev     the mapping halo2's permutation Assembly builds from E copies (d_edges, in call order) over
  *                                n_cols x 2^k cells: d_map (n_cols x 2^k u32) = the cell id each cell maps to (as
  *                                h2b_permutation_decode_dev decodes it).  A cell id >= n_cols 2^k is H2B_ERR_ARG.
@@ -486,6 +493,8 @@ int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_
 int h2b_keygen_copies_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
                           const void* d_lookup_index, size_t n_lookup, const void* d_pairs, size_t M, const void* d_consts,
                           const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status);
+int h2b_keygen_instance_edges_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
+                                  size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges, uint32_t* d_status);
 int h2b_keygen_sigma_map_dev(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map);
 int h2b_keygen_sigma_values_dev(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma);
 

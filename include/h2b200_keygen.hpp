@@ -7,9 +7,12 @@
 //   1. the break copies of assign_with_constraints: (a{j+1}, 0) ~ (a_j, bp_j), j = 0, 1, ..;
 //   2. L > 0: LookupAnyManager::assign_raw's copies raw(lookup_index[i]) ~ (l{i mod L}, i / L), i = 0, 1, ..;
 //   3. CopyConstraintManager::assign_raw: the advice equalities sorted by (a, b), then the constant equalities sorted by
-//      (constant, cell) as (c, the constant's row) ~ raw(cell), the distinct constants at rows 0, 1, .. of c in that order.
+//      (constant, cell) as (c, the constant's row) ~ raw(cell), the distinct constants at rows 0, 1, .. of c in that order;
+//   4. after the region, BaseCircuitBuilder::assign_instances: raw(instance_index_m[r]) ~ (i_m, r) for each instance column m
+//      (b.n_instance_columns of them) in order and r = 0, 1, .. (an index >= N: "instance not assigned"; r >= u: halo2's
+//      NotEnoughRowsAvailable).
 // So the builder's own order of its equalities does not change the keys.  Errors: halo2-base's panics as MockProver raises them.
-// Instance columns and several constants columns are not covered (the same boundary as MockProver).
+// Several constants columns are not covered (the same boundary as MockProver).
 #pragma once
 #include <chrono>
 
@@ -20,7 +23,7 @@ namespace h2b {
 // affine commitments (z = 1; the identity all zero) of the Lagrange columns, as ProverSession commits them
 struct VerifyingKey {
     std::vector<std::pair<std::string, G1>> fixed;  // the circuit's fixed_names order
-    std::vector<G1> permutation;                    // one per permutation column, perm_cols order
+    std::vector<G1> permutation;                    // one per permutation column, perm_cols order (instance columns last)
 };
 
 // milliseconds per phase of one keygen call (each phase ends with the stream synchronised)
@@ -48,12 +51,14 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         if (times) times->*field = std::chrono::duration<double, std::milli>(t - t0).count();
         t0 = t;
     };
-    const CircuitShape s = builder_shape("keygen", k, A, L, selector_lookup, lookup_bits, max_rows);
+    const CircuitShape s = builder_shape("keygen", k, A, L, selector_lookup, lookup_bits, max_rows, b.n_instance_columns);
     const size_t n = s.n, N = b.n_cells, M = b.n_advice_equalities, Mc = b.n_constant_equalities, NL = b.n_lookup;
     h2b_ctx* c = ctx.raw();
     KeygenResult out;
     out.break_points = builder_break_points(s, "keygen", max_rows, b, false);
-    const size_t nbp = out.break_points.size(), npc = s.perm_cols.size(), E = nbp + (L ? NL : 0) + M + Mc;
+    const size_t I = s.I, nbp = out.break_points.size(), npc = s.perm_cols.size(), E0 = nbp + (L ? NL : 0) + M + Mc;
+    size_t E = E0;
+    for (size_t m = 0; m < I; m++) E += b.n_instance[m];
     PolyPtr sel_d, lk_d, eq_d, const_d, const_idx_d;
     upload_bytes(ctx, sel_d, b.selectors, N);
     upload_bytes(ctx, lk_d, b.lookup_index, 8 * NL);
@@ -79,6 +84,23 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
                                     col(nf - 1), edges.at(), st));
     std::memcpy(v, status.download(0, 1)[0].data(), 8);
     builder_panics(s, v[0] & 1, false, v[1], v[0] & 2);
+    if (I) {  // the instance copies, after the region's
+        std::vector<uint64_t> idx;
+        for (size_t m = 0; m < I; m++) idx.insert(idx.end(), b.instance_index[m], b.instance_index[m] + b.n_instance[m]);
+        PolyPtr idx_d;
+        upload_bytes(ctx, idx_d, idx.data(), 8 * idx.size());
+        Poly inst_status(ctx, (I + 7) / 8);
+        ctx.check(h2b_keygen_instance_edges_dev(c, N, bp, nbp, k, A, L, s.u, I, b.n_instance, idx_d->at(), static_cast<char*>(edges.at()) + 8 * E0,
+                                                static_cast<uint32_t*>(inst_status.at())));
+        const std::vector<Fr> w = inst_status.download(0, inst_status.len());
+        const uint32_t* iv = reinterpret_cast<const uint32_t*>(w[0].data());
+        for (size_t m = 0; m < I; m++) {  // the first failing cell in assign_instances' order
+            if (iv[m] & 1) throw Error(H2B_ERR_ARG, "instance not assigned");
+            if (iv[m] & 2)
+                throw Error(H2B_ERR_ARG, "NotEnoughRowsAvailable { current_k: " + std::to_string(k) + " }: instance column i" + std::to_string(m) +
+                                             " has " + std::to_string(b.n_instance[m]) + " cells for its " + std::to_string(s.u) + " usable rows");
+        }
+    }
     lap(&KeygenTimes::copies);
     Poly map(ctx, (npc * n + 7) / 8), sigma(ctx, npc * n);
     ctx.check(h2b_keygen_sigma_map_dev(c, edges.at(), E, npc, k, map.at()));
@@ -89,7 +111,7 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
     for (size_t i = 0; i < nf; i++) fx[s.fixed_names[i]] = col(i);
     std::vector<const Fr*> sg;
     for (size_t i = 0; i < npc; i++) sg.push_back(static_cast<const Fr*>(sigma.at(i * n)));
-    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg);
+    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg, I);
     lap(&KeygenTimes::pk);
     // the vk: every fixed column, then every sigma column, committed in Lagrange form, up to 16 MSMs per batch
     std::vector<const void*> cols;

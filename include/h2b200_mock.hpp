@@ -9,16 +9,19 @@
 //   advice_equalities        the copy manager's (ContextCell, ContextCell) pairs as index pairs;
 //   constant_equalities      its (F, ContextCell) pairs: Montgomery constants + indices;
 //   lookup_index             L > 0: the looked-up cells in assign_raw order; L = 0 with the selector lookup: the cells whose
-//                            raw row gets q_lookup.
+//                            raw row gets q_lookup;
+//   instance_index           per instance column m < n_instance_columns, its assigned_instances as n_instance[m] indices;
+//   instance_values          per instance column (MockProver only), the n_instance[m] public values (Montgomery).
 // MockProver builds what the keygen pass would assign (assign_with_constraints: break points, advice and q_j columns;
 // assign_lookups_in_phase: q_lookup or the lookup-advice columns) and checks, on the device:
 //   gates[j]    rows r < u with q_j(r) (a_j(r) + a_j(r+1) a_j(r+2) - a_j(r+3)) != 0, u = 2^k - 7 (rows >= u read as 0);
 //   lookups[t]  rows r < u whose input (q_lookup * a0, or l_t) is not among the table's values 0 .. 2^lookup_bits - 1;
 //   equalities  advice equalities i with value(a_i) != value(b_i);
-//   constants   constant equalities i with value(cell_i) != c_i.
+//   constants   constant equalities i with value(cell_i) != c_i;
+//   instances[m] rows r of instance column m with value(instance_index_m[r]) != instance_values_m[r].
 // One deliberate difference from halo2's MockProver: a copy failure is counted per violated equality, not per cell against its
-// sigma image; both are zero exactly when every equality holds.  Instance columns and several constants columns are not
-// covered; the lookup-advice copies of assign_raw hold by construction (the columns are filled from the indices).
+// sigma image; both are zero exactly when every equality holds.  Several constants columns are not covered; the lookup-advice
+// copies of assign_raw hold by construction (the columns are filled from the indices).
 #pragma once
 #include <algorithm>
 #include <string>
@@ -41,6 +44,10 @@ struct BuilderView {
     size_t n_constant_equalities = 0;
     const uint64_t* lookup_index = nullptr;
     size_t n_lookup = 0;
+    const uint64_t* const* instance_index = nullptr;
+    const Fr* const* instance_values = nullptr;
+    const size_t* n_instance = nullptr;
+    size_t n_instance_columns = 0;
 };
 
 // a cell of the assignment: gate-advice column and row
@@ -56,14 +63,17 @@ struct MockReport {
     ReportItem equalities, constants;
     std::vector<std::pair<RawCell, RawCell>> equality_cells;  // both raw cells of every reported advice equality
     std::vector<RawCell> constant_cells;                      // the raw advice cell of every reported constant equality
+    std::vector<ReportItem> instances;                        // per instance column: the failing rows
+    std::vector<std::vector<RawCell>> instance_cells;         // per instance column: the raw advice cell of every reported row
 };
 
 // ------------------------------------------------------------------------------------------------ what MockProver and keygen share
 // the shape of a builder, checked; messages start with `who`.  max_rows = 2^k - unusable_rows, as calculate_params gets it; it
 // must leave the blinding rows alone (<= 2^k - 7)
-inline CircuitShape builder_shape(const std::string& who, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows) {
+inline CircuitShape builder_shape(const std::string& who, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows,
+                                  size_t I = 0) {
     if (k < 3 || k > 28) throw Error(H2B_ERR_ARG, who + ": k out of range (3..28)");
-    CircuitShape s(k, A, L, selector_lookup);
+    CircuitShape s(k, A, L, selector_lookup, I);
     if (A < 1) throw Error(H2B_ERR_ARG, who + ": no gate columns");
     if (s.selector_lookup && A != 1) throw Error(H2B_ERR_ARG, who + ": the selector lookup needs exactly one gate column");
     if (max_rows < 1 || max_rows > s.u) throw Error(H2B_ERR_ARG, who + ": max_rows must be in 1..2^k - 7");
@@ -112,6 +122,8 @@ inline std::vector<uint64_t> builder_break_points(const CircuitShape& s, const s
     if ((b.n_cells && !(b.selectors && (b.cells || !values))) || (values && b.n_rational && !(b.rational_index && b.rational_den)) ||
         (b.n_advice_equalities && !b.advice_equalities) || (b.n_constant_equalities && !(b.constants && b.constant_index)) || (b.n_lookup && !b.lookup_index))
         throw Error(H2B_ERR_ARG, who + ": a count > 0 needs its array");
+    check_instances(who, s, b.instance_index, b.n_instance, b.n_instance_columns, values);  // keygen: the copies find rows >= u
+    if (values) check_instances(who, s, b.instance_values, b.n_instance, b.n_instance_columns);
     std::vector<uint64_t> bps = break_points_of(b.selectors, b.n_cells, s.A, max_rows);
     if (b.n_lookup) {
         if (s.L && (b.n_lookup + s.L - 1) / s.L > max_rows) throw Error(H2B_ERR_ARG, "range lookups would be assigned to unusable rows");
@@ -134,8 +146,8 @@ inline void builder_panics(const CircuitShape& s, bool lookup_unassigned, bool u
 class MockProver : public CircuitShape {
 public:
     // max_rows as for builder_shape
-    MockProver(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows)
-        : CircuitShape(builder_shape("MockProver", k, A, L, selector_lookup, lookup_bits, max_rows)), ctx(ctx), lookup_bits(lookup_bits),
+    MockProver(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows, size_t I = 0)
+        : CircuitShape(builder_shape("MockProver", k, A, L, selector_lookup, lookup_bits, max_rows, I)), ctx(ctx), lookup_bits(lookup_bits),
           max_rows(max_rows) {
         adv = std::make_unique<Poly>(ctx, n * (A + L));
         q = std::make_unique<Poly>(ctx, n * A);
@@ -166,8 +178,9 @@ public:
         if (max_report < 1 || max_report > H2B_CHECK_MAX_REPORT) throw Error(H2B_ERR_ARG, "MockProver: max_report out of range");
         MockReport out;
         out.break_points = builder_break_points(*this, "MockProver", max_rows, b, true);
-        // element 0 of the report block: the verdict words (rational, lookup index, q_lookup, advice eq, constant eq, distinct)
-        const size_t W = max_report + 1, n_items = A + n_lookups + 2, elems = 1 + (n_items * W + 3) / 4;
+        // element 0 of the report block: the verdict words (rational, lookup index, q_lookup, advice eq, constant eq, distinct);
+        // then the reports (gates, lookups, equalities, constants, instances); then one status word per instance column
+        const size_t W = max_report + 1, n_items = A + n_lookups + 2 + I, rep_elems = 1 + (n_items * W + 3) / 4, elems = rep_elems + (I + 7) / 8;
         Poly* rep = grown(ctx, rep_, elems);
         const Fr zero{};
         rep->upload(&zero, 1);
@@ -201,6 +214,14 @@ public:
         upload_bytes(ctx, const_idx_, b.constant_index, 8 * Mc);
         ctx.check(h2b_check_constants_dev(c, cells, N, const_->at(), const_idx_->at(), Mc, max_report, at(A + n_lookups + 1), verdict + 4));
         ctx.check(h2b_count_distinct_dev(c, const_->at(), Mc, verdict + 5));
+        // the instance copies of assign_instances, as the constant check: cell instance_index_m[r] against public value r
+        inst_.resize(2 * I);
+        for (size_t m = 0; m < I; m++) {
+            upload_bytes(ctx, inst_[2 * m], b.instance_values[m], 32 * b.n_instance[m]);
+            upload_bytes(ctx, inst_[2 * m + 1], b.instance_index[m], 8 * b.n_instance[m]);
+            ctx.check(h2b_check_constants_dev(c, cells, N, inst_[2 * m]->at(), inst_[2 * m + 1]->at(), b.n_instance[m], max_report,
+                                              at(A + n_lookups + 2 + m), static_cast<uint32_t*>(rep->at(rep_elems)) + m));
+        }
         for (size_t j = 0; j < A; j++) {
             const BoundGraph g(ev, gate, {q->at(j * n)}, {adv->at(j * n)});
             ctx.check(h2b_check_graph_dev(c, g.get(), k, u, max_report, at(j)));
@@ -212,6 +233,9 @@ public:
         if (v[0] & 1) throw Error(H2B_ERR_ARG, "MockProver: a Rational index is >= the witness length");
         if (v[0] & 2) throw Error(H2B_ERR_ARG, "MockProver: the Rational indices do not strictly increase");
         builder_panics(*this, (v[1] | v[2]) & 1, v[2] & 2, v[5], (v[3] | v[4]) & 1);
+        const uint32_t* inst_status = reinterpret_cast<const uint32_t*>(raw[rep_elems].data());
+        for (size_t m = 0; m < I; m++)
+            if (inst_status[m] & 1) throw Error(H2B_ERR_ARG, "instance not assigned");
         const std::vector<ReportItem> items = decode_reports(raw[1].data(), n_items, max_report, out.satisfied);
         out.gates.assign(items.begin(), items.begin() + A);
         out.lookups.assign(items.begin() + A, items.begin() + A + n_lookups);
@@ -220,6 +244,11 @@ public:
         for (uint64_t i : out.equalities.second)
             out.equality_cells.push_back({raw_cell(out.break_points, b.advice_equalities[2 * i]), raw_cell(out.break_points, b.advice_equalities[2 * i + 1])});
         for (uint64_t i : out.constants.second) out.constant_cells.push_back(raw_cell(out.break_points, b.constant_index[i]));
+        out.instances.assign(items.begin() + A + n_lookups + 2, items.end());
+        for (size_t m = 0; m < I; m++) {
+            out.instance_cells.emplace_back();
+            for (uint64_t r : out.instances[m].second) out.instance_cells[m].push_back(raw_cell(out.break_points, b.instance_index[m][r]));
+        }
         return out;
     }
 
@@ -249,6 +278,7 @@ private:
     PolyPtr adv, q, q_lookup, input, table;
     WitnessBuffers wit_;
     PolyPtr sel_, eq_, const_, const_idx_, rep_;
+    std::vector<PolyPtr> inst_;  // per instance column: its public values, its indices
 };
 
 }  // namespace h2b

@@ -7,7 +7,9 @@
 // Circuit shape (halo2-base `BaseCircuitParams`): A gate-advice columns a0..a{A-1} with selectors q{j} and the vertical
 // gate q (a0 + a1 a2 - a3) (flex_gate/mod.rs:80-91); L lookup-advice columns l0..l{L-1} looked up in `table` as they are
 // (range/mod.rs:131-150), or with L = 0 the selector lookup q_lookup * a0 (range/mod.rs:92-94), or no lookup; one constants
-// column c; equality on [c, a0.., l0..].  Degree 5 / 4 / 3, permutation sets of degree - 2 columns, degree - 1 pieces of h.
+// column c; I instance columns i0..i{I-1} (BaseConfig::configure, gates/circuit/mod.rs:87-93); equality on [c, a0.., l0.., i0..].
+// Degree 5 / 4 / 3, permutation sets of degree - 2 columns, degree - 1 pieces of h.  Instance columns are not committed, blinded
+// or opened (KZG: QUERY_INSTANCE = false): their values enter the transcript and the permutation argument only.
 //
 // The host does what the Rust side does: the Blake2b transcript, the challenges, the blinding scalars and a handful of
 // 254-bit modular operations on them (`HostFr`); no polynomial arithmetic happens here.
@@ -318,11 +320,12 @@ inline Poly* upload_bytes(const Context& ctx, PolyPtr& p, const void* host, size
 }
 
 // ------------------------------------------------------------------------------------------------ the circuit's shape
-// What halo2-base's constraint system is for (k, A, L, selector_lookup): the one place the prover, the check, MockProver and
+// What halo2-base's constraint system is for (k, A, L, selector_lookup, I): the one place the prover, the check, MockProver and
 // keygen read it from.  The selector lookup needs L = 0; blinding factors max(3, queries of a gate column = 4) + 2 = 6.
+// Instance columns change neither the degree nor the blinding factors.
 struct CircuitShape {
-    CircuitShape(uint32_t k, size_t A, size_t L, bool selector_lookup)
-        : k(k), n(size_t(1) << k), A(A), L(L), selector_lookup(selector_lookup && L == 0) {
+    CircuitShape(uint32_t k, size_t A, size_t L, bool selector_lookup, size_t I = 0)
+        : k(k), n(size_t(1) << k), A(A), L(L), I(I), selector_lookup(selector_lookup && L == 0) {
         degree = L ? 4 : (this->selector_lookup ? 5 : 3);
         chunk = degree - 2;
         ext_k = k + (degree == 3 ? 1 : 2);
@@ -331,6 +334,8 @@ struct CircuitShape {
         for (size_t t = 0; t < L; t++) adv_names.push_back("l" + std::to_string(t));
         perm_cols.push_back("c");
         perm_cols.insert(perm_cols.end(), adv_names.begin(), adv_names.end());
+        for (size_t m = 0; m < I; m++) inst_names.push_back("i" + std::to_string(m));
+        perm_cols.insert(perm_cols.end(), inst_names.begin(), inst_names.end());
         n_sets = (perm_cols.size() + chunk - 1) / chunk;
         n_lookups = L ? L : (this->selector_lookup ? 1 : 0);
         for (size_t j = 0; j < A; j++) fixed_names.push_back("q" + std::to_string(j));
@@ -340,12 +345,12 @@ struct CircuitShape {
         for (auto& nm : perm_cols) sigma_names.push_back("sigma_" + nm);
     }
     uint32_t k, ext_k = 0;
-    size_t n, A, L;
+    size_t n, A, L, I;
     bool selector_lookup;
     size_t degree = 0, chunk = 0, n_sets = 0, n_lookups = 0, u = 0;
     uint32_t bf = 6;
-    // adv: a0.., l0..;  perm: c, adv;  fixed: q0.., [q_lookup], [table], c;  sigma: sigma_{perm}
-    std::vector<std::string> adv_names, perm_cols, fixed_names, sigma_names;
+    // adv: a0.., l0..;  inst: i0..;  perm: c, adv, inst;  fixed: q0.., [q_lookup], [table], c;  sigma: sigma_{perm}
+    std::vector<std::string> adv_names, inst_names, perm_cols, fixed_names, sigma_names;
 };
 
 // the vertical gate q (a0 + a1 a2 - a3) on fixed and advice slot `slot`, advice rotations 0..3 (flex_gate/mod.rs:80-91)
@@ -361,25 +366,25 @@ inline ValueSource add_vertical_gate(GraphEvaluator& ev, uint32_t slot) {
 class ProverCircuit : public CircuitShape {
 public:
     // fixed: Lagrange values (2^k each) by name — q0..q{A-1}, [q_lookup], [table], c; sigma: one column per permutation column
-    // in the order [c, a0.., l0..]
+    // in the order [c, a0.., l0.., i0..] (I instance columns)
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, std::vector<Fr>>& fixed,
-                  const std::vector<std::vector<Fr>>& sigma)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k)) {}
+                  const std::vector<std::vector<Fr>>& sigma, size_t I = 0)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k), false, I) {}
     // the same with every column as a pointer to its 2^k rows (nothing is copied on the host)
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
-                  const std::vector<const Fr*>& sigma)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false) {}
+                  const std::vector<const Fr*>& sigma, size_t I = 0)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false, I) {}
     // the same with every column as a DEVICE pointer to its 2^k Lagrange values (keygen on the device, h2b200_keygen.hpp): each is
     // copied on the device, then transformed as above
     struct OnDevice {};
     ProverCircuit(OnDevice, const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup,
-                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true) {}
+                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma, size_t I = 0)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true, I) {}
 
 private:
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
-                  const std::vector<const Fr*>& sigma, bool on_device)
-        : CircuitShape(k, A, L, selector_lookup), ctx(ctx) {
+                  const std::vector<const Fr*>& sigma, bool on_device, size_t I)
+        : CircuitShape(k, A, L, selector_lookup, I), ctx(ctx) {
         if (sigma.size() != perm_cols.size()) throw Error(H2B_ERR_ARG, "ProverCircuit: one sigma column per permutation column");
         std::vector<Fr> l0(n, Fr{}), ll(n, Fr{}), la(n, Fr{});
         l0[0] = HostFr::one();
@@ -529,7 +534,8 @@ struct AssignedWitness {
 // The witness of one proof or check as the caller holds it, pointer + count (nothing is copied on the host): the virtual
 // column of the gate cells (Montgomery), break_points as keygen pinned them, and the looked-up cells in assign_raw order (L > 0)
 // either as values (lookup_cells) or, in the halo2-base form, as virtual-column indices (lookup_index) — together with the
-// (index, d) pairs of its Rational cells (see AssignedWitness).
+// (index, d) pairs of its Rational cells (see AssignedWitness).  The public values: instance[m] holds the n_instance[m]
+// Montgomery values of instance column m, for the n_instance_columns = I columns of the circuit.
 struct WitnessView {
     const Fr* cells = nullptr;
     size_t n_cells = 0;
@@ -541,6 +547,9 @@ struct WitnessView {
     const uint64_t* rational_index = nullptr;
     const Fr* rational_den = nullptr;
     size_t n_rational = 0;
+    const Fr* const* instance = nullptr;
+    const size_t* n_instance = nullptr;
+    size_t n_instance_columns = 0;
     bool assigned_form() const { return n_rational || lookup_index; }
 };
 
@@ -590,6 +599,22 @@ inline size_t assign_witness(const Context& ctx, const CircuitShape& s, const Wi
     return bytes;
 }
 
+// the public values of a proof, check or MockProver run (or a builder's instance cells): one column per instance column of the
+// shape, each within the usable rows when `bounded` (halo2's InstanceTooLarge)
+template <class T>
+inline void check_instances(const std::string& who, const CircuitShape& s, const T* const* values, const size_t* counts, size_t n_columns,
+                            bool bounded = true) {
+    if (n_columns != s.I)
+        throw Error(H2B_ERR_ARG, who + ": " + std::to_string(n_columns) + " instance columns for a circuit with " + std::to_string(s.I));
+    if (s.I && !(counts && values)) throw Error(H2B_ERR_ARG, who + ": instance columns need their arrays and lengths");
+    for (size_t m = 0; m < s.I; m++) {
+        if (bounded && counts[m] > s.u)
+            throw Error(H2B_ERR_ARG, who + ": InstanceTooLarge: instance column i" + std::to_string(m) + " holds " + std::to_string(counts[m]) +
+                                         " values, more than the " + std::to_string(s.u) + " usable rows");
+        if (counts[m] && !values[m]) throw Error(H2B_ERR_ARG, who + ": instance column i" + std::to_string(m) + " is null");
+    }
+}
+
 // (failure count, the first min(count, max_report) failing rows or equality indices, ascending)
 using ReportItem = std::pair<uint64_t, std::vector<uint64_t>>;
 // n_items reports as the check kernels write them, max_report + 1 words each (the count, then the rows); a failure clears
@@ -633,6 +658,7 @@ public:
         adv_block = std::make_unique<Poly>(ctx, n * (cs.A + cs.L));
         for (size_t j = 0; j < cs.adv_names.size(); j++) lagr[cs.adv_names[j]] = ColRef{adv_block.get(), j * n};
         std::vector<std::string> names = cs.adv_names;
+        names.insert(names.end(), cs.inst_names.begin(), cs.inst_names.end());
         for (size_t t = 0; t < cs.n_lookups; t++)
             for (const char* p : {"pa", "ps", "zl"}) names.push_back(p + std::to_string(t));
         for (size_t s = 0; s < cs.n_sets; s++) names.push_back("zp" + std::to_string(s));
@@ -677,7 +703,7 @@ public:
         h2b_ctx* c = ctx.raw();
         Transcript tr;
         Proof res;
-        check_inputs(wit, "create_proof");
+        check_inputs(wit, "create_proof", cs);
         if (!random_poly) throw Error(H2B_ERR_ARG, "create_proof: null random polynomial");
         uint64_t verdict = 0;  // phase 0: the verdict words, read with the first download of its commitments
         auto commit = [&](const std::vector<std::pair<int, ColRef>>& items, bool absorb, bool with_verdict = false) {
@@ -738,8 +764,11 @@ public:
             }
         };
 
-        // ---- phase 0: witness up, assignment, advice commitments (the random polynomial goes up beside them)
+        // ---- phase 0: the public values into the transcript; witness up, assignment, advice commitments (the random polynomial
+        // and the instance columns go up beside them)
+        for (size_t m = 0; m < cs.I; m++) tr.absorb(wit.instance[m], wit.n_instance[m] * sizeof(Fr));
         res.h2d_bytes += assign_witness(ctx, cs, wit, wit.assigned_form(), verdict_words(), adv_block->at(), witness_bufs, random_poly, rnd);
+        res.h2d_bytes += upload_instances(wit);
         std::vector<std::pair<int, ColRef>> items;
         for (auto& nm : cs.adv_names) {
             blind_col(lagr[nm], u);
@@ -754,7 +783,9 @@ public:
         }
         res.theta = tr.squeeze();
         ctx.check(h2b_ctx_side_join(c));  // the random polynomial arrived while phase 0 ran
-        side_transforms(cs.adv_names);
+        std::vector<std::string> phase0 = cs.adv_names;
+        phase0.insert(phase0.end(), cs.inst_names.begin(), cs.inst_names.end());
+        side_transforms(phase0);
         // ---- lookups: compressed input, permuted pair (enqueue only; the verdict words are read after this phase's commitments)
         std::vector<void*> lk_in;
         items.clear();
@@ -988,10 +1019,11 @@ public:
         const uint32_t k = cs.k;
         const size_t n = cs.n, u = cs.u, A = cs.A, L = cs.L;
         h2b_ctx* c = ctx.raw();
-        check_inputs(wit, "check");
+        check_inputs(wit, "check", cs);
         if (max_report < 1 || max_report > H2B_CHECK_MAX_REPORT) throw Error(H2B_ERR_ARG, "check: max_report out of range");
         cs.prepare_check();
         assign_witness(ctx, cs, wit, wit.assigned_form(), verdict_words(), adv_block->at(), witness_bufs);
+        upload_instances(wit);
         Poly* zero_rows = grown(ctx, check_zero, n - u);  // zero-filled, never written
         for (auto& nm : cs.adv_names) ctx.check(h2b_poly_copy_dev(c, lagr[nm].ptr(u), zero_rows->at(), n - u));
         // report block: element 0 = the witness-form verdict words, then max_report + 1 words per gate, lookup, permutation column
@@ -1013,6 +1045,7 @@ public:
         }
         std::vector<const void*> cols{cs.lagr.at("c")->at()};
         for (auto& nm : cs.adv_names) cols.push_back(lagr[nm].ptr());
+        for (auto& nm : cs.inst_names) cols.push_back(lagr[nm].ptr());
         check_copies_dev(ctx, cols, cs.check_map->at(), k, max_report, at(A + cs.n_lookups));
         const std::vector<Fr> raw = rep->download(0, elems);
         const uint64_t* w = raw[0].data();
@@ -1064,10 +1097,22 @@ private:
         }
         return w;
     }
-    static void check_inputs(const WitnessView& w, const std::string& who) {
+    static void check_inputs(const WitnessView& w, const std::string& who, const CircuitShape& s) {
         if (w.lookup_cells && w.lookup_index) throw Error(H2B_ERR_ARG, who + ": pass the looked-up cells either as values or as indices");
         if (w.n_rational && !(w.rational_index && w.rational_den))
             throw Error(H2B_ERR_ARG, who + ": n_rational > 0 needs rational_index and rational_den");
+        check_instances(who, s, w.instance, w.n_instance, w.n_instance_columns);
+    }
+    // instance column m: rows [0, n_instance[m]) = its public values, the rest zero (beside phase 0 on the main queue)
+    size_t upload_instances(const WitnessView& w) {
+        size_t bytes = 0;
+        for (size_t m = 0; m < cs.I; m++) {
+            const ColRef& col = lagr[cs.inst_names[m]];
+            ctx.check(h2b_poly_zero(ctx.raw(), col.poly->raw()));
+            if (w.n_instance[m]) col.poly->upload(w.instance[m], w.n_instance[m]);
+            bytes += 32 * w.n_instance[m];
+        }
+        return bytes;
     }
     [[noreturn]] static void witness_error(uint32_t rat_bad, uint32_t lk_bad, const std::string& who) {
         std::string why;
