@@ -145,6 +145,8 @@ SIGNATURES = {
     "h2b_count_distinct_dev": (_int, [_vp, _vp, _sz, _vp]),
     "h2b_keygen_copies_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
     "h2b_keygen_instance_edges_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _sz, _sz, _vp, _vp, _vp, _vp]),
+    "h2b_keygen_copies_nf_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _sz, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]),
+    "h2b_keygen_instance_edges_nf_dev": (_int, [_vp, _sz, _vp, _sz, _u32, _sz, _sz, _sz, _sz, _sz, _vp, _vp, _vp, _vp]),
     "h2b_keygen_sigma_map_dev": (_int, [_vp, _vp, _sz, _sz, _u32, _vp]),
     "h2b_keygen_sigma_values_dev": (_int, [_vp, _vp, _sz, _u32, _vp]),
     "h2b_divide_by_vanishing_poly": (_int, [_vp, _vp, _u32, _u32]),
@@ -200,7 +202,7 @@ _witp = C.POINTER(Witness)
 _u64s = C.POINTER(C.c_uint64)
 
 PROVER_SIGNATURES = {
-    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, _sz, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp)]),
+    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, _sz, _sz, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp)]),
     "h2bp_circuit_free": (None, [_vp]),
     "h2bp_circuit_info": (_int, [_vp, _u64s, C.c_char_p, _sz]),
     "h2bp_circuit_column": (_int, [_vp, C.c_char_p, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
@@ -211,11 +213,11 @@ PROVER_SIGNATURES = {
     "h2bp_session_shard": (_int, [_vp, _sz, _sz, ALLREDUCE_FN, _vp]),
     "h2bp_prove": (_int, [_vp, _witp, _vp, BLIND_FN, _vp, COMMIT_FN, _vp, _vp, _vp, _vp, _vp]),
     "h2bp_check": (_int, [_vp, _witp, _sz, _vp]),
-    "h2bp_mock_create": (_int, [_vp, _u32, _sz, _sz, _int, _u32, _sz, _sz, C.POINTER(_vp), _u64s]),
+    "h2bp_mock_create": (_int, [_vp, _u32, _sz, _sz, _int, _u32, _sz, _sz, _sz, C.POINTER(_vp), _u64s]),
     "h2bp_mock_free": (None, [_vp]),
     "h2bp_mock_column": (_int, [_vp, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
-    "h2bp_mock_run": (_int, [_vp, C.POINTER(BuilderView), _sz, _vp, _u64s, _vp, _vp]),
-    "h2bp_keygen": (_int, [_vp, _vp, _u32, _sz, _sz, _sz, _int, _u32, _sz, C.POINTER(BuilderView), C.POINTER(_vp), _vp, _u64s, _vp, _vp]),
+    "h2bp_mock_run": (_int, [_vp, C.POINTER(BuilderView), _sz, _vp, _u64s, _vp, _vp, _u64s]),
+    "h2bp_keygen": (_int, [_vp, _vp, _u32, _sz, _sz, _sz, _int, _u32, _sz, _sz, C.POINTER(BuilderView), C.POINTER(_vp), _vp, _u64s, _vp, _vp]),
 }
 
 

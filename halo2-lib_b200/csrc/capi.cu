@@ -1424,27 +1424,37 @@ int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_
 }
 
 // ------------------------------------------------------------------------------------------------ keygen of a builder
-int h2b_keygen_copies_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
-                          const void* d_lookup_index, size_t n_lookup, const void* d_pairs, size_t M, const void* d_consts,
-                          const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status) {
+int h2b_keygen_copies_nf_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                             const void* d_lookup_index, size_t n_lookup, const void* d_pairs, size_t M, const void* d_consts,
+                             const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status) {
     return guarded(ctx, [&] {
         H2B_REQUIRE((break_points || nbp == 0) && (d_lookup_index || n_lookup == 0) && (d_pairs || M == 0) &&
-                        ((d_consts && d_const_index) || Mc == 0) && d_c && (d_edges || nbp + n_lookup + M + Mc == 0) && d_status,
+                        ((d_consts && d_const_index) || Mc == 0) && (d_c || F == 0) && (d_edges || nbp + n_lookup + M + Mc == 0) && d_status,
                     "keygen_copies: null pointer");
-        keygen_copies_run(ctx, N, break_points, nbp, k, A, L, (const uint64_t*)d_lookup_index, n_lookup, (const uint64_t*)d_pairs, M, d_consts,
+        keygen_copies_run(ctx, N, break_points, nbp, k, F, A, L, (const uint64_t*)d_lookup_index, n_lookup, (const uint64_t*)d_pairs, M, d_consts,
                           (const uint64_t*)d_const_index, Mc, d_c, d_edges, d_status);
     });
 }
-int h2b_keygen_instance_edges_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
-                                  size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges, uint32_t* d_status) {
+int h2b_keygen_copies_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
+                          const void* d_lookup_index, size_t n_lookup, const void* d_pairs, size_t M, const void* d_consts,
+                          const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status) {
+    return h2b_keygen_copies_nf_dev(ctx, N, break_points, nbp, k, 1, A, L, d_lookup_index, n_lookup, d_pairs, M, d_consts, d_const_index, Mc, d_c,
+                                    d_edges, d_status);
+}
+int h2b_keygen_instance_edges_nf_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                                     size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges, uint32_t* d_status) {
     return guarded(ctx, [&] {
         size_t total = 0;
         for (size_t m = 0; m < I && n_index; m++) total += n_index[m];
         H2B_REQUIRE((break_points || nbp == 0) && (n_index || I == 0) && (d_index || total == 0) && (d_edges || total == 0) &&
                         (d_status || I == 0),
                     "keygen_instance_edges: null pointer");
-        keygen_instance_edges_run(ctx, N, break_points, nbp, k, A, L, usable, I, n_index, (const uint64_t*)d_index, d_edges, d_status);
+        keygen_instance_edges_run(ctx, N, break_points, nbp, k, F, A, L, usable, I, n_index, (const uint64_t*)d_index, d_edges, d_status);
     });
+}
+int h2b_keygen_instance_edges_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
+                                  size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges, uint32_t* d_status) {
+    return h2b_keygen_instance_edges_nf_dev(ctx, N, break_points, nbp, k, 1, A, L, usable, I, n_index, d_index, d_edges, d_status);
 }
 int h2b_keygen_sigma_map_dev(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map) {
     return guarded(ctx, [&] {

@@ -272,11 +272,11 @@ void exclusive_scan(h2b_ctx* ctx, const uint32_t* d_in, uint32_t n, uint32_t* d_
 // ---- ntt.cu: omega^r = lo[r mod 2^h] * hi[r >> h] for the 2^k domain root (the power tables of its NTT plan)
 void domain_power_tables(h2b_ctx* ctx, uint32_t k, const void** lo, const void** hi, int* h);
 // ---- keygen.cu (include/h2b200.h, "keygen of a halo2-base builder")
-void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, const uint64_t* d_lookup_index,
-                       size_t n_lookup, const uint64_t* d_pairs, size_t M, const void* d_consts, const uint64_t* d_const_index, size_t Mc,
-                       void* d_c, void* d_edges, uint32_t* status);
-void keygen_instance_edges_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, size_t usable,
-                               size_t I, const size_t* n_index, const uint64_t* d_index, void* d_edges, uint32_t* status);
+void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                       const uint64_t* d_lookup_index, size_t n_lookup, const uint64_t* d_pairs, size_t M, const void* d_consts,
+                       const uint64_t* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* status);
+void keygen_instance_edges_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                               size_t usable, size_t I, const size_t* n_index, const uint64_t* d_index, void* d_edges, uint32_t* status);
 void keygen_sigma_map_run(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map);
 void keygen_sigma_values_run(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma);
 // ---- check.cu (MockProver::verify's checks; reports of max_report + 1 words per item, see include/h2b200.h)

@@ -1,14 +1,15 @@
 // keygen.cu — the permutation side of keygen_vk / keygen_pk for the circuit halo2-base builds, on the device: the constants
-// column, the copy calls in halo2-base's order, and sigma bit-exact to halo2's permutation Assembly (DESIGN.md §4.8).
+// columns, the copy calls in halo2-base's order, and sigma bit-exact to halo2's permutation Assembly (DESIGN.md §4.8, §4.11).
 //
 // Assembly::copy(a, b) returns when a and b are already in one cycle and otherwise swaps mapping[a] and mapping[b] (aux and
 // sizes only answer "same cycle?").  So the final mapping is the product of the transpositions of the copies that joined
 // two classes when they were made, in call order:  sigma = t_1 o t_2 o .. o t_F.  Those copies are the spanning forest
 // Kruskal builds with weight = call index (unique: the weights are distinct), found here by Borůvka; sigma(x) is the walk
 // from x that keeps crossing the largest forest edge below the last one crossed (t_F is applied first).
-//   copies:  u32 cell-id pairs (c n + r, permutation column c in [c, a0.., l0.., i0..] order) in call order: break copies,
-//            lookup copies, advice equalities sorted by (a, b), constant equalities sorted by (constant, cell), and then
-//            (assign_instances, after the region) the instance copies column by column;
+//   copies:  u32 cell-id pairs (c n + r, permutation column c in [c, c1.., a0.., l0.., i0..] order: F constants columns, then
+//            a_j = F + j, l_t = F + A + t, i_m = F + A + L + m) in call order: break copies, lookup copies, advice equalities
+//            sorted by (a, b), constant equalities sorted by (constant, cell) with distinct constant d in constants column
+//            d mod F, row d div F, and then (assign_instances, after the region) the instance copies column by column;
 //   forest:  hook-and-compress rounds: atomicMin of the incident edge index per component root; a root hooks onto the root
 //            across its edge (of two roots that chose the same edge the lower stays a root); pointer jumping until flat;
 //   walk:    2E darts (vertex, edge) sorted by lookup.cu's radix sort; a dart's successor is the dart before its twin at the
@@ -43,7 +44,7 @@ static u32 read_word(h2b_ctx* ctx, const u32* d) {
 // ------------------------------------------------------------------------------------------------------------ copies
 struct Layout {
     const uint64_t* ends;  // ends[j] = start of gate column j + 1 in the virtual column (= bp_0 + .. + bp_j), j < nbp
-    u32 nbp, n, A, L;
+    u32 nbp, n, F, A, L;  // F: the number of constants columns, the first F permutation columns
     uint64_t N;
 };
 
@@ -55,15 +56,16 @@ __device__ __forceinline__ u32 raw_cell(const Layout& y, uint64_t p) {
         if (__ldg(y.ends + mid) >= p) hi = mid; else lo = mid + 1;
     }
     const uint64_t s = lo ? __ldg(y.ends + lo - 1) : 0;
-    return (1 + lo) * y.n + (u32)(p - s);
+    return (y.F + lo) * y.n + (u32)(p - s);
 }
 
 // the gate walk's layout: ends[j] = bp_0 + .. + bp_j uploaded to d_ends (nbp + 1 words, stream-ordered)
-static Layout upload_layout(h2b_ctx* ctx, const char* who, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
-                            uint64_t* d_ends) {
+static Layout upload_layout(h2b_ctx* ctx, const char* who, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A,
+                            size_t L, uint64_t* d_ends) {
     Layout y;
     y.nbp = (u32)nbp;
     y.n = (u32)1 << k;
+    y.F = (u32)F;
     y.A = (u32)A;
     y.L = (u32)L;
     y.N = N;
@@ -85,7 +87,7 @@ __global__ void __launch_bounds__(256) k_kg_lookup_edges(Layout y, const uint64_
     if (i >= m) return;
     const uint64_t p = __ldg(index + i);
     if (p >= y.N) atomicOr(status, 1u);
-    edges[i] = make_uint2(p < y.N ? raw_cell(y, p) : 0, (1 + y.A + i % y.L) * y.n + i / y.L);
+    edges[i] = make_uint2(p < y.N ? raw_cell(y, p) : 0, (y.F + y.A + i % y.L) * y.n + i / y.L);
 }
 
 // 256-bit sort keys: (a << 32 | b) of advice equality i; an index >= N sets bit 1 of *status
@@ -139,26 +141,32 @@ __global__ void __launch_bounds__(256) k_kg_const_heads(const uint64_t* __restri
     heads[i] = head ? 1u : 0u;
 }
 
-// constant equality i of the sorted order: the constant's row of c (its distinct rank) ~ raw(cell); each head places its
-// constant at its row (rows >= n are not written: the caller raises NotEnoughRowsAvailable)
+// constant equality i of the sorted order: the cell of its constant ~ raw(cell).  Distinct constant d (the rank of its run's
+// head) goes left to right, then top to bottom: constants column d mod F, row d div F, cell id (d mod F) n + d div F, which is
+// also its offset in the F x n block c_block.  Each head places its constant there; a rank >= F n is not written (F = 0: none
+// is; the caller raises NotEnoughRowsAvailable, or the index-out-of-bounds panic when F = 0)
 __global__ void __launch_bounds__(256) k_kg_const_edges(Layout y, const uint64_t* __restrict__ consts, const uint64_t* __restrict__ index,
                                                         const u32* __restrict__ order, const u32* __restrict__ heads, const u32* __restrict__ rows,
-                                                        u32 m, uint64_t* __restrict__ c_col, uint2* __restrict__ edges) {
+                                                        u32 m, uint64_t* __restrict__ c_block, uint2* __restrict__ edges) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
-    const u32 src = __ldg(order + i), row = __ldg(rows + i) + __ldg(heads + i) - 1;  // the rank of this run's head
+    const u32 src = __ldg(order + i), d = __ldg(rows + i) + __ldg(heads + i) - 1;
     const uint64_t p = __ldg(index + src);
-    if (__ldg(heads + i) && row < y.n) Fr::load_nc(consts + 4 * (size_t)src).store(c_col + 4 * (size_t)row);
-    edges[i] = make_uint2(row < y.n ? row : 0, p < y.N ? raw_cell(y, p) : 0);
+    u32 cell = 0;
+    if (d < y.F * y.n) {
+        cell = (d % y.F) * y.n + d / y.F;
+        if (__ldg(heads + i)) Fr::load_nc(consts + 4 * (size_t)src).store(c_block + 4 * (size_t)cell);
+    }
+    edges[i] = make_uint2(cell, p < y.N ? raw_cell(y, p) : 0);
 }
 
-void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, const uint64_t* d_lookup_index,
-                       size_t n_lookup, const uint64_t* d_pairs, size_t M, const void* d_consts, const uint64_t* d_const_index, size_t Mc,
-                       void* d_c, void* d_edges, uint32_t* status) {
+void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                       const uint64_t* d_lookup_index, size_t n_lookup, const uint64_t* d_pairs, size_t M, const void* d_consts,
+                       const uint64_t* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* status) {
     H2B_REQUIRE(k >= 3 && k <= 28, "keygen_copies: k out of range (3..28)");
     const size_t n = (size_t)1 << k;
     H2B_REQUIRE(A >= 1 && nbp < A, "keygen_copies: need A >= 1 gate columns and fewer break points than that");
-    H2B_REQUIRE((1 + A + L) * n < NONE, "keygen_copies: the permutation columns hold more than 2^32 - 1 cells");
+    H2B_REQUIRE(F < NONE && (F + A + L) * n < NONE, "keygen_copies: the permutation columns hold more than 2^32 - 1 cells");
     H2B_REQUIRE(N < ((size_t)1 << 32) && n_lookup < ((size_t)1 << 31) && M < ((size_t)1 << 31) && Mc < ((size_t)1 << 31),
                 "keygen_copies: at most 2^32 - 1 cells and 2^31 - 1 copies of each kind");
     H2B_REQUIRE(L || n_lookup == 0, "keygen_copies: lookup copies need lookup-advice columns");
@@ -169,15 +177,15 @@ void keygen_copies_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, siz
                  o_ord2 = o_ord + al(4 * (size_t)m), o_heads = o_ord2 + al(4 * (size_t)m), o_rows = o_heads + al(4 * (size_t)m),
                  o_sort = o_rows + al(4 * (size_t)m), o_scan = o_sort + al(sort_keys_scratch(m, ctas));
     Scratch s(o_scan + al(exclusive_scan_scratch(m)));
-    const Layout y = upload_layout(ctx, "keygen_copies", N, break_points, nbp, k, A, L, s.at<uint64_t>(0));
+    const Layout y = upload_layout(ctx, "keygen_copies", N, break_points, nbp, k, F, A, L, s.at<uint64_t>(0));
     std::vector<uint32_t> brk(2 * nbp);
     for (size_t j = 0; j < nbp; j++) {
-        brk[2 * j] = (u32)((2 + j) * n);                      // (a_{j+1}, 0)
-        brk[2 * j + 1] = (u32)((1 + j) * n + break_points[j]);  // (a_j, bp_j)
+        brk[2 * j] = (u32)((F + 1 + j) * n);                    // (a_{j+1}, 0)
+        brk[2 * j + 1] = (u32)((F + j) * n + break_points[j]);  // (a_j, bp_j)
     }
     uint2* edges = (uint2*)d_edges;
     H2B_CUDA(cudaMemsetAsync(status, 0, 8, ctx->stream));
-    H2B_CUDA(cudaMemsetAsync(d_c, 0, 32 * n, ctx->stream));
+    if (F) H2B_CUDA(cudaMemsetAsync(d_c, 0, 32 * F * n, ctx->stream));
     if (nbp) H2B_CUDA(cudaMemcpyAsync(edges, brk.data(), 8 * nbp, cudaMemcpyHostToDevice, ctx->stream));
     edges += nbp;
     if (n_lookup) H2B_LAUNCH(ctx, k_kg_lookup_edges, ceil_div(n_lookup, 256), 256, 0, y, d_lookup_index, (u32)n_lookup, edges, status);
@@ -221,18 +229,18 @@ __global__ void __launch_bounds__(256) k_kg_instance_edges(Layout y, const uint6
     if (p >= y.N && r <= usable) atomicOr(status, 1u);
     if (r >= usable) atomicOr(status, 2u);
     const bool ok = p < y.N && r < usable;
-    edges[r] = ok ? make_uint2(raw_cell(y, p), (1 + y.A + y.L + col) * y.n + r) : make_uint2(0, 0);
+    edges[r] = ok ? make_uint2(raw_cell(y, p), (y.F + y.A + y.L + col) * y.n + r) : make_uint2(0, 0);
 }
 
-void keygen_instance_edges_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L, size_t usable,
-                               size_t I, const size_t* n_index, const uint64_t* d_index, void* d_edges, uint32_t* status) {
+void keygen_instance_edges_run(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                               size_t usable, size_t I, const size_t* n_index, const uint64_t* d_index, void* d_edges, uint32_t* status) {
     H2B_REQUIRE(k >= 3 && k <= 28, "keygen_instance_edges: k out of range (3..28)");
     const size_t n = (size_t)1 << k;
     H2B_REQUIRE(A >= 1 && nbp < A && usable <= n, "keygen_instance_edges: need A >= 1 gate columns, fewer break points and usable <= 2^k");
-    H2B_REQUIRE((1 + A + L + I) * n < NONE, "keygen_instance_edges: the permutation columns hold more than 2^32 - 1 cells");
+    H2B_REQUIRE(F < NONE && I < NONE && (F + A + L + I) * n < NONE, "keygen_instance_edges: the permutation columns hold more than 2^32 - 1 cells");
     H2B_REQUIRE(N < ((size_t)1 << 32), "keygen_instance_edges: at most 2^32 - 1 cells");
     Scratch s(8 * (nbp + 1));
-    const Layout y = upload_layout(ctx, "keygen_instance_edges", N, break_points, nbp, k, A, L, s.at<uint64_t>(0));
+    const Layout y = upload_layout(ctx, "keygen_instance_edges", N, break_points, nbp, k, F, A, L, s.at<uint64_t>(0));
     if (I) H2B_CUDA(cudaMemsetAsync(status, 0, 4 * I, ctx->stream));
     uint2* edges = (uint2*)d_edges;
     for (size_t col = 0; col < I; col++) {

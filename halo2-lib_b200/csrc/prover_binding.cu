@@ -32,8 +32,8 @@ struct BoundCircuit {
 struct BoundMock {
     Context ctx;
     MockProver mock;
-    BoundMock(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, uint32_t lookup_bits, size_t max_rows, size_t I)
-        : ctx(c), mock(ctx, k, A, L, sel, lookup_bits, max_rows, I) {}
+    BoundMock(h2b_ctx* c, uint32_t k, size_t A, size_t L, bool sel, uint32_t lookup_bits, size_t max_rows, size_t I, size_t F)
+        : ctx(c), mock(ctx, k, A, L, sel, lookup_bits, max_rows, I, F) {}
 };
 struct BoundSession {
     Context ctx;
@@ -106,8 +106,9 @@ typedef int (*h2bp_commit_fn)(void* user, int basis, const uint64_t* rows, size_
 
 #define H2BP_API extern "C" __attribute__((visibility("default")))
 
-// fixed: n_fixed named columns (at least the circuit's fixed_names), sigma: one per permutation column; 2^k rows each; I instance columns
-H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, size_t I, const char* const* fixed_names,
+// fixed: n_fixed named columns (at least the circuit's fixed_names), sigma: one per permutation column; 2^k rows each; I instance
+// columns, F constants columns
+H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, size_t I, size_t F, const char* const* fixed_names,
                                  const uint64_t* const* fixed, size_t n_fixed, const uint64_t* const* sigma, size_t n_sigma,
                                  BoundCircuit** out) {
     return run(ctx, [&] {
@@ -117,13 +118,14 @@ H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, i
         std::vector<const Fr*> s;
         for (size_t i = 0; i < n_sigma; i++) s.push_back(reinterpret_cast<const Fr*>(sigma[i]));
         auto b = std::make_unique<BoundCircuit>(ctx);
-        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s, I);
+        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s, I, F);
         *out = b.release();
     });
 }
 H2BP_API void h2bp_circuit_free(BoundCircuit* b) { delete b; }
 
-// shape: degree, chunk, ext_k, bf, u, n_sets, n_lookups, selector_lookup; names: "adv=..\nperm=..\nfixed=..\nsigma=.." (comma-separated)
+// shape: degree, chunk, ext_k, bf, u, n_sets, n_lookups, selector_lookup; names: "adv=..\nperm=..\nfixed=..\nsigma=..\nconst=.."
+// (comma-separated; const: the constants columns, empty when F = 0)
 H2BP_API int h2bp_circuit_info(BoundCircuit* b, uint64_t* shape, char* names, size_t cap) {
     return run(b ? b->ctx.raw() : nullptr, [&] {
         const ProverCircuit& cs = *b->cs;
@@ -131,7 +133,7 @@ H2BP_API int h2bp_circuit_info(BoundCircuit* b, uint64_t* shape, char* names, si
         if (!shape) throw Error(H2B_ERR_ARG, "circuit_info: null shape");
         std::copy(v, v + 8, shape);
         write_text("adv=" + join(cs.adv_names) + "\nperm=" + join(cs.perm_cols) + "\nfixed=" + join(cs.fixed_names) + "\nsigma=" +
-                       join(cs.sigma_names),
+                       join(cs.sigma_names) + "\nconst=" + join(cs.const_names),
                    names, cap);
     });
 }
@@ -214,13 +216,13 @@ H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report
     });
 }
 
-// MockProver of a builder (include/h2b200_mock.hpp), I instance columns.  n_lookups: the number of lookup reports (L, 1 for the
-// selector lookup, or 0)
+// MockProver of a builder (include/h2b200_mock.hpp), I instance columns, F constants columns.  n_lookups: the number of lookup
+// reports (L, 1 for the selector lookup, or 0)
 H2BP_API int h2bp_mock_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits, size_t max_rows, size_t I,
-                              BoundMock** out, uint64_t* n_lookups) {
+                              size_t F, BoundMock** out, uint64_t* n_lookups) {
     return run(ctx, [&] {
         if (!out || !n_lookups) throw Error(H2B_ERR_ARG, "mock_create: null argument");
-        *out = new BoundMock(ctx, k, A, L, selector_lookup != 0, lookup_bits, max_rows, I);
+        *out = new BoundMock(ctx, k, A, L, selector_lookup != 0, lookup_bits, max_rows, I, F);
         *n_lookups = (*out)->mock.n_lookups;
     });
 }
@@ -232,12 +234,14 @@ H2BP_API int h2bp_mock_column(BoundMock* b, const char* name, h2b_poly** poly, s
 // one run.  break_points: A - 1 words (the count in *n_break_points); report: max_report + 1 words per gate column, lookup, then
 // the advice equalities, the constant equalities and each instance column (as h2bp_check); cells: max_report x (column, row,
 // column, row) of the reported advice equalities, then max_report x (column, row) of the reported constant equalities, then
-// the same for the reported rows of each instance column
+// the same for the reported rows of each instance column; *distinct_constants: the number of distinct constants
 H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report, uint64_t* break_points, uint64_t* n_break_points,
-                           uint64_t* report, uint64_t* cells) {
+                           uint64_t* report, uint64_t* cells, uint64_t* distinct_constants) {
     return run(b ? b->ctx.raw() : nullptr, [&] {
-        if (!v || !n_break_points || !report || !cells || (b->mock.A > 1 && !break_points)) throw Error(H2B_ERR_ARG, "mock_run: null argument");
+        if (!v || !n_break_points || !report || !cells || !distinct_constants || (b->mock.A > 1 && !break_points))
+            throw Error(H2B_ERR_ARG, "mock_run: null argument");
         const MockReport r = b->mock.run(*v, max_report);
+        *distinct_constants = r.distinct_constants;
         *n_break_points = r.break_points.size();
         std::copy(r.break_points.begin(), r.break_points.end(), break_points);
         uint64_t* p = report;
@@ -265,16 +269,16 @@ H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report
 
 // keygen of a builder (include/h2b200_keygen.hpp).  Out: the circuit (freed with h2bp_circuit_free); break_points (A - 1 words,
 // the count in *n_break_points); vk: 12 limbs per commitment, the fixed columns in the circuit's fixed_names order, then the sigma
-// columns (1 + A + L + v->n_instance_columns); times: the five phases of KeygenTimes in ms (may be null)
+// columns (F + A + L + v->n_instance_columns); times: the five phases of KeygenTimes in ms (may be null); F constants columns
 H2BP_API int h2bp_keygen(h2b_ctx* ctx, h2b_srs* srs, uint32_t k, size_t srs_count, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits,
-                         size_t max_rows, const BuilderView* v, BoundCircuit** out, uint64_t* break_points, uint64_t* n_break_points, uint64_t* vk,
+                         size_t max_rows, size_t F, const BuilderView* v, BoundCircuit** out, uint64_t* break_points, uint64_t* n_break_points, uint64_t* vk,
                          double* times) {
     return run(ctx, [&] {
         if (!srs || !v || !out || !n_break_points || !vk || (A > 1 && !break_points)) throw Error(H2B_ERR_ARG, "keygen: null argument");
         auto b = std::make_unique<BoundCircuit>(ctx);
         const ParamsKZG params(b->ctx, k, srs, srs_count);
         KeygenTimes t;
-        KeygenResult r = keygen(b->ctx, params, k, A, L, selector_lookup != 0, lookup_bits, max_rows, *v, &t);
+        KeygenResult r = keygen(b->ctx, params, k, A, L, selector_lookup != 0, lookup_bits, max_rows, *v, &t, F);
         b->cs = std::move(r.pk);
         *n_break_points = r.break_points.size();
         std::copy(r.break_points.begin(), r.break_points.end(), break_points);

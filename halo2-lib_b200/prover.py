@@ -133,17 +133,17 @@ class Circuit:
     """The fixed side of a synthetic halo2-base circuit (what keygen_pk would hold), resident on the GPU in the three forms
     create_proof needs: Lagrange values, coefficients, extended-coset evaluations (h2b::ProverCircuit).
 
-    Shape (halo2-base `BaseCircuitParams`: num_advice_per_phase, num_lookup_advice_per_phase, num_fixed = 1):
+    Shape (halo2-base `BaseCircuitParams`: num_advice_per_phase, num_lookup_advice_per_phase, num_fixed = F):
       A gate-advice columns a0..a{A-1}, each with its selector q{j} and the vertical gate (flex_gate/mod.rs:80-91);
       L lookup-advice columns l0..l{L-1}, each looked up in `table` as it is (range/mod.rs:131-150); with L = 0 the one
       lookup is `q_lookup * a0 in table` (range/mod.rs:92-94), or none at all with selector_lookup = False;
-      one constants column c; I instance columns i0..i{I-1} (BaseConfig::configure, gates/circuit/mod.rs:87-93);
-      equality on [c, a0.., l0.., i0..] in that order (the permutation's column order).
+      F constants columns c, c1..c{F-1} (F = 0: none); I instance columns i0..i{I-1} (BaseConfig::configure,
+      gates/circuit/mod.rs:87-93); equality on [c, c1.., a0.., l0.., i0..] in that order (the permutation's column order).
     The shape numbers and column names are read from the compiled circuit.  `lagr`, `coeff`, `ext` (by column name) and
     `sigma_map` (the decoded sigma of the check) look up its device columns."""
 
     def __init__(self, ctx: Context, k: int, fixed_lagrange: dict, sigma_lagrange: list, A: int = 1, L: int = 0,
-                 selector_lookup: bool = True, I: int = 0):
+                 selector_lookup: bool = True, I: int = 0, F: int = 1):
         n = 1 << k
         fixed = {nm: _rows(a, n, nm) for nm, a in fixed_lagrange.items()}
         sigma = [_rows(a, n, "sigma %d" % i) for i, a in enumerate(sigma_lagrange)]
@@ -151,7 +151,7 @@ class Circuit:
         ptrs = (C.c_void_p * len(fixed))(*[a.ctypes.data for a in fixed.values()])
         sptrs = (C.c_void_p * len(sigma))(*[a.ctypes.data for a in sigma])
         h = C.c_void_p()
-        ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), I, names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h)))
+        ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), I, F, names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h)))
         self._bind(ctx, k, A, L, h)
 
     def _bind(self, ctx: Context, k: int, A: int, L: int, h: C.c_void_p):
@@ -162,9 +162,11 @@ class Circuit:
         ctx.check(lib.h2bp_circuit_info(h, shape, text, len(text)))
         self.degree, self.chunk, self.ext_k, self.bf, self.u, self.n_sets, self.n_lookups, sel = (int(v) for v in shape)
         self.selector_lookup = bool(sel)
-        lists = {key: v.split(",") for key, v in (line.split("=", 1) for line in text.value.decode().split("\n"))}
-        self.adv_names, self.perm_cols, self.fixed_names, self.sigma_names = (lists[key] for key in ("adv", "perm", "fixed", "sigma"))
-        self.I = len(self.perm_cols) - 1 - A - L
+        lists = {key: v.split(",") if v else [] for key, v in (line.split("=", 1) for line in text.value.decode().split("\n"))}
+        self.adv_names, self.perm_cols, self.fixed_names, self.sigma_names, self.const_names = (
+            lists[key] for key in ("adv", "perm", "fixed", "sigma", "const"))
+        self.F = len(self.const_names)
+        self.I = len(self.perm_cols) - self.F - A - L
         self.lagr, self.coeff, self.ext = _Columns(self, "lagr"), _Columns(self, "coeff"), _Columns(self, "ext")
 
     def column(self, table: str, name: str = "") -> Column:
@@ -340,13 +342,14 @@ def _builder_view(who: str, n_cells: int, selectors, advice_equalities, constant
 
 def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
            max_rows: int | None = None, selectors=(), advice_equalities=(), constant_equalities=None, lookups=(), timings: dict | None = None,
-           I: int = 0, instances=None):
+           I: int = 0, instances=None, F: int = 1):
     """keygen_vk + keygen_pk of a halo2-base builder in its keygen form, on the device (h2b::keygen, include/h2b200_keygen.hpp).
 
     The arguments mean what they mean for MockProver.run (selectors: one per cell of the virtual column, which fixes its length;
     no witness values are read).  sigma is the one halo2's permutation Assembly builds from halo2-base's copy calls, bit for bit.
     I instance columns, `instances` the indices of each one's cells (BaseCircuitBuilder::assigned_instances; None: all empty):
-    their copies follow the region's.
+    their copies follow the region's.  F constants columns c, c1.. (BaseCircuitParams::num_fixed, 0 when the builder has no
+    constant equalities): distinct constant d of the sorted order goes to column d mod F, row d div F.
     Returns (circuit, vk, break_points): `circuit` is a Circuit that ProverSession takes; vk = {"fixed": {name: commitment},
     "permutation": [commitment per permutation column, perm_cols order]}, each commitment affine as 12 Montgomery limbs
     (x, y, 1; the identity all zero), of the column's Lagrange values.  halo2-base's panics raise H2BError with its message.
@@ -355,11 +358,11 @@ def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, sele
     n_cells = len(np.asarray(selectors).reshape(-1))
     view, keep = _builder_view("keygen", n_cells, selectors, advice_equalities, constant_equalities, lookups, I=I, instances=instances)
     bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
-    n_fixed = A + (1 if selector_lookup and L == 0 else 0) + (1 if L or selector_lookup else 0) + 1
-    vk = np.zeros((n_fixed + 1 + A + L + I, 12), dtype=np.uint64)
+    n_fixed = A + (1 if selector_lookup and L == 0 else 0) + (1 if L or selector_lookup else 0) + F
+    vk = np.zeros((n_fixed + F + A + L + I, 12), dtype=np.uint64)
     times = np.zeros(5, dtype=np.float64)
     h = C.c_void_p()
-    ctx.check(lib.h2bp_keygen(ctx.h, params.h, k, params.count, A, L, int(selector_lookup), lookup_bits, max_rows, C.byref(view), C.byref(h),
+    ctx.check(lib.h2bp_keygen(ctx.h, params.h, k, params.count, A, L, int(selector_lookup), lookup_bits, max_rows, F, C.byref(view), C.byref(h),
                               C.c_void_p(bps.ctypes.data), C.byref(nbp), C.c_void_p(vk.ctypes.data), C.c_void_p(times.ctypes.data)))
     cs = Circuit.__new__(Circuit)
     cs._bind(ctx, k, A, L, h)
@@ -519,17 +522,17 @@ class MockProver:
     """MockProver::run + verify for a halo2-base builder in its keygen form, with no SRS, sigma or proving key
     (h2b::MockProver, include/h2b200_mock.hpp): what BaseTester::run_builder asks of halo2's MockProver.
 
-    Shape as `Circuit`: A gate-advice columns, L lookup-advice columns (or the selector lookup when L = 0, or no lookup), one
-    constants column, the table 0 .. 2^lookup_bits - 1, and max_rows = 2^k - unusable_rows as calculate_params gets it
-    (at most 2^k - 7; default 2^k - 9, BaseTester's unusable_rows), and I instance columns.  `lagr[name]` (a{j}, l{t}, q{j},
-    q_lookup, table) views the columns of the last run."""
+    Shape as `Circuit`: A gate-advice columns, L lookup-advice columns (or the selector lookup when L = 0, or no lookup), F
+    constants columns, the table 0 .. 2^lookup_bits - 1, and max_rows = 2^k - unusable_rows as calculate_params gets it
+    (at most 2^k - 7; default 2^k - 9, BaseTester's unusable_rows), and I instance columns.  F changes no value check, only how
+    many distinct constants fit (F u).  `lagr[name]` (a{j}, l{t}, q{j}, q_lookup, table) views the columns of the last run."""
 
     def __init__(self, ctx: Context, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
-                 max_rows: int | None = None, I: int = 0):
-        self.ctx, self.k, self.A, self.L, self.I = ctx, k, A, L, I
+                 max_rows: int | None = None, I: int = 0, F: int = 1):
+        self.ctx, self.k, self.A, self.L, self.I, self.F = ctx, k, A, L, I, F
         self.max_rows = (1 << k) - 9 if max_rows is None else max_rows
         h, nl = C.c_void_p(), C.c_uint64()
-        ctx.check(lib.h2bp_mock_create(ctx.h, k, A, L, int(selector_lookup), lookup_bits, self.max_rows, I, C.byref(h), C.byref(nl)))
+        ctx.check(lib.h2bp_mock_create(ctx.h, k, A, L, int(selector_lookup), lookup_bits, self.max_rows, I, F, C.byref(h), C.byref(nl)))
         self._h, self.n_lookups = h, int(nl.value)
         self.lagr = _Columns(self, "lagr")
 
@@ -553,7 +556,9 @@ class MockProver:
 
         instances / public: per instance column, the indices of its cells and its public values (Montgomery), one value per cell
         (None: all empty).  instances[m] reports the rows r whose cell differs from public[m][r], instance_cells[m] their raw
-        cells; more than u values raise H2BError (InstanceTooLarge)."""
+        cells; more than u values raise H2BError (InstanceTooLarge).
+
+        distinct_constants: the number D of distinct constants, from which calculate_params sets num_fixed = ceil(D / 2^k)."""
         if not 1 <= max_report <= CHECK_MAX_REPORT:
             raise ValueError("MockProver: max_report must be in 1..%d" % CHECK_MAX_REPORT)
         V = np.ascontiguousarray(cells, dtype=np.uint64).reshape(-1, 4)
@@ -561,11 +566,11 @@ class MockProver:
         view, keep = _builder_view("MockProver", len(V), selectors, advice_equalities, constant_equalities, lookups, V, rational_index,
                                    rational_den, I, instances, [()] * I if public is None else public)
         A, nl = self.A, self.n_lookups
-        bps, nbp = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64()
+        bps, nbp, distinct = np.zeros(max(A, 1), dtype=np.uint64), C.c_uint64(), C.c_uint64()
         words = np.empty((A + nl + 2 + I, max_report + 1), dtype=np.uint64)
         cells_out = np.empty((6 + 2 * I) * max_report, dtype=np.uint64)
         self.ctx.check(lib.h2bp_mock_run(self._h, C.byref(view), max_report, C.c_void_p(bps.ctypes.data), C.byref(nbp),
-                                         C.c_void_p(words.ctypes.data), C.c_void_p(cells_out.ctypes.data)))
+                                         C.c_void_p(words.ctypes.data), C.c_void_p(cells_out.ctypes.data), C.byref(distinct)))
         reports = _reports(words, max_report)
         eq, co = reports[A + nl], reports[A + nl + 1]
         ec = cells_out[:4 * max_report].reshape(-1, 4)
@@ -576,7 +581,8 @@ class MockProver:
                 "equality_cells": [((int(c[0]), int(c[1])), (int(c[2]), int(c[3]))) for c in ec[:len(eq[1])]],
                 "constant_cells": [(int(c[0]), int(c[1])) for c in cc[:len(co[1])]],
                 "break_points": [int(b) for b in bps[:nbp.value]], "satisfied": not any(c for c, _ in reports),
-                "instances": inst, "instance_cells": [[(int(c[0]), int(c[1])) for c in x] for x in ic]}
+                "instances": inst, "instance_cells": [[(int(c[0]), int(c[1])) for c in x] for x in ic],
+                "distinct_constants": int(distinct.value)}
 
     def free(self):
         if self._h:

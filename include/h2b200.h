@@ -466,9 +466,9 @@ int h2b_check_constants_dev(h2b_ctx* ctx, const void* d_cells, size_t N, const v
                             size_t max_report, void* d_report, uint32_t* d_status);
 int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count);
 
-/* ---- keygen of a halo2-base builder: the permutation side of keygen_vk / keygen_pk (see h2b200_keygen.hpp, DESIGN.md §4.8).
- * Cells are u32 ids c 2^k + r, c the permutation column in [c, a0.., a{A-1}, l0.., l{L-1}, i0.., i{I-1}] order.  Synchronous;
- * scratch is allocated and freed per call.
+/* ---- keygen of a halo2-base builder: the permutation side of keygen_vk / keygen_pk (see h2b200_keygen.hpp, DESIGN.md §4.8,
+ * §4.11).  Cells are u32 ids c 2^k + r, c the permutation column in [c, c1.., c{F-1}, a0.., a{A-1}, l0.., l{L-1}, i0.., i{I-1}]
+ * order (F constants columns; the calls without _nf have F = 1).  Synchronous; scratch is allocated and freed per call.
  *   h2b_keygen_copies_dev        the constants column and the copy calls of BaseCircuitBuilder::synthesize in halo2-base's order,
  *                                into d_edges (E = nbp + n_lookup + M + Mc u32 pairs): the break copies (a{j+1}, 0) ~ (a_j,
  *                                bp_j) (break_points: host); the lookup copies raw(index[i]) ~ (l{i mod L}, i / L); the M advice
@@ -486,6 +486,12 @@ int h2b_count_distinct_dev(h2b_ctx* ctx, const void* d_values, size_t m, uint32_
  *                                d_status (I words, zeroed first): word m bit 0 an index >= N at a row r <= usable (halo2-base's
  *                                "instance not assigned" comes before that row's copy), bit 1 a row r >= usable (halo2's copy
  *                                fails with NotEnoughRowsAvailable there); such copies are written as (0, 0), which joins nothing.
+ *   h2b_keygen_copies_nf_dev     h2b_keygen_copies_dev with F constants columns (num_fixed, F >= 0): distinct constant d goes to
+ *                                constants column d mod F, row d div F (left to right, then top to bottom), its copy is
+ *                                ((d mod F) 2^k + d div F) ~ raw(cell), and d_c is an F x 2^k block (column after column, zeroed
+ *                                first; null when F = 0).  d_status[1] is the number of distinct constants D; ranks >= F 2^k are
+ *                                not written (with F = 0 none is: D > 0 is halo2-base's index-out-of-bounds panic).
+ *   h2b_keygen_instance_edges_nf_dev  h2b_keygen_instance_edges_dev with F constants columns before the advice columns.
  *   h2b_keygen_sigma_map_dev     the mapping halo2's permutation Assembly builds from E copies (d_edges, in call order) over
  *                                n_cols x 2^k cells: d_map (n_cols x 2^k u32) = the cell id each cell maps to (as
  *                                h2b_permutation_decode_dev decodes it).  A cell id >= n_cols 2^k is H2B_ERR_ARG.
@@ -495,6 +501,12 @@ int h2b_keygen_copies_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, 
                           const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status);
 int h2b_keygen_instance_edges_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t A, size_t L,
                                   size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges, uint32_t* d_status);
+int h2b_keygen_copies_nf_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A, size_t L,
+                             const void* d_lookup_index, size_t n_lookup, const void* d_pairs, size_t M, const void* d_consts,
+                             const void* d_const_index, size_t Mc, void* d_c, void* d_edges, uint32_t* d_status);
+int h2b_keygen_instance_edges_nf_dev(h2b_ctx* ctx, size_t N, const uint64_t* break_points, size_t nbp, uint32_t k, size_t F, size_t A,
+                                     size_t L, size_t usable, size_t I, const size_t* n_index, const void* d_index, void* d_edges,
+                                     uint32_t* d_status);
 int h2b_keygen_sigma_map_dev(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map);
 int h2b_keygen_sigma_values_dev(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma);
 

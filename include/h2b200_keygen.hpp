@@ -1,18 +1,20 @@
 // h2b200_keygen.hpp — keygen_vk + keygen_pk for a halo2-base builder in its keygen form, on the device: the break points, the
-// fixed columns (q_j, q_lookup, the table, the constants column c), sigma bit-exact to what halo2's permutation Assembly builds
-// from halo2-base's copy calls, the proving key as a ProverCircuit and the verifying key's commitments.  DESIGN.md §4.8.
+// fixed columns (q_j, q_lookup, the table, the constants columns c, c1..), sigma bit-exact to what halo2's permutation Assembly
+// builds from halo2-base's copy calls, the proving key as a ProverCircuit and the verifying key's commitments.  DESIGN.md §4.8,
+// §4.11.
 //
 // The builder comes as MockProver takes it (BuilderView, include/h2b200_mock.hpp); keygen reads no witness values: `cells` and
 // the rational pairs are ignored, `n_cells` is used.  The copy calls of BaseCircuitBuilder::synthesize, in order:
 //   1. the break copies of assign_with_constraints: (a{j+1}, 0) ~ (a_j, bp_j), j = 0, 1, ..;
 //   2. L > 0: LookupAnyManager::assign_raw's copies raw(lookup_index[i]) ~ (l{i mod L}, i / L), i = 0, 1, ..;
 //   3. CopyConstraintManager::assign_raw: the advice equalities sorted by (a, b), then the constant equalities sorted by
-//      (constant, cell) as (c, the constant's row) ~ raw(cell), the distinct constants at rows 0, 1, .. of c in that order;
+//      (constant, cell) as (the constant's cell) ~ raw(cell), the distinct constants placed left to right, then top to bottom
+//      over the F constants columns in that order: distinct constant d at row d div F of column d mod F (c, c1, ..);
 //   4. after the region, BaseCircuitBuilder::assign_instances: raw(instance_index_m[r]) ~ (i_m, r) for each instance column m
 //      (b.n_instance_columns of them) in order and r = 0, 1, .. (an index >= N: "instance not assigned"; r >= u: halo2's
 //      NotEnoughRowsAvailable).
 // So the builder's own order of its equalities does not change the keys.  Errors: halo2-base's panics as MockProver raises them.
-// Several constants columns are not covered (the same boundary as MockProver).
+// F (BaseCircuitParams::num_fixed) may be 0 when the builder has no constant equalities.
 #pragma once
 #include <chrono>
 
@@ -41,9 +43,9 @@ struct KeygenResult {
     VerifyingKey vk;
 };
 
-// params: the SRS of the 2^k domain (its Lagrange bases commit the vk); max_rows as for MockProver (<= 2^k - 7)
+// params: the SRS of the 2^k domain (its Lagrange bases commit the vk); max_rows as for MockProver (<= 2^k - 7); F constants columns
 inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits,
-                           size_t max_rows, const BuilderView& b, KeygenTimes* times = nullptr) {
+                           size_t max_rows, const BuilderView& b, KeygenTimes* times = nullptr, size_t F = 1) {
     using clock = std::chrono::steady_clock;
     auto t0 = clock::now();
     auto lap = [&](double KeygenTimes::*field) {
@@ -51,7 +53,7 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         if (times) times->*field = std::chrono::duration<double, std::milli>(t - t0).count();
         t0 = t;
     };
-    const CircuitShape s = builder_shape("keygen", k, A, L, selector_lookup, lookup_bits, max_rows, b.n_instance_columns);
+    const CircuitShape s = builder_shape("keygen", k, A, L, selector_lookup, lookup_bits, max_rows, b.n_instance_columns, F);
     const size_t n = s.n, N = b.n_cells, M = b.n_advice_equalities, Mc = b.n_constant_equalities, NL = b.n_lookup;
     h2b_ctx* c = ctx.raw();
     KeygenResult out;
@@ -65,7 +67,7 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
     upload_bytes(ctx, eq_d, b.advice_equalities, 16 * M);
     upload_bytes(ctx, const_d, b.constants, 32 * Mc);
     upload_bytes(ctx, const_idx_d, b.constant_index, 8 * Mc);
-    // the fixed columns in the circuit's order: q0.., [q_lookup], [table], c
+    // the fixed columns in the circuit's order: q0.., [q_lookup], [table], c, c1.. (the F constants columns last, one block)
     const size_t nf = s.fixed_names.size();
     Poly fixed(ctx, nf * n), status(ctx, 1);
     auto col = [&](size_t i) { return static_cast<Fr*>(fixed.at(i * n)); };
@@ -78,10 +80,10 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         std::memcpy(v, status.download(0, 1)[0].data(), 8);
         builder_panics(s, v[0] & 1, v[0] & 2, 0, false);
     }
-    if (s.n_lookups) ctx.check(h2b_poly_upload(c, fixed.raw(), (nf - 2) * n, lookup_table(n, lookup_bits)[0].data(), n));
+    if (s.n_lookups) ctx.check(h2b_poly_upload(c, fixed.raw(), (nf - F - 1) * n, lookup_table(n, lookup_bits)[0].data(), n));
     Poly edges(ctx, (8 * E + 31) / 32 + 1);
-    ctx.check(h2b_keygen_copies_dev(c, N, bp, nbp, k, A, L, lk_d->at(), L ? NL : 0, eq_d->at(), M, const_d->at(), const_idx_d->at(), Mc,
-                                    col(nf - 1), edges.at(), st));
+    ctx.check(h2b_keygen_copies_nf_dev(c, N, bp, nbp, k, F, A, L, lk_d->at(), L ? NL : 0, eq_d->at(), M, const_d->at(), const_idx_d->at(), Mc,
+                                       F ? col(nf - F) : nullptr, edges.at(), st));
     std::memcpy(v, status.download(0, 1)[0].data(), 8);
     builder_panics(s, v[0] & 1, false, v[1], v[0] & 2);
     if (I) {  // the instance copies, after the region's
@@ -90,8 +92,8 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         PolyPtr idx_d;
         upload_bytes(ctx, idx_d, idx.data(), 8 * idx.size());
         Poly inst_status(ctx, (I + 7) / 8);
-        ctx.check(h2b_keygen_instance_edges_dev(c, N, bp, nbp, k, A, L, s.u, I, b.n_instance, idx_d->at(), static_cast<char*>(edges.at()) + 8 * E0,
-                                                static_cast<uint32_t*>(inst_status.at())));
+        ctx.check(h2b_keygen_instance_edges_nf_dev(c, N, bp, nbp, k, F, A, L, s.u, I, b.n_instance, idx_d->at(),
+                                                   static_cast<char*>(edges.at()) + 8 * E0, static_cast<uint32_t*>(inst_status.at())));
         const std::vector<Fr> w = inst_status.download(0, inst_status.len());
         const uint32_t* iv = reinterpret_cast<const uint32_t*>(w[0].data());
         for (size_t m = 0; m < I; m++) {  // the first failing cell in assign_instances' order
@@ -111,7 +113,7 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
     for (size_t i = 0; i < nf; i++) fx[s.fixed_names[i]] = col(i);
     std::vector<const Fr*> sg;
     for (size_t i = 0; i < npc; i++) sg.push_back(static_cast<const Fr*>(sigma.at(i * n)));
-    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg, I);
+    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg, I, F);
     lap(&KeygenTimes::pk);
     // the vk: every fixed column, then every sigma column, committed in Lagrange form, up to 16 MSMs per batch
     std::vector<const void*> cols;

@@ -20,8 +20,10 @@
 //   constants   constant equalities i with value(cell_i) != c_i;
 //   instances[m] rows r of instance column m with value(instance_index_m[r]) != instance_values_m[r].
 // One deliberate difference from halo2's MockProver: a copy failure is counted per violated equality, not per cell against its
-// sigma image; both are zero exactly when every equality holds.  Several constants columns are not covered; the lookup-advice
-// copies of assign_raw hold by construction (the columns are filled from the indices).
+// sigma image; both are zero exactly when every equality holds.  The lookup-advice copies of assign_raw hold by construction (the
+// columns are filled from the indices).  The number F of constants columns (num_fixed) changes no value check, only where the
+// constants fit: D distinct constants need D <= F u (DESIGN.md §4.11), and MockReport::distinct_constants returns D, the number
+// calculate_params sizes num_fixed from.
 #pragma once
 #include <algorithm>
 #include <string>
@@ -65,15 +67,17 @@ struct MockReport {
     std::vector<RawCell> constant_cells;                      // the raw advice cell of every reported constant equality
     std::vector<ReportItem> instances;                        // per instance column: the failing rows
     std::vector<std::vector<RawCell>> instance_cells;         // per instance column: the raw advice cell of every reported row
+    uint64_t distinct_constants = 0;                          // D: the distinct constants among the constant equalities
 };
 
 // ------------------------------------------------------------------------------------------------ what MockProver and keygen share
 // the shape of a builder, checked; messages start with `who`.  max_rows = 2^k - unusable_rows, as calculate_params gets it; it
 // must leave the blinding rows alone (<= 2^k - 7)
 inline CircuitShape builder_shape(const std::string& who, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows,
-                                  size_t I = 0) {
+                                  size_t I = 0, size_t F = 1) {
     if (k < 3 || k > 28) throw Error(H2B_ERR_ARG, who + ": k out of range (3..28)");
-    CircuitShape s(k, A, L, selector_lookup, I);
+    if (F >= (size_t(1) << 32)) throw Error(H2B_ERR_ARG, who + ": too many constants columns");
+    CircuitShape s(k, A, L, selector_lookup, I, F);
     if (A < 1) throw Error(H2B_ERR_ARG, who + ": no gate columns");
     if (s.selector_lookup && A != 1) throw Error(H2B_ERR_ARG, who + ": the selector lookup needs exactly one gate column");
     if (max_rows < 1 || max_rows > s.u) throw Error(H2B_ERR_ARG, who + ": max_rows must be in 1..2^k - 7");
@@ -133,21 +137,27 @@ inline std::vector<uint64_t> builder_break_points(const CircuitShape& s, const s
 }
 
 // halo2-base's panics for what the device found, in the order of the keygen pass: the lookups, then assign_raw (constants
-// placed first, then the equalities resolved)
+// placed first, then the equalities resolved).  assign_raw places distinct constant d at row d div F of constants column
+// d mod F, so the first one that does not fit is d = F u, whose row reaches u: D > F u distinct constants is halo2's
+// NotEnoughRowsAvailable.  calculate_params sizes F by 2^k, not u, so F u < D <= F 2^k fails in halo2-base too.  With F = 0
+// the first constant indexes an empty column list (`config[0]`).
 inline void builder_panics(const CircuitShape& s, bool lookup_unassigned, bool unusable_row, uint64_t distinct_constants, bool equality_unassigned) {
     if (lookup_unassigned) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
     if (unusable_row) throw Error(H2B_ERR_ARG, "range lookup assigned to an unusable row");
-    if (distinct_constants > s.u)
+    if (distinct_constants && s.F == 0) throw Error(H2B_ERR_ARG, "index out of bounds: the len is 0 but the index is 0");
+    if (distinct_constants > s.F * s.u)
         throw Error(H2B_ERR_ARG, "NotEnoughRowsAvailable { current_k: " + std::to_string(s.k) + " }: " + std::to_string(distinct_constants) +
-                                     " distinct constants for the " + std::to_string(s.u) + " usable rows of the constants column");
+                                     " distinct constants for the " + std::to_string(s.F * s.u) + " usable cells of " + std::to_string(s.F) +
+                                     " constants column" + (s.F > 1 ? "s" : ""));
     if (equality_unassigned) throw Error(H2B_ERR_ARG, "virtual cell not assigned");
 }
 
 class MockProver : public CircuitShape {
 public:
-    // max_rows as for builder_shape
-    MockProver(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows, size_t I = 0)
-        : CircuitShape(builder_shape("MockProver", k, A, L, selector_lookup, lookup_bits, max_rows, I)), ctx(ctx), lookup_bits(lookup_bits),
+    // max_rows as for builder_shape; F constants columns
+    MockProver(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits, size_t max_rows, size_t I = 0,
+               size_t F = 1)
+        : CircuitShape(builder_shape("MockProver", k, A, L, selector_lookup, lookup_bits, max_rows, I, F)), ctx(ctx), lookup_bits(lookup_bits),
           max_rows(max_rows) {
         adv = std::make_unique<Poly>(ctx, n * (A + L));
         q = std::make_unique<Poly>(ctx, n * A);
@@ -236,6 +246,7 @@ public:
         const uint32_t* inst_status = reinterpret_cast<const uint32_t*>(raw[rep_elems].data());
         for (size_t m = 0; m < I; m++)
             if (inst_status[m] & 1) throw Error(H2B_ERR_ARG, "instance not assigned");
+        out.distinct_constants = v[5];
         const std::vector<ReportItem> items = decode_reports(raw[1].data(), n_items, max_report, out.satisfied);
         out.gates.assign(items.begin(), items.begin() + A);
         out.lookups.assign(items.begin() + A, items.begin() + A + n_lookups);

@@ -6,8 +6,9 @@
 //
 // Circuit shape (halo2-base `BaseCircuitParams`): A gate-advice columns a0..a{A-1} with selectors q{j} and the vertical
 // gate q (a0 + a1 a2 - a3) (flex_gate/mod.rs:80-91); L lookup-advice columns l0..l{L-1} looked up in `table` as they are
-// (range/mod.rs:131-150), or with L = 0 the selector lookup q_lookup * a0 (range/mod.rs:92-94), or no lookup; one constants
-// column c; I instance columns i0..i{I-1} (BaseConfig::configure, gates/circuit/mod.rs:87-93); equality on [c, a0.., l0.., i0..].
+// (range/mod.rs:131-150), or with L = 0 the selector lookup q_lookup * a0 (range/mod.rs:92-94), or no lookup; F constants
+// columns c, c1..c{F-1} (num_fixed, flex_gate/mod.rs:123-129; F = 0 when the builder uses no constants); I instance columns
+// i0..i{I-1} (BaseConfig::configure, gates/circuit/mod.rs:87-93); equality on [c, c1.., a0.., l0.., i0..].
 // Degree 5 / 4 / 3, permutation sets of degree - 2 columns, degree - 1 pieces of h.  Instance columns are not committed, blinded
 // or opened (KZG: QUERY_INSTANCE = false): their values enter the transcript and the permutation argument only.
 //
@@ -320,19 +321,22 @@ inline Poly* upload_bytes(const Context& ctx, PolyPtr& p, const void* host, size
 }
 
 // ------------------------------------------------------------------------------------------------ the circuit's shape
-// What halo2-base's constraint system is for (k, A, L, selector_lookup, I): the one place the prover, the check, MockProver and
-// keygen read it from.  The selector lookup needs L = 0; blinding factors max(3, queries of a gate column = 4) + 2 = 6.
-// Instance columns change neither the degree nor the blinding factors.
+// What halo2-base's constraint system is for (k, A, L, selector_lookup, I, F): the one place the prover, the check, MockProver
+// and keygen read it from.  The selector lookup needs L = 0; blinding factors max(3, queries of a gate column = 4) + 2 = 6.
+// Instance columns and constants columns change neither the degree nor the blinding factors, only the number of permutation
+// columns (and with it n_sets).  The constants columns enter the permutation first, in the order FlexGateConfig::configure
+// enables equality on them, before the gate advice (the range config's lookup advice comes later).
 struct CircuitShape {
-    CircuitShape(uint32_t k, size_t A, size_t L, bool selector_lookup, size_t I = 0)
-        : k(k), n(size_t(1) << k), A(A), L(L), I(I), selector_lookup(selector_lookup && L == 0) {
+    CircuitShape(uint32_t k, size_t A, size_t L, bool selector_lookup, size_t I = 0, size_t F = 1)
+        : k(k), n(size_t(1) << k), A(A), L(L), I(I), F(F), selector_lookup(selector_lookup && L == 0) {
         degree = L ? 4 : (this->selector_lookup ? 5 : 3);
         chunk = degree - 2;
         ext_k = k + (degree == 3 ? 1 : 2);
         u = n - (bf + 1);
         for (size_t j = 0; j < A; j++) adv_names.push_back("a" + std::to_string(j));
         for (size_t t = 0; t < L; t++) adv_names.push_back("l" + std::to_string(t));
-        perm_cols.push_back("c");
+        for (size_t f = 0; f < F; f++) const_names.push_back(f ? "c" + std::to_string(f) : "c");
+        perm_cols = const_names;
         perm_cols.insert(perm_cols.end(), adv_names.begin(), adv_names.end());
         for (size_t m = 0; m < I; m++) inst_names.push_back("i" + std::to_string(m));
         perm_cols.insert(perm_cols.end(), inst_names.begin(), inst_names.end());
@@ -341,16 +345,19 @@ struct CircuitShape {
         for (size_t j = 0; j < A; j++) fixed_names.push_back("q" + std::to_string(j));
         if (this->selector_lookup) fixed_names.push_back("q_lookup");
         if (n_lookups) fixed_names.push_back("table");
-        fixed_names.push_back("c");
+        fixed_names.insert(fixed_names.end(), const_names.begin(), const_names.end());
         for (auto& nm : perm_cols) sigma_names.push_back("sigma_" + nm);
     }
+    // a permutation column that is a constants column (fixed: it lives in the circuit, not in the session)
+    bool is_const(const std::string& nm) const { return std::find(const_names.begin(), const_names.end(), nm) != const_names.end(); }
     uint32_t k, ext_k = 0;
-    size_t n, A, L, I;
+    size_t n, A, L, I, F;
     bool selector_lookup;
     size_t degree = 0, chunk = 0, n_sets = 0, n_lookups = 0, u = 0;
     uint32_t bf = 6;
-    // adv: a0.., l0..;  inst: i0..;  perm: c, adv, inst;  fixed: q0.., [q_lookup], [table], c;  sigma: sigma_{perm}
-    std::vector<std::string> adv_names, inst_names, perm_cols, fixed_names, sigma_names;
+    // adv: a0.., l0..;  inst: i0..;  const: c, c1..;  perm: const, adv, inst;  fixed: q0.., [q_lookup], [table], const;
+    // sigma: sigma_{perm}
+    std::vector<std::string> adv_names, inst_names, const_names, perm_cols, fixed_names, sigma_names;
 };
 
 // the vertical gate q (a0 + a1 a2 - a3) on fixed and advice slot `slot`, advice rotations 0..3 (flex_gate/mod.rs:80-91)
@@ -365,26 +372,26 @@ inline ValueSource add_vertical_gate(GraphEvaluator& ev, uint32_t slot) {
 // ------------------------------------------------------------------------------------------------ the fixed side of a circuit
 class ProverCircuit : public CircuitShape {
 public:
-    // fixed: Lagrange values (2^k each) by name — q0..q{A-1}, [q_lookup], [table], c; sigma: one column per permutation column
-    // in the order [c, a0.., l0.., i0..] (I instance columns)
+    // fixed: Lagrange values (2^k each) by name — q0..q{A-1}, [q_lookup], [table], c, c1..c{F-1}; sigma: one column per
+    // permutation column in the order [c, c1.., a0.., l0.., i0..] (F constants columns, I instance columns)
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, std::vector<Fr>>& fixed,
-                  const std::vector<std::vector<Fr>>& sigma, size_t I = 0)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k), false, I) {}
+                  const std::vector<std::vector<Fr>>& sigma, size_t I = 0, size_t F = 1)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k), false, I, F) {}
     // the same with every column as a pointer to its 2^k rows (nothing is copied on the host)
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
-                  const std::vector<const Fr*>& sigma, size_t I = 0)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false, I) {}
+                  const std::vector<const Fr*>& sigma, size_t I = 0, size_t F = 1)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false, I, F) {}
     // the same with every column as a DEVICE pointer to its 2^k Lagrange values (keygen on the device, h2b200_keygen.hpp): each is
     // copied on the device, then transformed as above
     struct OnDevice {};
     ProverCircuit(OnDevice, const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup,
-                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma, size_t I = 0)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true, I) {}
+                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma, size_t I = 0, size_t F = 1)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true, I, F) {}
 
 private:
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
-                  const std::vector<const Fr*>& sigma, bool on_device, size_t I)
-        : CircuitShape(k, A, L, selector_lookup, I), ctx(ctx) {
+                  const std::vector<const Fr*>& sigma, bool on_device, size_t I, size_t F)
+        : CircuitShape(k, A, L, selector_lookup, I, F), ctx(ctx) {
         if (sigma.size() != perm_cols.size()) throw Error(H2B_ERR_ARG, "ProverCircuit: one sigma column per permutation column");
         std::vector<Fr> l0(n, Fr{}), ll(n, Fr{}), la(n, Fr{});
         l0[0] = HostFr::one();
@@ -818,7 +825,7 @@ public:
         res.gamma = tr.squeeze();
         side_transforms(perm_names);
         // ---- product columns + the vanishing argument's random polynomial
-        auto col_lagr = [&](const std::string& nm) -> void* { return nm == "c" ? cs.lagr.at("c")->at() : lagr[nm].ptr(); };
+        auto col_lagr = [&](const std::string& nm) -> void* { return cs.is_const(nm) ? cs.lagr.at(nm)->at() : lagr[nm].ptr(); };
         for (size_t s = 0; s < cs.n_sets; s++) {
             std::vector<const void*> cols, sig;
             for (size_t i = s * cs.chunk; i < std::min(cs.perm_cols.size(), (s + 1) * cs.chunk); i++) {
@@ -864,7 +871,7 @@ public:
             std::vector<const void*> tz, tc, ts;
             for (size_t s = 0; s < cs.n_sets; s++) tz.push_back(ext["zp" + std::to_string(s)]->at());
             for (auto& nm : cs.perm_cols) {
-                tc.push_back(nm == "c" ? cs.ext.at("c")->at() : ext[nm]->at());
+                tc.push_back(cs.is_const(nm) ? cs.ext.at(nm)->at() : ext[nm]->at());
                 ts.push_back(cs.ext.at("sigma_" + nm)->at());
             }
             ctx.check(h2b_permutation_fold_dev(c, tz.data(), cs.n_sets, tc.data(), ts.data(), tc.size(), cs.chunk, cs.ext.at("l0")->at(),
@@ -1043,7 +1050,8 @@ public:
             }
             check_lookup_dev(ctx, in, cs.lagr.at("table")->at(), k, u, max_report, at(A + t));
         }
-        std::vector<const void*> cols{cs.lagr.at("c")->at()};
+        std::vector<const void*> cols;
+        for (auto& nm : cs.const_names) cols.push_back(cs.lagr.at(nm)->at());
         for (auto& nm : cs.adv_names) cols.push_back(lagr[nm].ptr());
         for (auto& nm : cs.inst_names) cols.push_back(lagr[nm].ptr());
         check_copies_dev(ctx, cols, cs.check_map->at(), k, max_report, at(A + cs.n_lookups));
