@@ -155,6 +155,8 @@ SIGNATURES = {
     "h2b_eval_polynomial_dev": (_int, [_vp, _vp, _sz, _vp, _vp]),
     "h2b_kate_division": (_int, [_vp, _vp, _sz, _vp, _vp]),
     "h2b_kate_division_dev": (_int, [_vp, _vp, _sz, _vp, _vp]),
+    "h2b_kate_division_multi": (_int, [_vp, _vp, _sz, _vp, _sz, _vp, _vp]),
+    "h2b_kate_division_multi_dev": (_int, [_vp, _vp, _sz, _vp, _sz, _vp, _vp]),
     "h2b_poly_lincomb": (_int, [_vp, _vpp, _vp, _sz, _sz, _vp]),
     "h2b_poly_lincomb_dev": (_int, [_vp, _vpp, _vp, _sz, _sz, _vp]),
     "h2b_poly_alloc": (_int, [_vp, _sz, C.POINTER(_vp)]),
@@ -212,6 +214,7 @@ PROVER_SIGNATURES = {
     "h2bp_session_column": (_int, [_vp, C.c_char_p, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
     "h2bp_session_shard": (_int, [_vp, _sz, _sz, ALLREDUCE_FN, _vp]),
     "h2bp_prove": (_int, [_vp, _witp, _vp, BLIND_FN, _vp, COMMIT_FN, _vp, _vp, _vp, _vp, _vp]),
+    "h2bp_prove_halo2": (_int, [_vp, _witp, _vp, BLIND_FN, _vp, _vp, _vp, _sz, C.POINTER(_sz)]),
     "h2bp_check": (_int, [_vp, _witp, _sz, _vp]),
     "h2bp_mock_create": (_int, [_vp, _u32, _sz, _sz, _int, _u32, _sz, _sz, _sz, C.POINTER(_vp), _u64s]),
     "h2bp_mock_free": (None, [_vp]),

@@ -1509,6 +1509,27 @@ int h2b_kate_division(h2b_ctx* ctx, const uint64_t* a, size_t n, const uint64_t 
         st.finish();
     });
 }
+int h2b_kate_division_multi_dev(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t* points, size_t m, const uint64_t* weights,
+                                void* d_q) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_a && points && weights && (d_q || n <= 1), "kate_division_multi: null pointer");
+        H2B_REQUIRE(d_a != d_q, "kate_division_multi: q must not alias a");
+        kate_division_multi_run(ctx, d_a, n, points, m, weights, d_q);
+    });
+}
+int h2b_kate_division_multi(h2b_ctx* ctx, const uint64_t* a, size_t n, const uint64_t* points, size_t m, const uint64_t* weights,
+                            uint64_t* q) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(a && points && weights && (q || n <= 1), "kate_division_multi: null pointer");
+        H2B_REQUIRE(n >= 1, "kate_division_multi: empty polynomial");  // before (n - 1) sizes the output
+        H2B_REQUIRE(m >= 1 && m <= H2B_KATE_MULTI_MAX, "kate_division_multi: 1..4 points");
+        if (n == 1) return;
+        Staging st(ctx, WS_ASSIGN_IN, 2 * n * 32);
+        void *d_a = st.up(a, n * 32), *d_q = st.out(q, (n - 1) * 32, n * 32);
+        kate_division_multi_run(ctx, d_a, n, points, m, weights, d_q);
+        st.finish();
+    });
+}
 int h2b_poly_lincomb_dev(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* scalars, size_t m, size_t n, void* d_out) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(d_polys && scalars && (d_out || n == 0), "poly_lincomb: null pointer");

@@ -301,6 +301,7 @@ void g1_compress_run(h2b_ctx* ctx, const void* d_xy, size_t n, void* d_bytes);
 void eval_polynomial_run(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t x[4], void* d_out);
 void eval_polynomial_batch_run(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* xs, size_t m, size_t n, void* d_out);
 void kate_division_run(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t z[4], void* d_q);
+void kate_division_multi_run(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t* points, size_t m, const uint64_t* weights, void* d_q);
 void poly_lincomb_run(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* scalars, size_t m, size_t n, void* d_out);
 // ---- scan.cu
 void batch_invert_run(h2b_ctx* ctx, void* d_a, size_t n);

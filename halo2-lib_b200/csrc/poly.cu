@@ -65,9 +65,8 @@ __global__ void __launch_bounds__(256) k_pd_tiles(const uint64_t* __restrict__ a
 }
 
 // carry[b] = V((b + 1) * TILE) = sum over the tiles above b; single CTA.  total = V(0) = a(x).
-__global__ void __launch_bounds__(256) k_pd_scan(const uint64_t* __restrict__ tile_val, u32 ntiles, const uint64_t* __restrict__ pw,
-                                                 uint64_t* __restrict__ carry, uint64_t* __restrict__ total) {
-    __shared__ Fr sh[256];
+__device__ __forceinline__ void pd_scan_block(const uint64_t* __restrict__ tile_val, u32 ntiles, const uint64_t* __restrict__ pw,
+                                              uint64_t* __restrict__ carry, uint64_t* __restrict__ total, Fr* sh /* 256 */) {
     const u32 per = (ntiles + 255) / 256;
     const u32 lo = min(threadIdx.x * per, ntiles), hi = min(lo + per, ntiles);
     const Fr xt = Fr::load_nc(pw + 4 * 11);  // x^2048
@@ -89,6 +88,11 @@ __global__ void __launch_bounds__(256) k_pd_scan(const uint64_t* __restrict__ ti
         run = Fr::load_nc(tile_val + 4 * (size_t)(j - 1)) + xt * run;
     }
     if (threadIdx.x == 0 && total) d.store(total);
+}
+__global__ void __launch_bounds__(256) k_pd_scan(const uint64_t* __restrict__ tile_val, u32 ntiles, const uint64_t* __restrict__ pw,
+                                                 uint64_t* __restrict__ carry, uint64_t* __restrict__ total) {
+    __shared__ Fr sh[256];
+    pd_scan_block(tile_val, ntiles, pw, carry, total, sh);
 }
 
 // q[i - 1] = V(i) for 1 <= i < n
@@ -147,6 +151,113 @@ void kate_division_run(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t z
     u32 ntiles;
     pd_prepare(ctx, d_a, n, z, &pw, &tv, &carry, &total, &ntiles);
     H2B_LAUNCH(ctx, k_pd_apply, ntiles, 256, 0, (const uint64_t*)d_a, n, pw, carry, (uint64_t*)d_q);
+}
+
+// ---------------------------------------------------------------- division by a vanishing polynomial of m <= 4 points
+// (a - r) / Z_T = sum_j w_j (a - a(z_j)) / (X - z_j),  Z_T = prod_j (X - z_j),  w_j = 1 / prod_{k != j} (z_j - z_k):
+// the quotient of a by Z_T is a weighted sum of m kate_division quotients, i.e. of m independent suffix recurrences
+// V_j(p) = a_p + z_j V_j(p + 1).  The passes of kate_division run for all m points at once: each CTA reads its tile of a
+// once and carries m values; the apply pass writes the weighted sum once.
+struct DivPoints {
+    Fr z[H2B_KATE_MULTI_MAX], w[H2B_KATE_MULTI_MAX];
+};
+// pw[j] = the 12 powers z_j^(2^i) (as k_pow2_table), one thread per point
+__global__ void k_pdm_pow2(DivPoints p, u32 m, uint64_t* __restrict__ pw) {
+    if (threadIdx.x >= m) return;
+    Fr x = p.z[threadIdx.x];
+    for (int i = 0; i < 12; i++) {
+        x.store(pw + 48 * threadIdx.x + 4 * i);
+        x = x.sqr();
+    }
+}
+// tile_val[j][b] as k_pd_tiles for every point
+template <int M>
+__global__ void __launch_bounds__(256) k_pdm_tiles(const uint64_t* __restrict__ a, size_t n, u32 ntiles, const uint64_t* __restrict__ pw,
+                                                   uint64_t* __restrict__ tile_val) {
+    __shared__ Fr sh[256];
+    const size_t base = (size_t)blockIdx.x * PD_TILE + (size_t)threadIdx.x * 8;
+    Fr v[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) v[j] = (base + j < n) ? Fr::load_nc(a + 4 * (base + j)) : Fr::zero();
+#pragma unroll 1
+    for (int j = 0; j < M; j++) {
+        const Fr x = Fr::load_nc(pw + 48 * j), x8 = Fr::load_nc(pw + 48 * j + 4 * 3);
+        Fr d = block_suffix_affine(chunk_value(v, x), x8, sh);
+        if (threadIdx.x == 0) d.store(tile_val + 4 * ((size_t)j * ntiles + blockIdx.x));
+        __syncthreads();  // the next point's scan rewrites sh
+    }
+}
+// carry[j][b] as k_pd_scan, one CTA per point
+__global__ void __launch_bounds__(256) k_pdm_scan(const uint64_t* __restrict__ tile_val, u32 ntiles, const uint64_t* __restrict__ pw,
+                                                  uint64_t* __restrict__ carry) {
+    __shared__ Fr sh[256];
+    const size_t j = blockIdx.x;
+    pd_scan_block(tile_val + 4 * j * ntiles, ntiles, pw + 48 * j, carry + 4 * j * ntiles, nullptr, sh);
+}
+// q[i - 1] = sum_j w_j V_j(i) for 1 <= i < n
+template <int M>
+__global__ void __launch_bounds__(256) k_pdm_apply(const uint64_t* __restrict__ a, size_t n, u32 ntiles, const uint64_t* __restrict__ pw,
+                                                   const uint64_t* __restrict__ carry, DivPoints p, uint64_t* __restrict__ q) {
+    __shared__ Fr sh[256];
+    const size_t base = (size_t)blockIdx.x * PD_TILE + (size_t)threadIdx.x * 8;
+    Fr v[8], acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        v[j] = (base + j < n) ? Fr::load_nc(a + 4 * (base + j)) : Fr::zero();
+        acc[j] = Fr::zero();
+    }
+#pragma unroll 1
+    for (int j = 0; j < M; j++) {
+        const Fr x = Fr::load_nc(pw + 48 * j), x8 = Fr::load_nc(pw + 48 * j + 4 * 3);
+        const Fr cin = Fr::load_nc(carry + 4 * ((size_t)j * ntiles + blockIdx.x));
+        Fr c = chunk_value(v, x);
+        if (threadIdx.x == 255) c = c + x8 * cin;
+        block_suffix_affine(c, x8, sh);
+        Fr run = (threadIdx.x == 255) ? cin : Fr::load(sh + threadIdx.x + 1);
+        __syncthreads();  // every thread has read sh before the next point's scan rewrites it
+        const Fr w = p.w[j];
+#pragma unroll
+        for (int t = 7; t >= 0; t--) {
+            run = v[t] + x * run;
+            acc[t] = acc[t] + w * run;
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < 8; t++) {
+        const size_t i = base + t;
+        if (i >= 1 && i < n) acc[t].store(q + 4 * (i - 1));
+    }
+}
+
+template <int M>
+static void kate_division_multi_launch(h2b_ctx* ctx, const uint64_t* a, size_t n, u32 ntiles, uint64_t* pw, uint64_t* tv, uint64_t* carry,
+                                       const DivPoints& p, uint64_t* q) {
+    H2B_LAUNCH(ctx, k_pdm_tiles<M>, ntiles, 256, 0, a, n, ntiles, pw, tv);
+    H2B_LAUNCH(ctx, k_pdm_scan, M, 256, 0, tv, ntiles, pw, carry);
+    H2B_LAUNCH(ctx, k_pdm_apply<M>, ntiles, 256, 0, a, n, ntiles, pw, carry, p, q);
+}
+
+void kate_division_multi_run(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t* points, size_t m, const uint64_t* weights, void* d_q) {
+    H2B_REQUIRE(n >= 1, "kate_division_multi: empty polynomial");
+    H2B_REQUIRE(m >= 1 && m <= H2B_KATE_MULTI_MAX, "kate_division_multi: 1..4 points");
+    if (n == 1) return;
+    DivPoints p;
+    memset(&p, 0, sizeof(p));
+    memcpy(p.z, points, 32 * m);
+    memcpy(p.w, weights, 32 * m);
+    const u32 ntiles = (u32)((n + PD_TILE - 1) / PD_TILE);
+    uint64_t* pw = (uint64_t*)ctx->get(WS_MISC2, 32 * (12 * m + 2 * m * (size_t)ntiles));
+    uint64_t* tv = pw + 48 * m;
+    uint64_t* carry = tv + 4 * m * (size_t)ntiles;
+    H2B_LAUNCH(ctx, k_pdm_pow2, 1, 32, 0, p, (u32)m, pw);
+    const uint64_t* a = (const uint64_t*)d_a;
+    uint64_t* q = (uint64_t*)d_q;
+    switch (m) {
+        case 1: kate_division_multi_launch<1>(ctx, a, n, ntiles, pw, tv, carry, p, q); break;
+        case 2: kate_division_multi_launch<2>(ctx, a, n, ntiles, pw, tv, carry, p, q); break;
+        case 3: kate_division_multi_launch<3>(ctx, a, n, ntiles, pw, tv, carry, p, q); break;
+        default: kate_division_multi_launch<4>(ctx, a, n, ntiles, pw, tv, carry, p, q); break;
+    }
 }
 
 // ---------------------------------------------------------------- batched evaluation

@@ -204,6 +204,28 @@ H2BP_API int h2bp_prove(BoundSession* b, const WitnessView* w, const uint64_t* r
     });
 }
 
+// one proof in halo2's form (ProverSession::create_proof_halo2): vk_repr (Montgomery, 4 limbs) absorbed first; the proof bytes
+// go to `proof` (capacity `cap` bytes), their number to *len
+H2BP_API int h2bp_prove_halo2(BoundSession* b, const WitnessView* w, const uint64_t* random_poly, h2bp_blind_fn blind, void* blind_user,
+                              const uint64_t* vk_repr, uint8_t* proof, size_t cap, size_t* len) {
+    return run(b ? b->ctx.raw() : nullptr, [&] {
+        if (!w || !blind || !vk_repr || !proof || !len) throw Error(H2B_ERR_ARG, "prove_halo2: null argument");
+        ProverSession& s = b->sess;
+        s.observer = nullptr;
+        auto source = [&](size_t rows) {
+            std::vector<Fr> out(rows);
+            if (blind(blind_user, rows, out[0].data())) throw Error(H2B_ERR_ARG, "the blinding callback failed");
+            return out;
+        };
+        Fr repr;
+        std::memcpy(repr.data(), vk_repr, 32);
+        const std::vector<uint8_t> bytes = s.create_proof_halo2(*w, reinterpret_cast<const Fr*>(random_poly), source, repr);
+        if (bytes.size() > cap) throw Error(H2B_ERR_ARG, "prove_halo2: the proof needs " + std::to_string(bytes.size()) + " bytes");
+        std::memcpy(proof, bytes.data(), bytes.size());
+        *len = bytes.size();
+    });
+}
+
 // the constraint check.  report: max_report + 1 words per gate column, lookup and permutation column (in that order, instance
 // columns last): the failure count, then the first min(count, max_report) failing rows ascending
 H2BP_API int h2bp_check(BoundSession* b, const WitnessView* w, size_t max_report, uint64_t* report) {

@@ -53,8 +53,8 @@ __global__ void __launch_bounds__(128) k_g1_decompress(const uint8_t* __restrict
     Fq x;
     x.l[0] = lo.x; x.l[1] = lo.y; x.l[2] = lo.z; x.l[3] = lo.w;
     x.l[4] = hi.x; x.l[5] = hi.y; x.l[6] = hi.z; x.l[7] = hi.w;
-    const bool inf = (x.l[7] >> 31) & 1, odd = (x.l[7] >> 30) & 1;
-    x.l[7] &= 0x3fffffffu;
+    const bool inf = x.l[7] & (H2B_G1_FLAG_IDENTITY << 24), odd = x.l[7] & (H2B_G1_FLAG_Y_ODD << 24);
+    x.l[7] &= ~((H2B_G1_FLAG_IDENTITY | H2B_G1_FLAG_Y_ODD) << 24);
     Affine r;
     r.x = Fq::zero();
     r.y = Fq::zero();
@@ -92,11 +92,11 @@ __global__ void __launch_bounds__(256) k_g1_compress(const Affine* __restrict__ 
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const Affine p = Affine::load(pts + i);
-    uint4 lo = make_uint4(0, 0, 0, 0), hi = make_uint4(0, 0, 0, 0x80000000u);
+    uint4 lo = make_uint4(0, 0, 0, 0), hi = make_uint4(0, 0, 0, H2B_G1_FLAG_IDENTITY << 24);
     if (!p.is_identity()) {
         const Fq x = p.x.from_mont(), y = p.y.from_mont();
         lo = make_uint4(x.l[0], x.l[1], x.l[2], x.l[3]);
-        hi = make_uint4(x.l[4], x.l[5], x.l[6], x.l[7] | ((y.l[0] & 1u) << 30));
+        hi = make_uint4(x.l[4], x.l[5], x.l[6], x.l[7] | ((y.l[0] & 1u) ? H2B_G1_FLAG_Y_ODD << 24 : 0u));
     }
     uint4* q = reinterpret_cast<uint4*>(bytes + 32 * i);
     q[0] = lo;

@@ -512,6 +512,23 @@ class ProverSession:
                 "challenges": dict(zip(("theta", "beta", "gamma", "y", "x"), (from_limbs(c) for c in ch))),
                 "h2d_bytes": int(nbytes[0]), "d2h_bytes": int(nbytes[1])}
 
+    def gen_proof(self, witness_ptr: int, n_cells: int, random_poly_ptr: int, vk_repr: int, instances=None, seed: int = 0, break_points=None,
+                  lookup_ptr: int = 0, n_lookup: int = 0, rational_index_ptr: int = 0, rational_den_ptr: int = 0, n_rational: int = 0,
+                  lookup_index_ptr: int = 0) -> bytes:
+        """The proof bytes halo2-base's gen_proof_with_instances returns (transcript.finalize() of halo2's Blake2bWrite), for the
+        witness as `prove` takes it: the same device phases up to the h pieces, then halo2's evaluations and ProverSHPLONK
+        (h2b::ProverSession::create_proof_halo2).  vk_repr: the verifying key's transcript_repr as a canonical integer (vk.hash_into
+        absorbs it first); instances: the public values as for `prove`.  Blinding scalars as for `prove` (`seed`, `blind_source`)."""
+        w, keep = self._witness("gen_proof", witness_ptr, n_cells, break_points, lookup_ptr, n_lookup, rational_index_ptr, rational_den_ptr,
+                                n_rational, lookup_index_ptr, instances)
+        self._rng = np.random.default_rng(seed)
+        repr_limbs = to_limbs(vk_repr)
+        cap = 32 * (self.n_commitments + len(self.queries) + 8)  # halo2's proof holds fewer points and scalars than `prove` returns
+        out, n = np.zeros(cap, dtype=np.uint8), C.c_size_t()
+        self._done(lib.h2bp_prove_halo2(self._h, C.byref(w), C.c_void_p(random_poly_ptr), self._blind_cb, None, C.c_void_p(repr_limbs.ctypes.data),
+                                        C.c_void_p(out.ctypes.data), cap, C.byref(n)))
+        return out[:n.value].tobytes()
+
     def free(self):
         if self._h:
             lib.h2bp_session_free(self._h)

@@ -142,6 +142,8 @@ int h2b_params_raw_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g
  * 64 B g2, 64 B s_g2).  h2b_srs_read_processed: the device side of `ParamsKZG::read` — decompress the shard
  * [begin, begin + count) (count = 0: everything) of both bases and build the SRS handle; H2B_ERR_ARG if the image is
  * malformed or holds an invalid encoding. */
+#define H2B_G1_FLAG_IDENTITY 128u /* the flag bits of byte 31 of a compressed G1 point */
+#define H2B_G1_FLAG_Y_ODD 64u
 int h2b_g1_decompress(h2b_ctx* ctx, const uint8_t* bytes, size_t n, uint64_t* out_xy, size_t* invalid);
 int h2b_g1_decompress_dev(h2b_ctx* ctx, const void* d_bytes, size_t n, void* d_out_xy, size_t* invalid);
 int h2b_params_processed_view(const uint8_t* bytes, size_t len, uint32_t* k, size_t* g_offset, size_t* g_lagrange_offset,
@@ -519,6 +521,15 @@ int h2b_eval_polynomial_dev(h2b_ctx* ctx, const void* d_coeffs, size_t n, const 
  * as `kate_division(a, z)` does. */
 int h2b_kate_division(h2b_ctx* ctx, const uint64_t* a, size_t n, const uint64_t z[4], uint64_t* q);
 int h2b_kate_division_dev(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t z[4], void* d_q);
+/* quotient of a(X) (n coefficients, n >= 1) by Z_T(X) = prod_j (X - points[j]) for 1 <= m <= H2B_KATE_MULTI_MAX distinct
+ * points, the remainder dropped (SHPLONK's div_by_vanishing), in one pass: q = sum_j weights[j] (a - a(z_j)) / (X - z_j) with
+ * weights[j] = 1 / prod_{k != j} (z_j - z_k), which the caller supplies (points, weights: m x 4 limbs, host).  q has n - 1
+ * coefficients, as kate_division writes them; those from n - m on are zero.  With m = 1 and weight 1 it is kate_division. */
+#define H2B_KATE_MULTI_MAX 4
+int h2b_kate_division_multi(h2b_ctx* ctx, const uint64_t* a, size_t n, const uint64_t* points, size_t m, const uint64_t* weights,
+                            uint64_t* q);
+int h2b_kate_division_multi_dev(h2b_ctx* ctx, const void* d_a, size_t n, const uint64_t* points, size_t m, const uint64_t* weights,
+                                void* d_q);
 /* out[i] = sum_j scalars[j] * polys[j][i], i < n, j < m (1 <= m <= 32); out may alias one of the inputs */
 int h2b_poly_lincomb(h2b_ctx* ctx, const uint64_t* const* polys, const uint64_t* scalars, size_t m, size_t n, uint64_t* out);
 int h2b_poly_lincomb_dev(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* scalars, size_t m, size_t n, void* d_out);

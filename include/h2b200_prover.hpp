@@ -98,6 +98,19 @@ struct HostField {
         if (carry || geq_mod(r)) sub_mod(r);
         return {r[0], r[1], r[2], r[3]};
     }
+    static E neg(const E& a) {
+        if (is_zero(a)) return a;
+        uint64_t r[4] = {P::MOD[0], P::MOD[1], P::MOD[2], P::MOD[3]};
+        unsigned __int128 borrow = 0;
+        for (int i = 0; i < 4; i++) {
+            unsigned __int128 t = (unsigned __int128)r[i] - a[i] - (uint64_t)borrow;
+            r[i] = (uint64_t)t;
+            borrow = (t >> 64) & 1;
+        }
+        return {r[0], r[1], r[2], r[3]};
+    }
+    static E sub(const E& a, const E& b) { return add(a, neg(b)); }
+    static E to_canonical(const E& a) { return mul(a, {1, 0, 0, 0}); }  // a R^-1: the value itself, little-endian limbs
     static E from_canonical(const uint64_t c[4]) { return mul({c[0], c[1], c[2], c[3]}, {P::R2[0], P::R2[1], P::R2[2], P::R2[3]}); }
     static E pow(E base, uint64_t e) {
         E acc = one();
@@ -176,6 +189,13 @@ public:
         for (int i = 0; i < 8; i++) h_[i] = IV[i];
         h_[0] ^= 0x01010000ULL ^ 64;  // digest length 64, no key
     }
+    // the same with the 16-byte personalization of the parameter block (bytes 48..63, i.e. h[6], h[7])
+    explicit Blake2b(const uint8_t personal[16]) : Blake2b() {
+        uint64_t p[2];
+        std::memcpy(p, personal, 16);
+        h_[6] ^= p[0];
+        h_[7] ^= p[1];
+    }
     void update(const void* data, size_t len) {
         const uint8_t* p = static_cast<const uint8_t*>(data);
         while (len) {
@@ -250,9 +270,77 @@ public:
         h_.update(&zero, 1);
         return HostFr::from_wide_bytes(d.data());
     }
+    // the writer interface ProverSession's shared phases use: m commitments (affine, Montgomery), m public values
+    void write_points(const G1* p, size_t m) { absorb(p, m * sizeof(G1)); }
+    void common_scalars(const Fr* v, size_t m) { absorb(v, m * sizeof(Fr)); }
 
 private:
     Blake2b h_;
+};
+
+// SerdeFormat::Processed encoding of an affine point (Montgomery; the identity (0, 0)): canonical x little-endian and the
+// flag bits of include/h2b200.h in byte 31 — the encoding h2b_g1_compress writes and h2b_g1_decompress reads
+inline std::array<uint8_t, 32> g1_compress_host(const G1& p) {
+    std::array<uint8_t, 32> out{};
+    if (HostFq::is_zero(p.x) && HostFq::is_zero(p.y)) {
+        out[31] = H2B_G1_FLAG_IDENTITY;
+        return out;
+    }
+    const Fq x = HostFq::to_canonical(p.x), y = HostFq::to_canonical(p.y);
+    std::memcpy(out.data(), x.data(), 32);
+    if (y[0] & 1) out[31] |= H2B_G1_FLAG_Y_ODD;
+    return out;
+}
+
+// halo2's Blake2bWrite<_, G1Affine, Challenge255> (transcript.rs, recalled from halo2-axiom 0.5.3): Blake2b-512 personalized
+// "Halo2-Transcript"; a point enters as 1 || x || y (canonical little-endian, the identity is an error), a scalar as 2 || its
+// canonical bytes, a challenge is 0 absorbed, then the digest of the state as a 512-bit little-endian integer mod r.
+// write_point / write_scalar also append the 32-byte encoding (g1_compress_host / canonical) to the proof.
+class Blake2bWrite {
+public:
+    Blake2bWrite() : h_(reinterpret_cast<const uint8_t*>("Halo2-Transcript")) {}
+    void common_point(const G1& p) {
+        if (HostFq::is_zero(p.x) && HostFq::is_zero(p.y)) throw Error(H2B_ERR_ARG, "Blake2bWrite: the identity cannot enter the transcript");
+        const uint8_t prefix = 1;
+        const Fq x = HostFq::to_canonical(p.x), y = HostFq::to_canonical(p.y);
+        h_.update(&prefix, 1);
+        h_.update(x.data(), 32);
+        h_.update(y.data(), 32);
+    }
+    void common_scalar(const Fr& v) {
+        const uint8_t prefix = 2;
+        const Fr c = HostFr::to_canonical(v);
+        h_.update(&prefix, 1);
+        h_.update(c.data(), 32);
+    }
+    void write_point(const G1& p) {
+        common_point(p);
+        const auto b = g1_compress_host(p);
+        out_.insert(out_.end(), b.begin(), b.end());
+    }
+    void write_scalar(const Fr& v) {
+        common_scalar(v);
+        const Fr c = HostFr::to_canonical(v);
+        const uint8_t* b = reinterpret_cast<const uint8_t*>(c.data());
+        out_.insert(out_.end(), b, b + 32);
+    }
+    Fr squeeze() {
+        const uint8_t prefix = 0;
+        h_.update(&prefix, 1);
+        return HostFr::from_wide_bytes(h_.digest().data());
+    }
+    void write_points(const G1* p, size_t m) {
+        for (size_t i = 0; i < m; i++) write_point(p[i]);
+    }
+    void common_scalars(const Fr* v, size_t m) {
+        for (size_t i = 0; i < m; i++) common_scalar(v[i]);
+    }
+    // the proof: what transcript.finalize() returns
+    const std::vector<uint8_t>& finalize() const { return out_; }
+
+private:
+    Blake2b h_;
+    std::vector<uint8_t> out_;
 };
 
 // ------------------------------------------------------------------------------------------------ device polynomials
@@ -705,213 +793,18 @@ public:
     }
     // random_poly: n coefficients in pinned host memory (uploaded asynchronously beside phase 0)
     Proof create_proof(const WitnessView& wit, const Fr* random_poly, const BlindSource& blind) {
-        const uint32_t k = cs.k, ext_k = cs.ext_k, bf = cs.bf;
-        const size_t n = cs.n, u = cs.u, L = cs.L;
+        const size_t n = cs.n;
         h2b_ctx* c = ctx.raw();
         Transcript tr;
         Proof res;
-        check_inputs(wit, "create_proof", cs);
-        if (!random_poly) throw Error(H2B_ERR_ARG, "create_proof: null random polynomial");
-        uint64_t verdict = 0;  // phase 0: the verdict words, read with the first download of its commitments
-        auto commit = [&](const std::vector<std::pair<int, ColRef>>& items, bool absorb, bool with_verdict = false) {
-            for (size_t lo = 0; lo < items.size(); lo += 16) {
-                const size_t m = std::min<size_t>(16, items.size() - lo);
-                std::vector<const void*> ptrs(m);
-                std::vector<int> bs(m);
-                for (size_t i = 0; i < m; i++) { bs[i] = items[lo + i].first; ptrs[i] = items[lo + i].second.ptr(shard_begin); }
-                ctx.check(h2b_msm_g1_batch_dev(c, params.raw(), bs.data(), ptrs.data(), m, n_loc, d_out->at()));
-                if (allreduce) allreduce(d_out->at(), m);
-                if (observer) {
-                    ctx.check(h2b_ctx_synchronize(c));
-                    for (size_t i = 0; i < m; i++) observer(bs[i], items[lo + i].second.poly->download(items[lo + i].second.offset, n));
-                }
-                const size_t cnt = with_verdict && lo == 0 ? 49 : m * 3;
-                std::vector<G1> out(m);
-                if (cnt == 49) {
-                    std::vector<Fr> raw = d_out->download(0, 49);
-                    std::memcpy(out[0].x.data(), raw.data(), m * sizeof(G1));
-                    verdict = raw[48][0];
-                } else {
-                    ctx.check(h2b_poly_download(c, d_out->raw(), 0, out[0].x.data(), m * 3));
-                }
-                res.d2h_bytes += cnt * 32;
-                g1_normalize_host_batch(out.data(), m);  // affine form: what the transcript and the proof hold
-                if (absorb) tr.absorb(out.data(), m * sizeof(G1));
-                res.commitments.insert(res.commitments.end(), out.begin(), out.end());
-            }
-        };
-        auto blind_col = [&](const ColRef& col, size_t first_row) {
-            const std::vector<Fr> b = blind(n - first_row);
-            if (b.size() != n - first_row) throw Error(H2B_ERR_ARG, "blind source returned the wrong number of rows");
-            ctx.check(h2b_poly_upload(c, col.poly->raw(), col.offset + first_row, b[0].data(), b.size()));
-            res.h2d_bytes += b.size() * 32;
-        };
-        auto side_transforms = [&](const std::vector<std::string>& names) {
-            ctx.check(h2b_ctx_side_begin(c));
-            try {
-                for (auto& nm : names) {
-                    ctx.check(h2b_poly_copy_dev(c, coef[nm]->at(), lagr[nm].ptr(), n));
-                    ctx.check(h2b_lagrange_to_coeff_dev(c, coef[nm]->at(), k));
-                    ctx.check(h2b_coeff_to_extended_dev(c, coef[nm]->at(), n, ext_k, ext[nm]->at()));
-                }
-            } catch (...) {
-                h2b_ctx_side_end(c);
-                throw;
-            }
-            ctx.check(h2b_ctx_side_end(c));
-        };
-        auto lincomb = [&](const std::vector<const void*>& ptrs, const std::vector<Fr>& scalars, Poly* out) {
-            bool first = true;  // h2b_poly_lincomb takes at most 32 polynomials a call
-            for (size_t lo = 0; lo < ptrs.size(); lo += 31) {
-                std::vector<const void*> pp(ptrs.begin() + lo, ptrs.begin() + std::min(ptrs.size(), lo + 31));
-                std::vector<Fr> sc(scalars.begin() + lo, scalars.begin() + std::min(ptrs.size(), lo + 31));
-                if (!first) { pp.insert(pp.begin(), out->at()); sc.insert(sc.begin(), HostFr::one()); }
-                ctx.check(h2b_poly_lincomb_dev(c, pp.data(), sc[0].data(), pp.size(), n, out->at()));
-                first = false;
-            }
-        };
-
-        // ---- phase 0: the public values into the transcript; witness up, assignment, advice commitments (the random polynomial
-        // and the instance columns go up beside them)
-        for (size_t m = 0; m < cs.I; m++) tr.absorb(wit.instance[m], wit.n_instance[m] * sizeof(Fr));
-        res.h2d_bytes += assign_witness(ctx, cs, wit, wit.assigned_form(), verdict_words(), adv_block->at(), witness_bufs, random_poly, rnd);
-        res.h2d_bytes += upload_instances(wit);
-        std::vector<std::pair<int, ColRef>> items;
-        for (auto& nm : cs.adv_names) {
-            blind_col(lagr[nm], u);
-            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm]});
-        }
-        commit(items, true, wit.assigned_form());
-        const uint32_t rat_bad = uint32_t(verdict), lk_bad = L && wit.lookup_index ? uint32_t(verdict >> 32) : 0;
-        if (rat_bad || lk_bad) {
-            h2b_ctx_side_join(c);  // nothing of this proof stays in flight behind the error
-            h2b_ctx_synchronize(c);
-            witness_error(rat_bad, lk_bad, "create_proof");
-        }
-        res.theta = tr.squeeze();
-        ctx.check(h2b_ctx_side_join(c));  // the random polynomial arrived while phase 0 ran
-        std::vector<std::string> phase0 = cs.adv_names;
-        phase0.insert(phase0.end(), cs.inst_names.begin(), cs.inst_names.end());
-        side_transforms(phase0);
-        // ---- lookups: compressed input, permuted pair (enqueue only; the verdict words are read after this phase's commitments)
-        std::vector<void*> lk_in;
-        items.clear();
-        std::vector<std::string> perm_names;
-        for (size_t t = 0; t < cs.n_lookups; t++) {
-            const std::string ts = std::to_string(t);
-            if (L == 0) {
-                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at("q_lookup")->at(), lagr["a0"].ptr(), n, inp->at()));
-                lk_in.push_back(inp->at());
-            } else {
-                lk_in.push_back(lagr["l" + ts].ptr());
-            }
-            const ColRef &pa = lagr["pa" + ts], &ps = lagr["ps" + ts];
-            ctx.check(h2b_permute_expression_pair_async_dev(c, lk_in[t], cs.lagr.at("table")->at(), k, bf, pa.ptr(), ps.ptr(),
-                                                            static_cast<uint32_t*>(d_status->at(t))));
-            blind_col(pa, u);
-            blind_col(ps, u);
-            items.push_back({H2B_BASIS_LAGRANGE, pa});
-            items.push_back({H2B_BASIS_LAGRANGE, ps});
-            perm_names.push_back("pa" + ts);
-            perm_names.push_back("ps" + ts);
-        }
-        if (cs.n_lookups) {
-            commit(items, true);
-            for (auto& w : d_status->download(0, cs.n_lookups))
-                if (w[0]) throw Error(H2B_ERR_UNSATISFIED, "permute_expression_pair: an input value is not in the table (ConstraintSystemFailure)");
-            res.d2h_bytes += 32 * cs.n_lookups;
-        }
-        res.beta = tr.squeeze();
-        res.gamma = tr.squeeze();
-        side_transforms(perm_names);
-        // ---- product columns + the vanishing argument's random polynomial
-        auto col_lagr = [&](const std::string& nm) -> void* { return cs.is_const(nm) ? cs.lagr.at(nm)->at() : lagr[nm].ptr(); };
-        for (size_t s = 0; s < cs.n_sets; s++) {
-            std::vector<const void*> cols, sig;
-            for (size_t i = s * cs.chunk; i < std::min(cs.perm_cols.size(), (s + 1) * cs.chunk); i++) {
-                cols.push_back(col_lagr(cs.perm_cols[i]));
-                sig.push_back(cs.lagr.at("sigma_" + cs.perm_cols[i])->at());
-            }
-            const void* start = s == 0 ? nullptr : lagr["zp" + std::to_string(s - 1)].ptr(u);  // chained through the previous set's closing value
-            ctx.check(h2b_permutation_product_dev(c, cols.data(), sig.data(), cols.size(), s * cs.chunk, res.beta.data(), res.gamma.data(), k, bf, start,
-                                                  lagr["zp" + std::to_string(s)].ptr()));
-        }
-        for (size_t t = 0; t < cs.n_lookups; t++) {
-            const std::string ts = std::to_string(t);
-            ctx.check(h2b_lookup_product_dev(c, lk_in[t], cs.lagr.at("table")->at(), lagr["pa" + ts].ptr(), lagr["ps" + ts].ptr(), res.beta.data(),
-                                             res.gamma.data(), k, bf, lagr["zl" + ts].ptr()));
-        }
-        std::vector<std::string> prod_names;
-        for (size_t s = 0; s < cs.n_sets; s++) prod_names.push_back("zp" + std::to_string(s));
-        for (size_t t = 0; t < cs.n_lookups; t++) prod_names.push_back("zl" + std::to_string(t));
-        items.clear();
-        for (auto& nm : prod_names) {
-            blind_col(lagr[nm], u + 1);
-            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm]});
-        }
-        side_transforms(prod_names);  // beside the commitments below
-        items.push_back({H2B_BASIS_MONOMIAL, ColRef{rnd, 0}});
-        commit(items, true);
-        res.y = tr.squeeze();
-        ctx.check(h2b_ctx_side_join(c));  // every column is now in coefficient and extended form
-        // ---- quotient: gate, permutation and lookup terms folded with y on the extended coset
-        Challenges ch;
-        ch.beta = res.beta; ch.gamma = res.gamma; ch.theta = res.theta; ch.y = res.y;
-        ctx.check(h2b_poly_zero(c, h->raw()));
-        for (auto& gp : cs.gate_programs) {
-            std::vector<const void*> fx, ad;
-            for (size_t j : gp.cols) {
-                fx.push_back(cs.ext.at("q" + std::to_string(j))->at());
-                ad.push_back(ext["a" + std::to_string(j)]->at());
-            }
-            const BoundGraph g(gp.ev, gp.result, fx, ad, ch);
-            ctx.check(h2b_quotient_graph_dev(c, g.get(), k, ext_k, h->at()));
-        }
-        {
-            std::vector<const void*> tz, tc, ts;
-            for (size_t s = 0; s < cs.n_sets; s++) tz.push_back(ext["zp" + std::to_string(s)]->at());
-            for (auto& nm : cs.perm_cols) {
-                tc.push_back(cs.is_const(nm) ? cs.ext.at(nm)->at() : ext[nm]->at());
-                ts.push_back(cs.ext.at("sigma_" + nm)->at());
-            }
-            ctx.check(h2b_permutation_fold_dev(c, tz.data(), cs.n_sets, tc.data(), ts.data(), tc.size(), cs.chunk, cs.ext.at("l0")->at(),
-                                               cs.ext.at("l_last")->at(), cs.ext.at("l_active")->at(), res.beta.data(), res.gamma.data(), res.y.data(), bf, k,
-                                               ext_k, h->at()));
-        }
-        for (size_t t = 0; t < cs.n_lookups; t++) {
-            const std::string ts = std::to_string(t);
-            std::vector<const void*> fx, ad;
-            if (L == 0) {
-                fx = {cs.ext.at("q_lookup")->at(), cs.ext.at("table")->at()};
-                ad = {ext["a0"]->at()};
-            } else {
-                fx = {cs.ext.at("table")->at()};
-                ad = {ext["l" + ts]->at()};
-            }
-            const BoundGraph g(cs.lookup_ev, cs.lookup_result, fx, ad, ch);
-            ctx.check(h2b_lookup_fold_dev(c, g.get(), ext["zl" + ts]->at(), ext["pa" + ts]->at(), ext["ps" + ts]->at(), cs.ext.at("l0")->at(),
-                                          cs.ext.at("l_last")->at(), cs.ext.at("l_active")->at(), k, ext_k, h->at()));
-        }
-        ctx.check(h2b_divide_by_vanishing_poly_dev(c, h->at(), k, ext_k));
-        ctx.check(h2b_extended_to_coeff_dev(c, h->at(), ext_k));
-        const size_t pieces = cs.degree - 1;
-        items.clear();
-        for (size_t j = 0; j < pieces; j++) items.push_back({H2B_BASIS_MONOMIAL, ColRef{h, j * n}});
-        commit(items, true);
-        res.x = tr.squeeze();
+        prove_to_x(wit, random_poly, blind, tr, res, "create_proof");
+        auto rot = [&](int r) { return rotate(res.x, r); };
         // ---- evaluations at x and its rotations
-        const Fr w = HostFr::omega(k);
-        auto rot = [&](int r) { return HostFr::mul(res.x, HostFr::pow(w, uint64_t(((r % (long long)n) + (long long)n) % (long long)n))); };
         const std::vector<Query> queries = this->queries();
         {
-            const size_t m = queries.size();
-            std::vector<const void*> polys(m);
-            std::vector<Fr> xs(m), out(m);
-            for (size_t i = 0; i < m; i++) { polys[i] = queries[i].ptr; xs[i] = rot(queries[i].rot); }
-            ctx.check(h2b_eval_polynomial_batch_dev(c, polys.data(), xs[0].data(), m, n, out[0].data()));
-            res.d2h_bytes += m * 32;
-            tr.absorb(out.data(), m * sizeof(Fr));
-            for (size_t i = 0; i < m; i++) res.evals.push_back({{queries[i].name, queries[i].rot}, out[i]});
+            const std::vector<Fr> out = evaluate(queries, res);
+            tr.absorb(out.data(), out.size() * sizeof(Fr));
+            for (size_t i = 0; i < out.size(); i++) res.evals.push_back({{queries[i].name, queries[i].rot}, out[i]});
         }
         // ---- SHPLONK-shaped opening: per rotation set sum_i v^i p_i, divided by (X - point) for every point of the set
         const Fr v_ch = tr.squeeze(), mu = tr.squeeze();
@@ -969,14 +862,121 @@ public:
         ctx.check(h2b_ctx_side_join(c));
         if (have_main) lincomb({tmp[2]->at(), tmp_side[2]->at()}, {HostFr::one(), HostFr::one()}, tmp[2]);
         else ctx.check(h2b_poly_copy_dev(c, tmp[2]->at(), tmp_side[2]->at(), n));
-        commit({{H2B_BASIS_MONOMIAL, ColRef{tmp[2], 0}}}, true);
+        commit({{H2B_BASIS_MONOMIAL, ColRef{tmp[2], 0}}}, res, &tr);
         const Fr u_ch = tr.squeeze();
         // final quotient: W' = L / (X - u) (the remainder is dropped by kate_division)
         ctx.check(h2b_kate_division_dev(c, tmp[2]->at(), n, u_ch.data(), tmp[3]->at()));
         ctx.check(h2b_poly_copy_dev(c, tmp[3]->at(n - 1), zero->at(), 1));
-        commit({{H2B_BASIS_MONOMIAL, ColRef{tmp[3], 0}}}, false);
+        commit({{H2B_BASIS_MONOMIAL, ColRef{tmp[3], 0}}}, res, static_cast<Transcript*>(nullptr));
         return res;
     }
+
+    // halo2's create_proof with ProverSHPLONK (halo2-axiom 0.5.3, recalled; DESIGN §2): the same device phases as create_proof
+    // up to the h pieces (prove_to_x), written through halo2's Blake2bWrite, then halo2's evaluations and multi-open.
+    // vk_repr: the verifying key's transcript_repr, absorbed first (vk.hash_into; the caller computes it from the pinned vk).
+    // Returns transcript.finalize(): the bytes gen_proof_with_instances returns.
+    std::vector<uint8_t> create_proof_halo2(const WitnessView& wit, const Fr* random_poly, const BlindSource& blind, const Fr& vk_repr) {
+        const size_t n = cs.n;
+        h2b_ctx* c = ctx.raw();
+        Blake2bWrite tr;
+        Proof res;
+        tr.common_scalar(vk_repr);
+        prove_to_x(wit, random_poly, blind, tr, res, "create_proof_halo2");
+        // ---- evaluations: advice, fixed, random_poly, sigma, permutation sets, lookups (h(x) is not written)
+        for (const Fr& e : evaluate(halo2_evaluations(), res)) tr.write_scalar(e);
+        // ---- the vanishing argument opens h(X) = sum_i x^(n i) h_i
+        Poly* hx = tmp_side[0];
+        {
+            std::vector<const void*> pp;
+            std::vector<Fr> sc;
+            const Fr xn = HostFr::pow(res.x, n);
+            Fr s = HostFr::one();
+            for (size_t j = 0; j + 1 < cs.degree; j++) {
+                pp.push_back(h->at(j * n));
+                sc.push_back(s);
+                s = HostFr::mul(s, xn);
+            }
+            lincomb(pp, sc, hx);
+        }
+        // ---- ProverSHPLONK: commitments grouped by identity in first-appearance order, then by equal point sets
+        std::vector<std::pair<const void*, std::vector<int>>> by_poly;
+        for (auto& q : halo2_openings(hx)) {
+            auto it = std::find_if(by_poly.begin(), by_poly.end(), [&](auto& e) { return e.first == q.ptr; });
+            if (it == by_poly.end()) by_poly.push_back({q.ptr, {q.rot}});
+            else if (std::find(it->second.begin(), it->second.end(), q.rot) == it->second.end()) it->second.push_back(q.rot);
+        }
+        std::vector<std::pair<std::vector<int>, std::vector<const void*>>> sets;  // (points as rotations, sorted; polynomials)
+        std::vector<int> all;                                                       // T: every point of every set
+        for (auto& e : by_poly) {
+            const void* ptr = e.first;
+            std::vector<int>& rots = e.second;
+            std::sort(rots.begin(), rots.end());
+            if (rots.size() > H2B_KATE_MULTI_MAX) throw Error(H2B_ERR_ARG, "create_proof_halo2: a rotation set of more than 4 points");
+            auto it = std::find_if(sets.begin(), sets.end(), [&](auto& s) { return s.first == rots; });
+            if (it == sets.end()) sets.push_back({rots, {ptr}});
+            else it->second.push_back(ptr);
+            for (int r : rots)
+                if (std::find(all.begin(), all.end(), r) == all.end()) all.push_back(r);
+        }
+        const Fr y = tr.squeeze();
+        const Fr v = tr.squeeze();
+        auto y_powers = [&](size_t m) {
+            std::vector<Fr> p(m, HostFr::one());
+            for (size_t i = 1; i < m; i++) p[i] = HostFr::mul(p[i - 1], y);
+            return p;
+        };
+        // h_x = sum_s v^(S-1-s) (q_s - r_s) / Z_{T_s},  q_s = sum_j y^j p_sj  (Horner in v over the sets)
+        Poly *f = tmp[0], *qd = tmp[1], *hacc = tmp[2], *lin = tmp[3];
+        for (size_t s = 0; s < sets.size(); s++) {
+            const auto& [rots, plist] = sets[s];
+            lincomb(plist, y_powers(plist.size()), f);
+            const size_t m = rots.size();
+            std::vector<Fr> pts(m), ws(m, HostFr::one());
+            for (size_t j = 0; j < m; j++) pts[j] = rotate(res.x, rots[j]);
+            for (size_t j = 0; j < m; j++)
+                for (size_t t = 0; t < m; t++)
+                    if (t != j) ws[j] = HostFr::mul(ws[j], HostFr::sub(pts[j], pts[t]));
+            for (auto& w : ws) w = HostFr::inv(w);
+            ctx.check(h2b_kate_division_multi_dev(c, f->at(), n, pts[0].data(), m, ws[0].data(), qd->at()));
+            ctx.check(h2b_poly_copy_dev(c, qd->at(n - 1), zero->at(), 1));  // n - 1 coefficients written, used as n
+            if (s == 0) ctx.check(h2b_poly_copy_dev(c, hacc->at(), qd->at(), n));
+            else lincomb({hacc->at(), qd->at()}, {v, HostFr::one()}, hacc);
+        }
+        commit({{H2B_BASIS_MONOMIAL, ColRef{hacc, 0}}}, res, &tr);
+        const Fr u = tr.squeeze();
+        // L = sum_s v^(S-1-s) Z_{T\T_s}(u) q_s - Z_T(u) h_x, without the constants r_s(u): they change only the remainder of
+        // L / (X - u), which kate_division drops
+        auto vanishing_at_u = [&](const std::vector<int>& rots) {
+            Fr z = HostFr::one();
+            for (int r : rots) z = HostFr::mul(z, HostFr::sub(u, rotate(res.x, r)));
+            return z;
+        };
+        std::vector<const void*> lp;
+        std::vector<Fr> ls;
+        Fr vs = HostFr::one();  // v^(S-1-s), s from the last set down
+        for (size_t s = sets.size(); s-- > 0;) {
+            const auto& [rots, plist] = sets[s];
+            std::vector<int> diff;
+            for (int r : all)
+                if (std::find(rots.begin(), rots.end(), r) == rots.end()) diff.push_back(r);
+            const Fr coef = HostFr::mul(vs, vanishing_at_u(diff));
+            const std::vector<Fr> yp = y_powers(plist.size());
+            for (size_t j = 0; j < plist.size(); j++) {
+                lp.push_back(plist[j]);
+                ls.push_back(HostFr::mul(coef, yp[j]));
+            }
+            vs = HostFr::mul(vs, v);
+        }
+        lp.push_back(hacc->at());
+        ls.push_back(HostFr::neg(vanishing_at_u(all)));
+        lincomb(lp, ls, lin);
+        // W' = L / (X - u)
+        ctx.check(h2b_kate_division_dev(c, lin->at(), n, u.data(), f->at()));
+        ctx.check(h2b_poly_copy_dev(c, f->at(n - 1), zero->at(), 1));
+        commit({{H2B_BASIS_MONOMIAL, ColRef{f, 0}}}, res, &tr);
+        return tr.finalize();
+    }
+
     // commitments per proof, in commit order: advice | permuted pairs | product columns + random | h pieces | two openings
     size_t commitments_per_proof() const {
         return cs.adv_names.size() + 2 * cs.n_lookups + (cs.n_sets + cs.n_lookups + 1) + (cs.degree - 1) + 2;
@@ -1012,6 +1012,60 @@ public:
         }
         for (size_t j = 0; j + 1 < cs.degree; j++) q.push_back({"h" + std::to_string(j), h->at(j * cs.n), 0});
         q.push_back({"rnd", rnd->at(), 0});
+        return q;
+    }
+
+    // the evaluations of create_proof_halo2 in the order halo2 writes them: advice (advice_queries), fixed (fixed_queries),
+    // random_poly, sigma, per permutation set z(x), z(omega x) and, but for the last set, z(omega^last x), per lookup z(x),
+    // z(omega x), A'(x), A'(omega^-1 x), S'(x)
+    std::vector<Query> halo2_evaluations() const {
+        const int last = -int(cs.bf + 1);
+        std::vector<Query> q = advice_queries();
+        for (auto& nm : cs.fixed_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        q.push_back({"rnd", rnd->at(), 0});
+        for (auto& nm : cs.sigma_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (size_t s = 0; s < cs.n_sets; s++) {
+            const std::string nm = "zp" + std::to_string(s);
+            for (int r : {0, 1}) q.push_back({nm, coef.at(nm)->at(), r});
+            if (s + 1 < cs.n_sets) q.push_back({nm, coef.at(nm)->at(), last});
+        }
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const std::string ts = std::to_string(t);
+            for (auto [nm, r] : std::initializer_list<std::pair<const char*, int>>{{"zl", 0}, {"zl", 1}, {"pa", 0}, {"pa", -1}, {"ps", 0}})
+                q.push_back({nm + ts, coef.at(nm + ts)->at(), r});
+        }
+        return q;
+    }
+    // the opening queries of create_proof_halo2 in halo2's order (it fixes the rotation sets): advice, permutation sets at x
+    // and omega x then omega^last x for the sets in reverse order but the last, per lookup z(x), A'(x), S'(x), A'(omega^-1 x),
+    // z(omega x), fixed, sigma, h(X) = `hx`, random_poly
+    std::vector<Query> halo2_openings(const Poly* hx) const {
+        const int last = -int(cs.bf + 1);
+        std::vector<Query> q = advice_queries();
+        for (size_t s = 0; s < cs.n_sets; s++) {
+            const std::string nm = "zp" + std::to_string(s);
+            for (int r : {0, 1}) q.push_back({nm, coef.at(nm)->at(), r});
+        }
+        for (size_t s = cs.n_sets; s-- > 1;) {
+            const std::string nm = "zp" + std::to_string(s - 1);
+            q.push_back({nm, coef.at(nm)->at(), last});
+        }
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const std::string ts = std::to_string(t);
+            for (auto [nm, r] : std::initializer_list<std::pair<const char*, int>>{{"zl", 0}, {"pa", 0}, {"ps", 0}, {"pa", -1}, {"zl", 1}})
+                q.push_back({nm + ts, coef.at(nm + ts)->at(), r});
+        }
+        for (auto& nm : cs.fixed_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (auto& nm : cs.sigma_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        q.push_back({"h", hx->at(), 0});
+        q.push_back({"rnd", rnd->at(), 0});
+        return q;
+    }
+    std::vector<Query> advice_queries() const {
+        std::vector<Query> q;
+        for (size_t j = 0; j < cs.A; j++)
+            for (int r : {0, 1, 2, 3}) q.push_back({"a" + std::to_string(j), coef.at("a" + std::to_string(j))->at(), r});
+        for (size_t t = 0; t < cs.L; t++) q.push_back({"l" + std::to_string(t), coef.at("l" + std::to_string(t))->at(), 0});
         return q;
     }
 
@@ -1081,6 +1135,224 @@ public:
     }
 
 private:
+    // phase 0 up to the commitments of the h pieces and the challenge x, the device work create_proof and create_proof_halo2
+    // share: `tr` (Transcript or Blake2bWrite) takes the public values (common_scalars) and every commitment (write_points);
+    // res receives the commitments, the challenges theta .. x and the byte counts
+    template <class TR>
+    void prove_to_x(const WitnessView& wit, const Fr* random_poly, const BlindSource& blind, TR& tr, Proof& res, const std::string& who) {
+        const uint32_t k = cs.k, ext_k = cs.ext_k, bf = cs.bf;
+        const size_t n = cs.n, u = cs.u, L = cs.L;
+        h2b_ctx* c = ctx.raw();
+        check_inputs(wit, who, cs);
+        if (!random_poly) throw Error(H2B_ERR_ARG, who + ": null random polynomial");
+        uint64_t verdict = 0;  // phase 0: the verdict words, read with the first download of its commitments
+        auto blind_col = [&](const ColRef& col, size_t first_row) {
+            const std::vector<Fr> b = blind(n - first_row);
+            if (b.size() != n - first_row) throw Error(H2B_ERR_ARG, "blind source returned the wrong number of rows");
+            ctx.check(h2b_poly_upload(c, col.poly->raw(), col.offset + first_row, b[0].data(), b.size()));
+            res.h2d_bytes += b.size() * 32;
+        };
+        auto side_transforms = [&](const std::vector<std::string>& names) {
+            ctx.check(h2b_ctx_side_begin(c));
+            try {
+                for (auto& nm : names) {
+                    ctx.check(h2b_poly_copy_dev(c, coef[nm]->at(), lagr[nm].ptr(), n));
+                    ctx.check(h2b_lagrange_to_coeff_dev(c, coef[nm]->at(), k));
+                    ctx.check(h2b_coeff_to_extended_dev(c, coef[nm]->at(), n, ext_k, ext[nm]->at()));
+                }
+            } catch (...) {
+                h2b_ctx_side_end(c);
+                throw;
+            }
+            ctx.check(h2b_ctx_side_end(c));
+        };
+
+        // ---- phase 0: the public values into the transcript; witness up, assignment, advice commitments (the random polynomial
+        // and the instance columns go up beside them)
+        for (size_t m = 0; m < cs.I; m++) tr.common_scalars(wit.instance[m], wit.n_instance[m]);
+        res.h2d_bytes += assign_witness(ctx, cs, wit, wit.assigned_form(), verdict_words(), adv_block->at(), witness_bufs, random_poly, rnd);
+        res.h2d_bytes += upload_instances(wit);
+        std::vector<std::pair<int, ColRef>> items;
+        for (auto& nm : cs.adv_names) {
+            blind_col(lagr[nm], u);
+            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm]});
+        }
+        commit(items, res, &tr, wit.assigned_form() ? &verdict : nullptr);
+        const uint32_t rat_bad = uint32_t(verdict), lk_bad = L && wit.lookup_index ? uint32_t(verdict >> 32) : 0;
+        if (rat_bad || lk_bad) {
+            h2b_ctx_side_join(c);  // nothing of this proof stays in flight behind the error
+            h2b_ctx_synchronize(c);
+            witness_error(rat_bad, lk_bad, who);
+        }
+        res.theta = tr.squeeze();
+        ctx.check(h2b_ctx_side_join(c));  // the random polynomial arrived while phase 0 ran
+        std::vector<std::string> phase0 = cs.adv_names;
+        phase0.insert(phase0.end(), cs.inst_names.begin(), cs.inst_names.end());
+        side_transforms(phase0);
+        // ---- lookups: compressed input, permuted pair (enqueue only; the verdict words are read after this phase's commitments)
+        std::vector<void*> lk_in;
+        items.clear();
+        std::vector<std::string> perm_names;
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const std::string ts = std::to_string(t);
+            if (L == 0) {
+                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at("q_lookup")->at(), lagr["a0"].ptr(), n, inp->at()));
+                lk_in.push_back(inp->at());
+            } else {
+                lk_in.push_back(lagr["l" + ts].ptr());
+            }
+            const ColRef &pa = lagr["pa" + ts], &ps = lagr["ps" + ts];
+            ctx.check(h2b_permute_expression_pair_async_dev(c, lk_in[t], cs.lagr.at("table")->at(), k, bf, pa.ptr(), ps.ptr(),
+                                                            static_cast<uint32_t*>(d_status->at(t))));
+            blind_col(pa, u);
+            blind_col(ps, u);
+            items.push_back({H2B_BASIS_LAGRANGE, pa});
+            items.push_back({H2B_BASIS_LAGRANGE, ps});
+            perm_names.push_back("pa" + ts);
+            perm_names.push_back("ps" + ts);
+        }
+        if (cs.n_lookups) {
+            commit(items, res, &tr);
+            for (auto& w : d_status->download(0, cs.n_lookups))
+                if (w[0]) throw Error(H2B_ERR_UNSATISFIED, "permute_expression_pair: an input value is not in the table (ConstraintSystemFailure)");
+            res.d2h_bytes += 32 * cs.n_lookups;
+        }
+        res.beta = tr.squeeze();
+        res.gamma = tr.squeeze();
+        side_transforms(perm_names);
+        // ---- product columns + the vanishing argument's random polynomial
+        auto col_lagr = [&](const std::string& nm) -> void* { return cs.is_const(nm) ? cs.lagr.at(nm)->at() : lagr[nm].ptr(); };
+        for (size_t s = 0; s < cs.n_sets; s++) {
+            std::vector<const void*> cols, sig;
+            for (size_t i = s * cs.chunk; i < std::min(cs.perm_cols.size(), (s + 1) * cs.chunk); i++) {
+                cols.push_back(col_lagr(cs.perm_cols[i]));
+                sig.push_back(cs.lagr.at("sigma_" + cs.perm_cols[i])->at());
+            }
+            const void* start = s == 0 ? nullptr : lagr["zp" + std::to_string(s - 1)].ptr(u);  // chained through the previous set's closing value
+            ctx.check(h2b_permutation_product_dev(c, cols.data(), sig.data(), cols.size(), s * cs.chunk, res.beta.data(), res.gamma.data(), k, bf, start,
+                                                  lagr["zp" + std::to_string(s)].ptr()));
+        }
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const std::string ts = std::to_string(t);
+            ctx.check(h2b_lookup_product_dev(c, lk_in[t], cs.lagr.at("table")->at(), lagr["pa" + ts].ptr(), lagr["ps" + ts].ptr(), res.beta.data(),
+                                             res.gamma.data(), k, bf, lagr["zl" + ts].ptr()));
+        }
+        std::vector<std::string> prod_names;
+        for (size_t s = 0; s < cs.n_sets; s++) prod_names.push_back("zp" + std::to_string(s));
+        for (size_t t = 0; t < cs.n_lookups; t++) prod_names.push_back("zl" + std::to_string(t));
+        items.clear();
+        for (auto& nm : prod_names) {
+            blind_col(lagr[nm], u + 1);
+            items.push_back({H2B_BASIS_LAGRANGE, lagr[nm]});
+        }
+        side_transforms(prod_names);  // beside the commitments below
+        items.push_back({H2B_BASIS_MONOMIAL, ColRef{rnd, 0}});
+        commit(items, res, &tr);
+        res.y = tr.squeeze();
+        ctx.check(h2b_ctx_side_join(c));  // every column is now in coefficient and extended form
+        // ---- quotient: gate, permutation and lookup terms folded with y on the extended coset
+        Challenges ch;
+        ch.beta = res.beta; ch.gamma = res.gamma; ch.theta = res.theta; ch.y = res.y;
+        ctx.check(h2b_poly_zero(c, h->raw()));
+        for (auto& gp : cs.gate_programs) {
+            std::vector<const void*> fx, ad;
+            for (size_t j : gp.cols) {
+                fx.push_back(cs.ext.at("q" + std::to_string(j))->at());
+                ad.push_back(ext["a" + std::to_string(j)]->at());
+            }
+            const BoundGraph g(gp.ev, gp.result, fx, ad, ch);
+            ctx.check(h2b_quotient_graph_dev(c, g.get(), k, ext_k, h->at()));
+        }
+        {
+            std::vector<const void*> tz, tc, ts;
+            for (size_t s = 0; s < cs.n_sets; s++) tz.push_back(ext["zp" + std::to_string(s)]->at());
+            for (auto& nm : cs.perm_cols) {
+                tc.push_back(cs.is_const(nm) ? cs.ext.at(nm)->at() : ext[nm]->at());
+                ts.push_back(cs.ext.at("sigma_" + nm)->at());
+            }
+            ctx.check(h2b_permutation_fold_dev(c, tz.data(), cs.n_sets, tc.data(), ts.data(), tc.size(), cs.chunk, cs.ext.at("l0")->at(),
+                                               cs.ext.at("l_last")->at(), cs.ext.at("l_active")->at(), res.beta.data(), res.gamma.data(), res.y.data(), bf, k,
+                                               ext_k, h->at()));
+        }
+        for (size_t t = 0; t < cs.n_lookups; t++) {
+            const std::string ts = std::to_string(t);
+            std::vector<const void*> fx, ad;
+            if (L == 0) {
+                fx = {cs.ext.at("q_lookup")->at(), cs.ext.at("table")->at()};
+                ad = {ext["a0"]->at()};
+            } else {
+                fx = {cs.ext.at("table")->at()};
+                ad = {ext["l" + ts]->at()};
+            }
+            const BoundGraph g(cs.lookup_ev, cs.lookup_result, fx, ad, ch);
+            ctx.check(h2b_lookup_fold_dev(c, g.get(), ext["zl" + ts]->at(), ext["pa" + ts]->at(), ext["ps" + ts]->at(), cs.ext.at("l0")->at(),
+                                          cs.ext.at("l_last")->at(), cs.ext.at("l_active")->at(), k, ext_k, h->at()));
+        }
+        ctx.check(h2b_divide_by_vanishing_poly_dev(c, h->at(), k, ext_k));
+        ctx.check(h2b_extended_to_coeff_dev(c, h->at(), ext_k));
+        const size_t pieces = cs.degree - 1;
+        items.clear();
+        for (size_t j = 0; j < pieces; j++) items.push_back({H2B_BASIS_MONOMIAL, ColRef{h, j * n}});
+        commit(items, res, &tr);
+        res.x = tr.squeeze();
+    }
+    // commits `items` (batched MSMs of at most 16), appends the affine points to res.commitments and writes them to `tr` (none:
+    // null); with `verdict`, the first download also brings the phase-0 verdict words
+    template <class TR>
+    void commit(const std::vector<std::pair<int, ColRef>>& items, Proof& res, TR* tr, uint64_t* verdict = nullptr) {
+        h2b_ctx* c = ctx.raw();
+        for (size_t lo = 0; lo < items.size(); lo += 16) {
+            const size_t m = std::min<size_t>(16, items.size() - lo);
+            std::vector<const void*> ptrs(m);
+            std::vector<int> bs(m);
+            for (size_t i = 0; i < m; i++) { bs[i] = items[lo + i].first; ptrs[i] = items[lo + i].second.ptr(shard_begin); }
+            ctx.check(h2b_msm_g1_batch_dev(c, params.raw(), bs.data(), ptrs.data(), m, n_loc, d_out->at()));
+            if (allreduce) allreduce(d_out->at(), m);
+            if (observer) {
+                ctx.check(h2b_ctx_synchronize(c));
+                for (size_t i = 0; i < m; i++) observer(bs[i], items[lo + i].second.poly->download(items[lo + i].second.offset, cs.n));
+            }
+            const size_t cnt = verdict && lo == 0 ? 49 : m * 3;
+            std::vector<G1> out(m);
+            if (cnt == 49) {
+                std::vector<Fr> raw = d_out->download(0, 49);
+                std::memcpy(out[0].x.data(), raw.data(), m * sizeof(G1));
+                *verdict = raw[48][0];
+            } else {
+                ctx.check(h2b_poly_download(c, d_out->raw(), 0, out[0].x.data(), m * 3));
+            }
+            res.d2h_bytes += cnt * 32;
+            g1_normalize_host_batch(out.data(), m);  // affine form: what the transcript and the proof hold
+            if (tr) tr->write_points(out.data(), m);
+            res.commitments.insert(res.commitments.end(), out.begin(), out.end());
+        }
+    }
+    // out = sum_i scalars[i] ptrs[i] over n coefficients (h2b_poly_lincomb takes at most 32 polynomials a call)
+    void lincomb(const std::vector<const void*>& ptrs, const std::vector<Fr>& scalars, Poly* out) {
+        bool first = true;
+        for (size_t lo = 0; lo < ptrs.size(); lo += 31) {
+            std::vector<const void*> pp(ptrs.begin() + lo, ptrs.begin() + std::min(ptrs.size(), lo + 31));
+            std::vector<Fr> sc(scalars.begin() + lo, scalars.begin() + std::min(ptrs.size(), lo + 31));
+            if (!first) { pp.insert(pp.begin(), out->at()); sc.insert(sc.begin(), HostFr::one()); }
+            ctx.check(h2b_poly_lincomb_dev(ctx.raw(), pp.data(), sc[0].data(), pp.size(), cs.n, out->at()));
+            first = false;
+        }
+    }
+    // x omega^r
+    Fr rotate(const Fr& x, int r) const {
+        const long long n = (long long)cs.n;
+        return HostFr::mul(x, HostFr::pow(HostFr::omega(cs.k), uint64_t(((r % n) + n) % n)));
+    }
+    // the queries' values at x omega^rot, in one batch
+    std::vector<Fr> evaluate(const std::vector<Query>& q, Proof& res) {
+        const size_t m = q.size();
+        std::vector<const void*> polys(m);
+        std::vector<Fr> xs(m), out(m);
+        for (size_t i = 0; i < m; i++) { polys[i] = q[i].ptr; xs[i] = rotate(res.x, q[i].rot); }
+        ctx.check(h2b_eval_polynomial_batch_dev(ctx.raw(), polys.data(), xs[0].data(), m, cs.n, out[0].data()));
+        res.d2h_bytes += m * 32;
+        return out;
+    }
     static WitnessView view(const std::vector<Fr>& witness, const std::vector<uint64_t>& break_points, const std::vector<Fr>& lookup_cells,
                             const AssignedWitness* form, const std::string& who) {
         WitnessView w;
