@@ -157,6 +157,8 @@ SIGNATURES = {
     "h2b_kate_division_dev": (_int, [_vp, _vp, _sz, _vp, _vp]),
     "h2b_kate_division_multi": (_int, [_vp, _vp, _sz, _vp, _sz, _vp, _vp]),
     "h2b_kate_division_multi_dev": (_int, [_vp, _vp, _sz, _vp, _sz, _vp, _vp]),
+    "h2b_selector_conflicts": (_int, [_vp, _vpp, _sz, _u32, _vp]),
+    "h2b_selector_conflicts_dev": (_int, [_vp, _vpp, _sz, _u32, _vp]),
     "h2b_poly_lincomb": (_int, [_vp, _vpp, _vp, _sz, _sz, _vp]),
     "h2b_poly_lincomb_dev": (_int, [_vp, _vpp, _vp, _sz, _sz, _vp]),
     "h2b_poly_alloc": (_int, [_vp, _sz, C.POINTER(_vp)]),
@@ -204,7 +206,7 @@ _witp = C.POINTER(Witness)
 _u64s = C.POINTER(C.c_uint64)
 
 PROVER_SIGNATURES = {
-    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, _sz, _sz, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp)]),
+    "h2bp_circuit_create": (_int, [_vp, _u32, _sz, _sz, _int, _sz, _sz, C.POINTER(C.c_char_p), _vpp, _sz, _vpp, _sz, C.POINTER(_vp), _int]),
     "h2bp_circuit_free": (None, [_vp]),
     "h2bp_circuit_info": (_int, [_vp, _u64s, C.c_char_p, _sz]),
     "h2bp_circuit_column": (_int, [_vp, C.c_char_p, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
@@ -220,7 +222,7 @@ PROVER_SIGNATURES = {
     "h2bp_mock_free": (None, [_vp]),
     "h2bp_mock_column": (_int, [_vp, C.c_char_p, C.POINTER(_vp), C.POINTER(_sz), C.POINTER(_sz)]),
     "h2bp_mock_run": (_int, [_vp, C.POINTER(BuilderView), _sz, _vp, _u64s, _vp, _vp, _u64s]),
-    "h2bp_keygen": (_int, [_vp, _vp, _u32, _sz, _sz, _sz, _int, _u32, _sz, _sz, C.POINTER(BuilderView), C.POINTER(_vp), _vp, _u64s, _vp, _vp]),
+    "h2bp_keygen": (_int, [_vp, _vp, _u32, _sz, _sz, _sz, _int, _u32, _sz, _sz, C.POINTER(BuilderView), C.POINTER(_vp), _vp, _u64s, _vp, _vp, _int]),
 }
 
 

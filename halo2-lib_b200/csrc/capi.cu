@@ -1530,6 +1530,26 @@ int h2b_kate_division_multi(h2b_ctx* ctx, const uint64_t* a, size_t n, const uin
         st.finish();
     });
 }
+int h2b_selector_conflicts_dev(h2b_ctx* ctx, const void* const* d_selectors, size_t S, uint32_t k, uint8_t* conflicts) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(d_selectors && conflicts, "selector_conflicts: null pointer");
+        selector_conflicts_run(ctx, d_selectors, S, k, conflicts);
+    });
+}
+int h2b_selector_conflicts(h2b_ctx* ctx, const uint64_t* const* selectors, size_t S, uint32_t k, uint8_t* conflicts) {
+    return guarded(ctx, [&] {
+        H2B_REQUIRE(selectors && conflicts, "selector_conflicts: null pointer");
+        H2B_REQUIRE(S >= 1 && S <= H2B_SELECTORS_MAX && k >= 1 && k <= 28, "selector_conflicts: 1..4096 columns, k in 1..28");
+        const size_t bytes = ((size_t)32) << k;
+        Staging st(ctx, WS_ASSIGN_IN, S * (bytes + 32));
+        std::vector<const void*> d;
+        for (size_t c = 0; c < S; c++) {
+            H2B_REQUIRE(selectors[c], "selector_conflicts: null column");
+            d.push_back(st.up(selectors[c], bytes));
+        }
+        selector_conflicts_run(ctx, d.data(), S, k, conflicts);
+    });
+}
 int h2b_poly_lincomb_dev(h2b_ctx* ctx, const void* const* d_polys, const uint64_t* scalars, size_t m, size_t n, void* d_out) {
     return guarded(ctx, [&] {
         H2B_REQUIRE(d_polys && scalars && (d_out || n == 0), "poly_lincomb: null pointer");

@@ -291,6 +291,8 @@ void check_equalities_run(h2b_ctx* ctx, const void* d_cells, size_t N, const uin
 void check_constants_run(h2b_ctx* ctx, const void* d_cells, size_t N, const void* d_consts, const uint64_t* d_index, size_t m,
                          size_t max_report, void* d_report, uint32_t* d_status);
 void count_distinct_run(h2b_ctx* ctx, const void* d_values, size_t m, uint32_t* d_count);
+// ---- selectors.cu (host output, synchronises)
+void selector_conflicts_run(h2b_ctx* ctx, const void* const* d_cols, size_t S, uint32_t k, uint8_t* conflicts);
 // ---- srs.cu
 void g_to_lagrange_run(h2b_ctx* ctx, const void* d_g, uint32_t k, void* d_g_lagrange);
 void srs_setup_run(h2b_ctx* ctx, const uint64_t tau[4], const uint64_t base_xy[8], uint32_t k, void* d_g, void* d_g_lagrange);

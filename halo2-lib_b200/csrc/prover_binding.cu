@@ -107,10 +107,10 @@ typedef int (*h2bp_commit_fn)(void* user, int basis, const uint64_t* rows, size_
 #define H2BP_API extern "C" __attribute__((visibility("default")))
 
 // fixed: n_fixed named columns (at least the circuit's fixed_names), sigma: one per permutation column; 2^k rows each; I instance
-// columns, F constants columns
+// columns, F constants columns; compress_selectors: halo2's keygen_vk layout (ProverCircuit)
 H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, int selector_lookup, size_t I, size_t F, const char* const* fixed_names,
                                  const uint64_t* const* fixed, size_t n_fixed, const uint64_t* const* sigma, size_t n_sigma,
-                                 BoundCircuit** out) {
+                                 BoundCircuit** out, int compress_selectors) {
     return run(ctx, [&] {
         if (!out || (n_fixed && (!fixed_names || !fixed)) || (n_sigma && !sigma)) throw Error(H2B_ERR_ARG, "circuit_create: null argument");
         std::map<std::string, const Fr*> f;
@@ -118,22 +118,26 @@ H2BP_API int h2bp_circuit_create(h2b_ctx* ctx, uint32_t k, size_t A, size_t L, i
         std::vector<const Fr*> s;
         for (size_t i = 0; i < n_sigma; i++) s.push_back(reinterpret_cast<const Fr*>(sigma[i]));
         auto b = std::make_unique<BoundCircuit>(ctx);
-        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s, I, F);
+        b->cs = std::make_unique<ProverCircuit>(b->ctx, k, A, L, selector_lookup != 0, f, s, I, F, compress_selectors != 0);
         *out = b.release();
     });
 }
 H2BP_API void h2bp_circuit_free(BoundCircuit* b) { delete b; }
 
-// shape: degree, chunk, ext_k, bf, u, n_sets, n_lookups, selector_lookup; names: "adv=..\nperm=..\nfixed=..\nsigma=..\nconst=.."
-// (comma-separated; const: the constants columns, empty when F = 0)
+// shape: degree, chunk, ext_k, bf, u, n_sets, n_lookups, selector_lookup; names: "adv=..\nperm=..\nfixed=..\nsigma=..\nconst=..
+// \nqueries=..\nselectors=.." (comma-separated; fixed: the fixed columns in column order, queries: in query order; const: the
+// constants columns, empty when F = 0; selectors: name:column:root:len per selector)
 H2BP_API int h2bp_circuit_info(BoundCircuit* b, uint64_t* shape, char* names, size_t cap) {
     return run(b ? b->ctx.raw() : nullptr, [&] {
         const ProverCircuit& cs = *b->cs;
         const uint64_t v[8] = {cs.degree, cs.chunk, cs.ext_k, cs.bf, cs.u, cs.n_sets, cs.n_lookups, cs.selector_lookup};
         if (!shape) throw Error(H2B_ERR_ARG, "circuit_info: null shape");
         std::copy(v, v + 8, shape);
-        write_text("adv=" + join(cs.adv_names) + "\nperm=" + join(cs.perm_cols) + "\nfixed=" + join(cs.fixed_names) + "\nsigma=" +
-                       join(cs.sigma_names) + "\nconst=" + join(cs.const_names),
+        std::vector<std::string> sel;
+        for (auto& [nm, a] : cs.layout.selectors) sel.push_back(nm + ":" + a.column + ":" + std::to_string(a.root) + ":" + std::to_string(a.len));
+        write_text("adv=" + join(cs.adv_names) + "\nperm=" + join(cs.perm_cols) + "\nfixed=" + join(cs.layout.fixed_columns) + "\nsigma=" +
+                       join(cs.sigma_names) + "\nconst=" + join(cs.const_names) + "\nqueries=" + join(cs.layout.fixed_queries) +
+                       "\nselectors=" + join(sel),
                    names, cap);
     });
 }
@@ -291,16 +295,17 @@ H2BP_API int h2bp_mock_run(BoundMock* b, const BuilderView* v, size_t max_report
 
 // keygen of a builder (include/h2b200_keygen.hpp).  Out: the circuit (freed with h2bp_circuit_free); break_points (A - 1 words,
 // the count in *n_break_points); vk: 12 limbs per commitment, the fixed columns in the circuit's fixed_names order, then the sigma
-// columns (F + A + L + v->n_instance_columns); times: the five phases of KeygenTimes in ms (may be null); F constants columns
+// columns (F + A + L + v->n_instance_columns); times: the five phases of KeygenTimes in ms (may be null); F constants columns;
+// compress_selectors: halo2's keygen_vk layout (the vk's fixed commitments in the circuit's column order)
 H2BP_API int h2bp_keygen(h2b_ctx* ctx, h2b_srs* srs, uint32_t k, size_t srs_count, size_t A, size_t L, int selector_lookup, uint32_t lookup_bits,
                          size_t max_rows, size_t F, const BuilderView* v, BoundCircuit** out, uint64_t* break_points, uint64_t* n_break_points, uint64_t* vk,
-                         double* times) {
+                         double* times, int compress_selectors) {
     return run(ctx, [&] {
         if (!srs || !v || !out || !n_break_points || !vk || (A > 1 && !break_points)) throw Error(H2B_ERR_ARG, "keygen: null argument");
         auto b = std::make_unique<BoundCircuit>(ctx);
         const ParamsKZG params(b->ctx, k, srs, srs_count);
         KeygenTimes t;
-        KeygenResult r = keygen(b->ctx, params, k, A, L, selector_lookup != 0, lookup_bits, max_rows, *v, &t, F);
+        KeygenResult r = keygen(b->ctx, params, k, A, L, selector_lookup != 0, lookup_bits, max_rows, *v, &t, F, compress_selectors != 0);
         b->cs = std::move(r.pk);
         *n_break_points = r.break_points.size();
         std::copy(r.break_points.begin(), r.break_points.end(), break_points);

@@ -140,10 +140,16 @@ class Circuit:
       F constants columns c, c1..c{F-1} (F = 0: none); I instance columns i0..i{I-1} (BaseConfig::configure,
       gates/circuit/mod.rs:87-93); equality on [c, c1.., a0.., l0.., i0..] in that order (the permutation's column order).
     The shape numbers and column names are read from the compiled circuit.  `lagr`, `coeff`, `ext` (by column name) and
-    `sigma_map` (the decoded sigma of the check) look up its device columns."""
+    `sigma_map` (the decoded sigma of the check) look up its device columns.
+
+    compress_selectors: lay the fixed side out as halo2's keygen_vk does (DESIGN.md §4.13).  The columns passed are the same
+    (q{j}, [q_lookup], [table], c..; every selector value 0 or 1); the circuit combines the selectors into the columns s0, s1..
+    itself.  `fixed_names` lists the fixed columns in column order (the vk's), `fixed_queries` in query order (the evaluations
+    and openings), and `selectors` maps each selector to (column, root, combination length); without compression every
+    selector is its own column with root 1 and both orders are q0.., [q_lookup], [table], c.."""
 
     def __init__(self, ctx: Context, k: int, fixed_lagrange: dict, sigma_lagrange: list, A: int = 1, L: int = 0,
-                 selector_lookup: bool = True, I: int = 0, F: int = 1):
+                 selector_lookup: bool = True, I: int = 0, F: int = 1, compress_selectors: bool = False):
         n = 1 << k
         fixed = {nm: _rows(a, n, nm) for nm, a in fixed_lagrange.items()}
         sigma = [_rows(a, n, "sigma %d" % i) for i, a in enumerate(sigma_lagrange)]
@@ -151,7 +157,8 @@ class Circuit:
         ptrs = (C.c_void_p * len(fixed))(*[a.ctypes.data for a in fixed.values()])
         sptrs = (C.c_void_p * len(sigma))(*[a.ctypes.data for a in sigma])
         h = C.c_void_p()
-        ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), I, F, names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h)))
+        ctx.check(lib.h2bp_circuit_create(ctx.h, k, A, L, int(selector_lookup), I, F, names, ptrs, len(fixed), sptrs, len(sigma), C.byref(h),
+                                          int(compress_selectors)))
         self._bind(ctx, k, A, L, h)
 
     def _bind(self, ctx: Context, k: int, A: int, L: int, h: C.c_void_p):
@@ -165,6 +172,9 @@ class Circuit:
         lists = {key: v.split(",") if v else [] for key, v in (line.split("=", 1) for line in text.value.decode().split("\n"))}
         self.adv_names, self.perm_cols, self.fixed_names, self.sigma_names, self.const_names = (
             lists[key] for key in ("adv", "perm", "fixed", "sigma", "const"))
+        self.fixed_queries = lists["queries"]
+        self.selectors = {nm: (col, int(root), int(ln)) for nm, col, root, ln in (e.split(":") for e in lists["selectors"])}
+        self.compressed = any(col != nm for nm, (col, _, _) in self.selectors.items())
         self.F = len(self.const_names)
         self.I = len(self.perm_cols) - self.F - A - L
         self.lagr, self.coeff, self.ext = _Columns(self, "lagr"), _Columns(self, "coeff"), _Columns(self, "ext")
@@ -342,7 +352,7 @@ def _builder_view(who: str, n_cells: int, selectors, advice_equalities, constant
 
 def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, selector_lookup: bool = True, lookup_bits: int = 8,
            max_rows: int | None = None, selectors=(), advice_equalities=(), constant_equalities=None, lookups=(), timings: dict | None = None,
-           I: int = 0, instances=None, F: int = 1):
+           I: int = 0, instances=None, F: int = 1, compress_selectors: bool = False):
     """keygen_vk + keygen_pk of a halo2-base builder in its keygen form, on the device (h2b::keygen, include/h2b200_keygen.hpp).
 
     The arguments mean what they mean for MockProver.run (selectors: one per cell of the virtual column, which fixes its length;
@@ -353,7 +363,9 @@ def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, sele
     Returns (circuit, vk, break_points): `circuit` is a Circuit that ProverSession takes; vk = {"fixed": {name: commitment},
     "permutation": [commitment per permutation column, perm_cols order]}, each commitment affine as 12 Montgomery limbs
     (x, y, 1; the identity all zero), of the column's Lagrange values.  halo2-base's panics raise H2BError with its message.
-    `timings`, when a dict, receives the milliseconds of the phases copies / forest / sigma / pk / vk."""
+    `timings`, when a dict, receives the milliseconds of the phases copies / forest / sigma / pk / vk.
+    compress_selectors: keygen_vk's selector compression (see Circuit; its time counts in `pk`): vk["fixed"] then holds halo2's
+    fixed columns in halo2's column order, [table], c.., s0, s1.."""
     max_rows = (1 << k) - 9 if max_rows is None else max_rows
     n_cells = len(np.asarray(selectors).reshape(-1))
     view, keep = _builder_view("keygen", n_cells, selectors, advice_equalities, constant_equalities, lookups, I=I, instances=instances)
@@ -363,12 +375,14 @@ def keygen(ctx: Context, params: ParamsKZG, k: int, A: int = 1, L: int = 0, sele
     times = np.zeros(5, dtype=np.float64)
     h = C.c_void_p()
     ctx.check(lib.h2bp_keygen(ctx.h, params.h, k, params.count, A, L, int(selector_lookup), lookup_bits, max_rows, F, C.byref(view), C.byref(h),
-                              C.c_void_p(bps.ctypes.data), C.byref(nbp), C.c_void_p(vk.ctypes.data), C.c_void_p(times.ctypes.data)))
+                              C.c_void_p(bps.ctypes.data), C.byref(nbp), C.c_void_p(vk.ctypes.data), C.c_void_p(times.ctypes.data),
+                              int(compress_selectors)))
     cs = Circuit.__new__(Circuit)
     cs._bind(ctx, k, A, L, h)
     if timings is not None:
         timings.update(zip(("copies", "forest", "sigma", "pk", "vk"), (float(t) for t in times)))
-    out = {"fixed": {nm: vk[i] for i, nm in enumerate(cs.fixed_names)}, "permutation": list(vk[len(cs.fixed_names):])}
+    nf = len(cs.fixed_names)
+    out = {"fixed": {nm: vk[i] for i, nm in enumerate(cs.fixed_names)}, "permutation": list(vk[nf:nf + len(cs.perm_cols)])}
     return cs, out, [int(b) for b in bps[:nbp.value]]
 
 

@@ -512,6 +512,15 @@ int h2b_keygen_instance_edges_nf_dev(h2b_ctx* ctx, size_t N, const uint64_t* bre
 int h2b_keygen_sigma_map_dev(h2b_ctx* ctx, const void* d_edges, size_t E, size_t n_cols, uint32_t k, void* d_map);
 int h2b_keygen_sigma_values_dev(h2b_ctx* ctx, const void* d_map, size_t n_cols, uint32_t k, void* d_sigma);
 
+/* ---- selector compression (halo2's keygen_vk with compress_selectors, DESIGN.md §4.13): which selector columns are active on a
+ * common row.  S (1 <= S <= H2B_SELECTORS_MAX) selector columns of 2^k Lagrange values each, every value 0 or 1 (Montgomery);
+ * conflicts: S x S bytes on the HOST in both forms, row-major, conflicts[i S + j] = 1 iff some row has both i and j set (the
+ * diagonal: column i is set on some row), else 0.  A value other than 0 or 1: H2B_ERR_ARG naming the first such column and row
+ * (column-major order).  Synchronises. */
+#define H2B_SELECTORS_MAX 4096
+int h2b_selector_conflicts(h2b_ctx* ctx, const uint64_t* const* selectors, size_t S, uint32_t k, uint8_t* conflicts);
+int h2b_selector_conflicts_dev(h2b_ctx* ctx, const void* const* d_selectors, size_t S, uint32_t k, uint8_t* conflicts);
+
 /* ---- opening arithmetic (SURVEY.md §8(f) rank 4): halo2-axiom 0.5.3 `arithmetic::{eval_polynomial, kate_division}`
  * and the polynomial linear combinations of `poly/kzg/multiopen/shplonk/prover.rs` ------------------------------- */
 /* out = sum_i coeffs[i] * x^i */

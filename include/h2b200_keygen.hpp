@@ -24,7 +24,7 @@ namespace h2b {
 
 // affine commitments (z = 1; the identity all zero) of the Lagrange columns, as ProverSession commits them
 struct VerifyingKey {
-    std::vector<std::pair<std::string, G1>> fixed;  // the circuit's fixed_names order
+    std::vector<std::pair<std::string, G1>> fixed;  // the circuit's column order (its layout.fixed_columns)
     std::vector<G1> permutation;                    // one per permutation column, perm_cols order (instance columns last)
 };
 
@@ -43,9 +43,11 @@ struct KeygenResult {
     VerifyingKey vk;
 };
 
-// params: the SRS of the 2^k domain (its Lagrange bases commit the vk); max_rows as for MockProver (<= 2^k - 7); F constants columns
+// params: the SRS of the 2^k domain (its Lagrange bases commit the vk); max_rows as for MockProver (<= 2^k - 7); F constants columns;
+// compress_selectors: keygen_vk's selector compression (h2b200_selectors.hpp, timed in `pk`): the vk's fixed commitments are then
+// halo2's columns in halo2's column order, [table], c.., s0, s1..
 inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t k, size_t A, size_t L, bool selector_lookup, uint32_t lookup_bits,
-                           size_t max_rows, const BuilderView& b, KeygenTimes* times = nullptr, size_t F = 1) {
+                           size_t max_rows, const BuilderView& b, KeygenTimes* times = nullptr, size_t F = 1, bool compress_selectors = false) {
     using clock = std::chrono::steady_clock;
     auto t0 = clock::now();
     auto lap = [&](double KeygenTimes::*field) {
@@ -113,11 +115,14 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
     for (size_t i = 0; i < nf; i++) fx[s.fixed_names[i]] = col(i);
     std::vector<const Fr*> sg;
     for (size_t i = 0; i < npc; i++) sg.push_back(static_cast<const Fr*>(sigma.at(i * n)));
-    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg, I, F);
+    out.pk = std::make_unique<ProverCircuit>(ProverCircuit::OnDevice{}, ctx, k, A, L, selector_lookup, fx, sg, I, F, compress_selectors);
     lap(&KeygenTimes::pk);
-    // the vk: every fixed column, then every sigma column, committed in Lagrange form, up to 16 MSMs per batch
+    // the vk: every fixed column (compressed: the circuit's, in its column order), then every sigma column, committed in Lagrange
+    // form, up to 16 MSMs per batch
+    const std::vector<std::string>& fixed_order = compress_selectors ? out.pk->layout.fixed_columns : s.fixed_names;
+    const size_t nvf = fixed_order.size();
     std::vector<const void*> cols;
-    for (size_t i = 0; i < nf; i++) cols.push_back(col(i));
+    for (size_t i = 0; i < nvf; i++) cols.push_back(compress_selectors ? out.pk->lagr.at(fixed_order[i])->at() : col(i));
     for (size_t i = 0; i < npc; i++) cols.push_back(sigma.at(i * n));
     std::vector<G1> pts(cols.size());
     Poly d_out(ctx, 48);
@@ -128,8 +133,8 @@ inline KeygenResult keygen(const Context& ctx, const ParamsKZG& params, uint32_t
         ctx.check(h2b_poly_download(c, d_out.raw(), 0, pts[lo].x.data(), m * 3));
         g1_normalize_host_batch(pts.data() + lo, m);
     }
-    for (size_t i = 0; i < nf; i++) out.vk.fixed.push_back({s.fixed_names[i], pts[i]});
-    out.vk.permutation.assign(pts.begin() + nf, pts.end());
+    for (size_t i = 0; i < nvf; i++) out.vk.fixed.push_back({fixed_order[i], pts[i]});
+    out.vk.permutation.assign(pts.begin() + nvf, pts.end());
     lap(&KeygenTimes::vk);
     return out;
 }

@@ -22,6 +22,7 @@
 #include <utility>
 
 #include "h2b200.hpp"
+#include "h2b200_selectors.hpp"
 
 namespace h2b {
 
@@ -448,9 +449,25 @@ struct CircuitShape {
     std::vector<std::string> adv_names, inst_names, const_names, perm_cols, fixed_names, sigma_names;
 };
 
-// the vertical gate q (a0 + a1 a2 - a3) on fixed and advice slot `slot`, advice rotations 0..3 (flex_gate/mod.rs:80-91)
-inline ValueSource add_vertical_gate(GraphEvaluator& ev, uint32_t slot) {
+// a selector as the gates read it from fixed slot `slot`: the column itself (root 1 of a combination of 1), or, compressed, member
+// `root` of a combination of `len`: S prod_{t = 1..len, t != root} (t - S) (halo2's substitution, not normalised; DESIGN §2 (12))
+inline ValueSource add_selector(GraphEvaluator& ev, uint32_t slot, size_t root = 1, size_t len = 1) {
     const ValueSource q = ev.add_calculation(Calculation::Store(ValueSource::Fixed(slot, ev.add_rotation(0))));
+    ValueSource acc = q;
+    for (size_t t = 1; t <= len; t++)
+        if (t != root) {
+            const Fr c = HostFr::from_canonical(std::array<uint64_t, 4>{t, 0, 0, 0}.data());
+            acc = ev.add_calculation(Calculation::Mul(acc, ev.add_calculation(Calculation::Sub(ev.add_constant(c), q))));
+        }
+    return acc;
+}
+// calculations of one vertical gate whose selector is a member of a combination of `len` (see ProverCircuit's gate programs)
+inline size_t vertical_gate_calculations(size_t len) { return 9 + 2 * (len - 1); }
+
+// the vertical gate q (a0 + a1 a2 - a3) on fixed and advice slot `slot`, advice rotations 0..3 (flex_gate/mod.rs:80-91); q as
+// add_selector reads it
+inline ValueSource add_vertical_gate(GraphEvaluator& ev, uint32_t slot, size_t root = 1, size_t len = 1) {
+    const ValueSource q = add_selector(ev, slot, root, len);
     ValueSource a[4];
     for (int r = 0; r < 4; r++) a[r] = ev.add_calculation(Calculation::Store(ValueSource::Advice(slot, ev.add_rotation(r))));
     const ValueSource sum = ev.add_calculation(Calculation::Add(a[0], ev.add_calculation(Calculation::Mul(a[1], a[2]))));
@@ -461,24 +478,27 @@ inline ValueSource add_vertical_gate(GraphEvaluator& ev, uint32_t slot) {
 class ProverCircuit : public CircuitShape {
 public:
     // fixed: Lagrange values (2^k each) by name — q0..q{A-1}, [q_lookup], [table], c, c1..c{F-1}; sigma: one column per
-    // permutation column in the order [c, c1.., a0.., l0.., i0..] (F constants columns, I instance columns)
+    // permutation column in the order [c, c1.., a0.., l0.., i0..] (F constants columns, I instance columns).
+    // compress_selectors: lay the fixed side out as halo2's keygen_vk does (h2b200_selectors.hpp): the selectors q{j} and
+    // q_lookup (0/1 values) become the combination columns s0, s1.. and `layout` says where each one went
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, std::vector<Fr>>& fixed,
-                  const std::vector<std::vector<Fr>>& sigma, size_t I = 0, size_t F = 1)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k), false, I, F) {}
+                  const std::vector<std::vector<Fr>>& sigma, size_t I = 0, size_t F = 1, bool compress_selectors = false)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, rows_of(fixed, k), rows_of(sigma, k), false, I, F, compress_selectors) {}
     // the same with every column as a pointer to its 2^k rows (nothing is copied on the host)
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
-                  const std::vector<const Fr*>& sigma, size_t I = 0, size_t F = 1)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false, I, F) {}
+                  const std::vector<const Fr*>& sigma, size_t I = 0, size_t F = 1, bool compress_selectors = false)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, false, I, F, compress_selectors) {}
     // the same with every column as a DEVICE pointer to its 2^k Lagrange values (keygen on the device, h2b200_keygen.hpp): each is
     // copied on the device, then transformed as above
     struct OnDevice {};
     ProverCircuit(OnDevice, const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup,
-                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma, size_t I = 0, size_t F = 1)
-        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true, I, F) {}
+                  const std::map<std::string, const Fr*>& fixed, const std::vector<const Fr*>& sigma, size_t I = 0, size_t F = 1,
+                  bool compress_selectors = false)
+        : ProverCircuit(ctx, k, A, L, selector_lookup, fixed, sigma, true, I, F, compress_selectors) {}
 
 private:
     ProverCircuit(const Context& ctx, uint32_t k, size_t A, size_t L, bool selector_lookup, const std::map<std::string, const Fr*>& fixed,
-                  const std::vector<const Fr*>& sigma, bool on_device, size_t I, size_t F)
+                  const std::vector<const Fr*>& sigma, bool on_device, size_t I, size_t F, bool compress)
         : CircuitShape(k, A, L, selector_lookup, I, F), ctx(ctx) {
         if (sigma.size() != perm_cols.size()) throw Error(H2B_ERR_ARG, "ProverCircuit: one sigma column per permutation column");
         std::vector<Fr> l0(n, Fr{}), ll(n, Fr{}), la(n, Fr{});
@@ -501,24 +521,71 @@ private:
             coeff[name] = std::move(cf);
             ext[name] = std::move(ex);
         };
-        for (auto& nm : fixed_names) {
-            auto it = fixed.find(nm);
-            if (it == fixed.end()) throw Error(H2B_ERR_ARG, "ProverCircuit: missing fixed column " + nm);
-            add(nm, it->second, on_device);
+        for (auto& nm : fixed_names)
+            if (!fixed.count(nm)) throw Error(H2B_ERR_ARG, "ProverCircuit: missing fixed column " + nm);
+        std::vector<std::string> selectors;  // selector index order: q0.., q_lookup (convention 14)
+        for (size_t j = 0; j < A; j++) selectors.push_back("q" + std::to_string(j));
+        if (this->selector_lookup) selectors.push_back("q_lookup");
+        std::vector<PolyPtr> staged;  // host selector columns, uploaded for the conflict kernel
+        if (!compress) {
+            layout = uncompressed_layout(fixed_names, selectors);
+            for (auto& nm : fixed_names) add(nm, fixed.at(nm), on_device);
+        } else {
+            std::vector<const void*> d_sel;
+            std::vector<size_t> deg;  // the vertical gate has degree 3; q_lookup is complex (degree 0)
+            for (auto& nm : selectors) {
+                if (on_device) {
+                    d_sel.push_back(fixed.at(nm));
+                } else {
+                    staged.push_back(std::make_unique<Poly>(ctx, n));
+                    staged.back()->upload(fixed.at(nm), n);
+                    d_sel.push_back(staged.back()->at());
+                }
+                deg.push_back(nm == "q_lookup" ? 0 : 3);
+            }
+            const auto combos = compress_selectors_process(deg, degree, selector_conflicts_dev(ctx, d_sel, k));
+            // column order [table], c.. (RangeConfig creates the table before FlexGateConfig its constants columns); query order
+            // c.., [table] (enable_equality queries the constants, the lookup queries the table)
+            std::vector<std::string> columns, queries = const_names;
+            if (n_lookups) {
+                columns.push_back("table");
+                queries.push_back("table");
+            }
+            columns.insert(columns.end(), const_names.begin(), const_names.end());
+            layout = compressed_layout(columns, queries, selectors, combos);
+            for (auto& nm : columns) add(nm, fixed.at(nm), on_device);
+            Poly comb(ctx, n);
+            for (size_t c = 0; c < combos.size(); c++) {  // S_c = sum_m root_m q_m (the members are active on disjoint rows)
+                std::vector<const void*> pp;
+                std::vector<Fr> roots;
+                for (size_t m = 0; m < combos[c].size(); m++) {
+                    pp.push_back(d_sel[combos[c][m]]);
+                    roots.push_back(HostFr::from_canonical(std::array<uint64_t, 4>{m + 1, 0, 0, 0}.data()));
+                }
+                ctx.check(h2b_poly_lincomb_dev(ctx.raw(), pp.data(), roots[0].data(), pp.size(), n, comb.at()));
+                add(layout.combinations[c].first, static_cast<const Fr*>(comb.at()), true);
+            }
+            h2b_ctx_synchronize(ctx.raw());
         }
         for (size_t i = 0; i < perm_cols.size(); i++) add(sigma_names[i], sigma[i], on_device);
         add("l0", l0.data(), false);
         add("l_last", ll.data(), false);
         add("l_active", la.data(), false);
         h2b_ctx_synchronize(ctx.raw());
-        // gate programs: GATES_PER_PROGRAM vertical gates each (a program holds at most 64 calculations); every program continues
-        // the Horner fold in y from the previous value, so the chain of programs is the one fold evaluate_h does
-        for (size_t j0 = 0; j0 < A; j0 += GATES_PER_PROGRAM) {
+        // gate programs: GATES_PER_PROGRAM vertical gates each, fewer when compressed selectors add calculations (a program holds
+        // at most 64 calculations, one of them the fold); every program continues the Horner fold in y from the previous value,
+        // so the chain of programs is the one fold evaluate_h does
+        size_t max_len = 1;
+        for (auto& e : layout.selectors) max_len = std::max(max_len, e.second.len);
+        const size_t per_program = std::min(GATES_PER_PROGRAM, (H2B_GRAPH_MAX_CALCULATIONS - 1) / vertical_gate_calculations(max_len));
+        for (size_t j0 = 0; j0 < A; j0 += per_program) {
             GateProgram gp;
             std::vector<ValueSource> parts;
-            for (size_t j = j0; j < std::min(A, j0 + GATES_PER_PROGRAM); j++) {
-                parts.push_back(add_vertical_gate(gp.ev, uint32_t(j - j0)));
+            for (size_t j = j0; j < std::min(A, j0 + per_program); j++) {
+                const SelectorAssignment& a = layout.selectors.at("q" + std::to_string(j));
+                parts.push_back(add_vertical_gate(gp.ev, uint32_t(j - j0), a.root, a.len));
                 gp.cols.push_back(j);
+                gp.fixed.push_back(a.column);
             }
             gp.result = gp.ev.add_calculation(Calculation::Horner(ValueSource::PreviousValue(), parts, ValueSource::Y()));
             gate_programs.push_back(std::move(gp));
@@ -552,6 +619,12 @@ public:
         if (check_map) return;
         GraphEvaluator ev;
         const ValueSource res = add_vertical_gate(ev, 0);
+        for (auto& e : layout.selectors)  // compressed: one program per (root, len) of a gate's selector
+            if (layout.compressed && e.first != "q_lookup" && !check_subst.count({e.second.root, e.second.len})) {
+                GraphEvaluator sev;
+                const ValueSource sres = add_vertical_gate(sev, 0, e.second.root, e.second.len);
+                check_subst[{e.second.root, e.second.len}] = {std::move(sev), sres};
+            }
         const size_t npc = perm_cols.size();
         auto map = std::make_unique<Poly>(ctx, (npc * n + 7) / 8);
         Poly rep(ctx, (2 * npc + 3) / 4);  // max_report = 1: count and first row per column
@@ -582,13 +655,18 @@ public:
         return {{t->at(name).get(), 0}, t->at(name)->len()};
     }
 
+    // the column that holds selector `sel` (q{j}, q_lookup)
+    const std::string& selector_column(const std::string& sel) const { return layout.selectors.at(sel).column; }
+
     static constexpr size_t GATES_PER_PROGRAM = 5;
     struct GateProgram {
         GraphEvaluator ev;
         ValueSource result{};
-        std::vector<size_t> cols;
+        std::vector<size_t> cols;         // the gate columns of the program's advice slots
+        std::vector<std::string> fixed;   // the fixed column of each slot (q{j}, or its combination column)
     };
     const Context& ctx;
+    SelectorLayout layout;  // where the selectors are, the fixed columns in column and in query order
     std::map<std::string, PolyPtr> lagr, coeff, ext;
     std::vector<GateProgram> gate_programs;
     GraphEvaluator lookup_ev;
@@ -596,6 +674,7 @@ public:
     mutable GraphEvaluator check_ev;  // prepare_check()
     mutable ValueSource check_result{};
     mutable PolyPtr check_map;
+    mutable std::map<std::pair<size_t, size_t>, std::pair<GraphEvaluator, ValueSource>> check_subst;  // compressed: by (root, len)
 
 private:
     static std::map<std::string, const Fr*> rows_of(const std::map<std::string, std::vector<Fr>>& cols, uint32_t k) {
@@ -994,7 +1073,7 @@ public:
         for (size_t j = 0; j < cs.A; j++)
             for (int r : {0, 1, 2, 3}) add("a" + std::to_string(j), r);
         for (size_t t = 0; t < cs.L; t++) add("l" + std::to_string(t), 0);
-        for (auto& nm : cs.fixed_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (auto& nm : cs.layout.fixed_queries) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
         for (auto& nm : cs.sigma_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
         for (size_t s = 0; s < cs.n_sets; s++) {  // every set at x and omega x; all but the last one also at omega^last x
             const std::string nm = "zp" + std::to_string(s);
@@ -1021,7 +1100,7 @@ public:
     std::vector<Query> halo2_evaluations() const {
         const int last = -int(cs.bf + 1);
         std::vector<Query> q = advice_queries();
-        for (auto& nm : cs.fixed_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (auto& nm : cs.layout.fixed_queries) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
         q.push_back({"rnd", rnd->at(), 0});
         for (auto& nm : cs.sigma_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
         for (size_t s = 0; s < cs.n_sets; s++) {
@@ -1055,7 +1134,7 @@ public:
             for (auto [nm, r] : std::initializer_list<std::pair<const char*, int>>{{"zl", 0}, {"pa", 0}, {"ps", 0}, {"pa", -1}, {"zl", 1}})
                 q.push_back({nm + ts, coef.at(nm + ts)->at(), r});
         }
-        for (auto& nm : cs.fixed_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
+        for (auto& nm : cs.layout.fixed_queries) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
         for (auto& nm : cs.sigma_names) q.push_back({nm, cs.coeff.at(nm)->at(), 0});
         q.push_back({"h", hx->at(), 0});
         q.push_back({"rnd", rnd->at(), 0});
@@ -1093,13 +1172,16 @@ public:
         auto at = [&](size_t i) { return static_cast<char*>(rep->at(1)) + 8 * W * i; };
         if (wit.assigned_form()) ctx.check(h2b_poly_copy_dev(c, rep->at(), verdict_words(), 1));
         for (size_t j = 0; j < A; j++) {
-            const BoundGraph g(cs.check_ev, cs.check_result, {cs.lagr.at("q" + std::to_string(j))->at()}, {lagr["a" + std::to_string(j)].ptr()});
+            const SelectorAssignment& sa = cs.layout.selectors.at("q" + std::to_string(j));
+            const GraphEvaluator& gev = cs.layout.compressed ? cs.check_subst.at({sa.root, sa.len}).first : cs.check_ev;
+            const ValueSource gres = cs.layout.compressed ? cs.check_subst.at({sa.root, sa.len}).second : cs.check_result;
+            const BoundGraph g(gev, gres, {cs.lagr.at(sa.column)->at()}, {lagr["a" + std::to_string(j)].ptr()});
             check_graph_dev(ctx, *g.get(), k, u, max_report, at(j));
         }
         for (size_t t = 0; t < cs.n_lookups; t++) {
             const void* in = lagr[L ? "l" + std::to_string(t) : "a0"].ptr();
             if (L == 0) {
-                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at("q_lookup")->at(), in, n, inp->at()));
+                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at(cs.selector_column("q_lookup"))->at(), in, n, inp->at()));
                 in = inp->at();
             }
             check_lookup_dev(ctx, in, cs.lagr.at("table")->at(), k, u, max_report, at(A + t));
@@ -1196,7 +1278,7 @@ private:
         for (size_t t = 0; t < cs.n_lookups; t++) {
             const std::string ts = std::to_string(t);
             if (L == 0) {
-                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at("q_lookup")->at(), lagr["a0"].ptr(), n, inp->at()));
+                ctx.check(h2b_fr_mul_elementwise_dev(c, cs.lagr.at(cs.selector_column("q_lookup"))->at(), lagr["a0"].ptr(), n, inp->at()));
                 lk_in.push_back(inp->at());
             } else {
                 lk_in.push_back(lagr["l" + ts].ptr());
@@ -1256,9 +1338,9 @@ private:
         ctx.check(h2b_poly_zero(c, h->raw()));
         for (auto& gp : cs.gate_programs) {
             std::vector<const void*> fx, ad;
-            for (size_t j : gp.cols) {
-                fx.push_back(cs.ext.at("q" + std::to_string(j))->at());
-                ad.push_back(ext["a" + std::to_string(j)]->at());
+            for (size_t i = 0; i < gp.cols.size(); i++) {
+                fx.push_back(cs.ext.at(gp.fixed[i])->at());
+                ad.push_back(ext["a" + std::to_string(gp.cols[i])]->at());
             }
             const BoundGraph g(gp.ev, gp.result, fx, ad, ch);
             ctx.check(h2b_quotient_graph_dev(c, g.get(), k, ext_k, h->at()));
@@ -1278,7 +1360,7 @@ private:
             const std::string ts = std::to_string(t);
             std::vector<const void*> fx, ad;
             if (L == 0) {
-                fx = {cs.ext.at("q_lookup")->at(), cs.ext.at("table")->at()};
+                fx = {cs.ext.at(cs.selector_column("q_lookup"))->at(), cs.ext.at("table")->at()};
                 ad = {ext["a0"]->at()};
             } else {
                 fx = {cs.ext.at("table")->at()};
